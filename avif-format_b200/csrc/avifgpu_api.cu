@@ -173,9 +173,18 @@ struct avifgpu_context
     };
     std::vector<Gray16Lut> gray16Luts;
     int premultiplyState[3] = { -1, -1, -1 }; // image depth 8 / 10 / 12: -1 not checked yet, 0 keep the reference sequence, 1 fast form verified
+    // The first-use helpers below take `capturing`: the call is being recorded into a CUDA graph, where nothing but kernel
+    // launches on the caller's stream may happen.  What is not prepared yet then answers "not verified" / nullptr for
+    // this call only -- the path that needs no preparation, with bit-identical outputs -- and nothing is cached.  (The
+    // verify sweeps, LUT and table builds allocate and synchronise; BuildCurveTable's cudaGetDeviceProperties is only
+    // reached from a build.)
+    //
+    // A captured graph holds the device pointers of the step tables and Gray16 LUTs it was recorded with: those are only
+    // ever added to (never freed, moved or rebuilt) until avifgpu_destroy.
+
     // The tuned integer encode kernel premultiplies with a 6-instruction form, but only after it has been compared with
     // PremultiplyColor's own sequence for every (colour, alpha) code pair of the depth, on this device.
-    int VerifiedPremultiply(const avifgpu_encode_desc& d)
+    int VerifiedPremultiply(const avifgpu_encode_desc& d, bool capturing)
     {
         if (d.alpha_state != AVIFGPU_ALPHA_PREMULTIPLIED || d.host_depth == 32 || d.host_channels != 4 || d.layout != AVIFGPU_LAYOUT_PLANAR_YCBCR)
         {
@@ -184,6 +193,10 @@ struct avifgpu_context
         const int slot = d.image_bit_depth == 8 ? 0 : d.image_bit_depth == 10 ? 1 : 2;
         if (premultiplyState[slot] < 0)
         {
+            if (capturing)
+            {
+                return 0;
+            }
             premultiplyState[slot] = VerifyFastPremultiply((1u << d.image_bit_depth) - 1u, streams[0]) == 0 ? 1 : 0;
             launches += 1;
         }
@@ -193,10 +206,14 @@ struct avifgpu_context
 
     // HLG decode replaces two constant divisions by a 3-instruction form, but only after comparing it with the
     // IEEE division over every numerator the call sites can produce, on this device.
-    int VerifiedHlgDivisions()
+    int VerifiedHlgDivisions(bool capturing)
     {
         if (hlgDivisionState < 0)
         {
+            if (capturing)
+            {
+                return 0;
+            }
             const long long disagreements = VerifyHlgDivisions(streams[0]);
             hlgDivisionState = disagreements == 0 ? 1 : 0;
             launches += 1;
@@ -207,10 +224,14 @@ struct avifgpu_context
     // The quotient inside PQToLinear (ColorTransfer.cpp:110-112): the tuned float decode kernel uses a branch-free division
     // once it has been compared with the IEEE one for every value the quotient's operands can take, on this device.
     int pqRatioState = -1;
-    int VerifiedPqRatio()
+    int VerifiedPqRatio(bool capturing)
     {
         if (pqRatioState < 0)
         {
+            if (capturing)
+            {
+                return 0;
+            }
             const long long disagreements = VerifyPqRatio(streams[0]);
             pqRatioState = disagreements == 0 ? 1 : 0;
             launches += 1;
@@ -228,7 +249,7 @@ struct avifgpu_context
         int state;
     };
     std::vector<GreenDivision> greenDivisions;
-    int VerifiedGreenDivision(const DecodeParams& p)
+    int VerifiedGreenDivision(const DecodeParams& p, bool capturing)
     {
         if (p.colorspace != AVIFGPU_COLORSPACE_YCBCR || p.bitDepth > 12)
         {
@@ -241,6 +262,10 @@ struct avifgpu_context
                 return g.state;
             }
         }
+        if (capturing)
+        {
+            return 0;
+        }
         GreenDivision g{};
         g.matrix = p.matrix;
         g.range = p.range;
@@ -252,7 +277,7 @@ struct avifgpu_context
     }
 
     // The 65536-entry code table of a Gray16 host configuration (built on the device on first use), or nullptr.
-    const uint16_t* Gray16LutFor(const avifgpu_encode_desc& d)
+    const uint16_t* Gray16LutFor(const avifgpu_encode_desc& d, bool capturing)
     {
         if (d.host_depth != 16 || d.host_channels != 1 || d.layout != AVIFGPU_LAYOUT_REFERENCE || d.image_bit_depth <= 8)
         {
@@ -265,6 +290,10 @@ struct avifgpu_context
             {
                 return l.device;
             }
+        }
+        if (capturing)
+        {
+            return nullptr;
         }
         Gray16Lut lut;
         lut.depth = d.image_bit_depth;
@@ -288,8 +317,9 @@ struct avifgpu_context
 
     // The verified step table for a float-host encode description, or nullptr when the description does not use
     // one / the table could not be verified / building it has not paid off yet (then the generic exact kernel serves
-    // the call).  `pixels` = the size of the call that asks; `force` = avifgpu_prepare_encode.
-    CurveTable* CurveTableFor(const avifgpu_encode_desc& d, int64_t pixels, bool force)
+    // the call).  `pixels` = the size of the call that asks; `force` = avifgpu_prepare_encode.  A capturing call neither
+    // builds a table nor counts its pixels towards one.
+    CurveTable* CurveTableFor(const avifgpu_encode_desc& d, int64_t pixels, bool force, bool capturing)
     {
         if (d.host_depth != 32 || d.image_bit_depth > 12)
         {
@@ -320,6 +350,10 @@ struct avifgpu_context
             {
                 return t;
             }
+        }
+        if (capturing)
+        {
+            return nullptr;
         }
         if (!force)
         {
@@ -354,6 +388,25 @@ struct avifgpu_context
         return t;
     }
 
+    // The first-use state an encode call reads: step table, Gray16 LUT, premultiply check.
+    void FirstUseEncode(const avifgpu_encode_desc& d, int64_t pixels, bool capturing, EncodeParams* p)
+    {
+        if (CurveTable* table = CurveTableFor(d, pixels, false, capturing))
+        {
+            p->curveTable = table->valid ? &table->view : nullptr;
+        }
+        p->gray16Lut = Gray16LutFor(d, capturing);
+        p->verifiedPremultiply = VerifiedPremultiply(d, capturing);
+    }
+
+    // The first-use state a decode call reads: the verified HLG, green-channel and PQ divisions.
+    void FirstUseDecode(const avifgpu_decode_desc& d, int32_t transfer, bool capturing, DecodeParams* p)
+    {
+        p->verifiedHlgDivisions = (d.host_depth == 32 && transfer == AVIFGPU_TRANSFER_HLG) ? VerifiedHlgDivisions(capturing) : 0;
+        p->verifiedGreenDivision = VerifiedGreenDivision(*p, capturing);
+        p->verifiedPqRatio = (d.host_depth == 32 && transfer == AVIFGPU_TRANSFER_PQ && d.colorspace == AVIFGPU_COLORSPACE_YCBCR) ? VerifiedPqRatio(capturing) : 0;
+    }
+
     int Fail(int status, const std::string& message)
     {
         lastError = message;
@@ -362,13 +415,13 @@ struct avifgpu_context
 
     // A launcher returned a negative status: report the CUDA error it recorded (it has already cleared CUDA's own
     // slot), after draining the pipeline streams so that no copy of an earlier slice is still writing into caller memory
-    // when the entry point returns.
-    int LaunchFailed(int status, const char* what)
+    // when the entry point returns.  A capturing call synchronises nothing: ending the capture is the caller's business.
+    int LaunchFailed(int status, const char* what, bool capturing = false)
     {
         const int code = TakeLaunchFailure();
         for (cudaStream_t stream : streams)
         {
-            if (stream)
+            if (stream && !capturing)
             {
                 cudaStreamSynchronize(stream);
             }
@@ -483,6 +536,21 @@ namespace
             }
         }
     };
+
+    // Whether work enqueued on `stream` is being recorded into a CUDA graph (in any capture mode).  The query itself
+    // fails for the legacy NULL stream while a blocking stream of the device is being captured.
+    int QueryCapture(avifgpu_context* ctx, void* stream, bool* capturing)
+    {
+        cudaStreamCaptureStatus status = cudaStreamCaptureStatusNone;
+        const cudaError_t e = cudaStreamIsCapturing(static_cast<cudaStream_t>(stream), &status);
+        *capturing = status != cudaStreamCaptureStatusNone;
+        if (e != cudaSuccess)
+        {
+            cudaGetLastError();
+            return ctx->Fail(AVIFGPU_ERR_CUDA, std::string("cudaStreamIsCapturing: ") + cudaGetErrorString(e));
+        }
+        return AVIFGPU_OK;
+    }
 
     int CheckBlock(avifgpu_context* ctx, int height, int ys, int y0, int nrows)
     {
@@ -793,17 +861,17 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_device(avifgpu_context* ctx, const avifgp
         p.planeStride[k] = device_dst->stride[k];
     }
     DeviceGuard guard(ctx->device);
-    p.smCount = ctx->smCount;
-    if (CurveTable* table = ctx->CurveTableFor(*desc, static_cast<int64_t>(desc->width) * nrows, false))
+    bool capturing;
+    if ((status = QueryCapture(ctx, cuda_stream, &capturing)) != AVIFGPU_OK)
     {
-        p.curveTable = table->valid ? &table->view : nullptr;
+        return status;
     }
-    p.gray16Lut = ctx->Gray16LutFor(*desc);
-    p.verifiedPremultiply = ctx->VerifiedPremultiply(*desc);
+    p.smCount = ctx->smCount;
+    ctx->FirstUseEncode(*desc, static_cast<int64_t>(desc->width) * nrows, capturing, &p);
     const int launched = LaunchEncode(p, desc->host_depth, cuda_stream);
     if (launched < 0)
     {
-        return ctx->LaunchFailed(launched, "encode kernel launch");
+        return ctx->LaunchFailed(launched, "encode kernel launch", capturing);
     }
     ctx->launches += launched;
     return AVIFGPU_OK;
@@ -847,9 +915,12 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_device(avifgpu_context* ctx, const avifgp
     p.yPhase = y0 & p.ys;
     p.smCount = ctx->smCount;
     DeviceGuard deviceGuardForTables(ctx->device);
-    p.verifiedHlgDivisions = (desc->host_depth == 32 && transfer == AVIFGPU_TRANSFER_HLG) ? ctx->VerifiedHlgDivisions() : 0;
-    p.verifiedGreenDivision = ctx->VerifiedGreenDivision(p);
-    p.verifiedPqRatio = (desc->host_depth == 32 && transfer == AVIFGPU_TRANSFER_PQ && desc->colorspace == AVIFGPU_COLORSPACE_YCBCR) ? ctx->VerifiedPqRatio() : 0;
+    bool capturing;
+    if ((status = QueryCapture(ctx, cuda_stream, &capturing)) != AVIFGPU_OK)
+    {
+        return status;
+    }
+    ctx->FirstUseDecode(*desc, transfer, capturing, &p);
     for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
     {
         const PlaneGeometry g = DecodePlaneGeometry(*desc, k);
@@ -868,7 +939,7 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_device(avifgpu_context* ctx, const avifgp
     const int launched = LaunchDecode(p, cuda_stream);
     if (launched < 0)
     {
-        return ctx->LaunchFailed(launched, "decode kernel launch");
+        return ctx->LaunchFailed(launched, "decode kernel launch", capturing);
     }
     ctx->launches += launched;
     return AVIFGPU_OK;
@@ -1185,12 +1256,7 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
     }
 
     base.smCount = ctx->smCount;
-    if (CurveTable* table = ctx->CurveTableFor(*desc, static_cast<int64_t>(desc->width) * nrows, false))
-    {
-        base.curveTable = table->valid ? &table->view : nullptr;
-    }
-    base.gray16Lut = ctx->Gray16LutFor(*desc);
-    base.verifiedPremultiply = ctx->VerifiedPremultiply(*desc);
+    ctx->FirstUseEncode(*desc, static_cast<int64_t>(desc->width) * nrows, false, &base);
     const int64_t rowPayload = static_cast<int64_t>(desc->width) * EncodeHostColBytes(*desc);
     const int64_t deviceRowStride = (rowPayload + 255) & ~255ll;
     const bool rowsPinned = IsPinned(host_rows);
@@ -1360,9 +1426,7 @@ static int DecodeRowsHost(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
         planePinned[k] = geometry[k].present && IsPinned(src->data[k]);
     }
 
-    base.verifiedHlgDivisions = (desc->host_depth == 32 && transfer == AVIFGPU_TRANSFER_HLG) ? ctx->VerifiedHlgDivisions() : 0;
-    base.verifiedGreenDivision = ctx->VerifiedGreenDivision(base);
-    base.verifiedPqRatio = (desc->host_depth == 32 && transfer == AVIFGPU_TRANSFER_PQ && desc->colorspace == AVIFGPU_COLORSPACE_YCBCR) ? ctx->VerifiedPqRatio() : 0;
+    ctx->FirstUseDecode(*desc, transfer, false, &base);
     const int64_t rowPayload = static_cast<int64_t>(desc->width) * DecodeHostColBytes(*desc);
     const int64_t deviceRowStride = (rowPayload + 255) & ~255ll;
     const int sliceRows = SliceRows(nrows, rowPayload);
@@ -1828,8 +1892,8 @@ AVIFGPU_EXPORT int avifgpu_prepare_encode(avifgpu_context* ctx, const avifgpu_en
         return ctx->Fail(status, error);
     }
     DeviceGuard guard(ctx->device);
-    CurveTable* table = ctx->CurveTableFor(*desc, 0, true);
-    ctx->Gray16LutFor(*desc);
+    CurveTable* table = ctx->CurveTableFor(*desc, 0, true, false);
+    ctx->Gray16LutFor(*desc, false);
     if (out_stats != nullptr)
     {
         std::memset(out_stats, 0, sizeof(*out_stats));
@@ -1851,6 +1915,29 @@ AVIFGPU_EXPORT int avifgpu_prepare_encode(avifgpu_context* ctx, const avifgpu_en
     {
         ctx->lastError = "step table not used (generic exact kernel serves this configuration): " + table->error;
     }
+    return AVIFGPU_OK;
+}
+
+AVIFGPU_EXPORT int avifgpu_prepare_decode(avifgpu_context* ctx, const avifgpu_decode_desc* desc)
+{
+    if (ctx == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    std::string error;
+    int32_t transfer;
+    const int status = ValidateDecodeDesc(desc, &transfer, &error);
+    if (status != AVIFGPU_OK)
+    {
+        return ctx->Fail(status, error);
+    }
+    DecodeParams p;
+    if (!FillDecodeParams(*desc, transfer, &p, &error))
+    {
+        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, error);
+    }
+    DeviceGuard guard(ctx->device);
+    ctx->FirstUseDecode(*desc, transfer, false, &p);
     return AVIFGPU_OK;
 }
 

@@ -20,6 +20,8 @@ namespace avifgpu
 #if defined(__CUDACC__)
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device setting; `configuredDevices` (one static per kernel
 // instantiation) remembers the devices it has been made on, so a process that drives several GPUs configures each.
+// It enqueues nothing, so a first launch inside a CUDA graph capture may make it (as may the table decode's occupancy
+// query): tests/test_gpu_graph_capture.py captures every tuned kernel's first launch in a fresh process.
 template <typename Kernel>
 inline cudaError_t AllowDynamicShared(Kernel kernel, int bytes, std::atomic<uint64_t>& configuredDevices)
 {

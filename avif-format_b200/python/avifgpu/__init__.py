@@ -70,6 +70,7 @@ def library():
         [ctx_p, C.POINTER(abi.DecodeDesc), C.POINTER(abi.Planes), C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p])
     sig("avifgpu_transfer_f32", C.c_int, [ctx_p, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_size_t])
     sig("avifgpu_prepare_encode", C.c_int, [ctx_p, C.POINTER(abi.EncodeDesc), C.POINTER(abi.CurveStats)])
+    sig("avifgpu_prepare_decode", C.c_int, [ctx_p, C.POINTER(abi.DecodeDesc)])
     sig("avifgpu_set_table_autobuild", C.c_int, [ctx_p, C.c_int64])
     sig("avifgpu_hlg_ootf_f32", C.c_int, [ctx_p, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_size_t])
     sig("avifgpu_encode_rows_async", C.c_int,
@@ -126,7 +127,7 @@ EXPORTED_SYMBOLS = [
     "avifgpu_decode_plane_geometry", "avifgpu_get_yuv_coefficients", "avifgpu_get_hlg_luma_coefficients",
     "avifgpu_build_yuv_tables", "avifgpu_encode_rows", "avifgpu_decode_rows", "avifgpu_encode_rows_device",
     "avifgpu_decode_rows_device", "avifgpu_transfer_f32", "avifgpu_prepare_encode", "avifgpu_set_table_autobuild",
-    "avifgpu_hlg_ootf_f32",
+    "avifgpu_hlg_ootf_f32", "avifgpu_prepare_decode",
     "avifgpu_encode_rows_async", "avifgpu_decode_rows_async", "avifgpu_wait",
     "avifgpu_shard_group_create", "avifgpu_shard_group_destroy", "avifgpu_shard_group_size", "avifgpu_shard_group_context",
     "avifgpu_shard_group_peer_access", "avifgpu_shard_group_last_error", "avifgpu_shard_group_prepare_encode",
@@ -273,6 +274,10 @@ class Context:
         stats = abi.CurveStats()
         self._check(self.lib.avifgpu_prepare_encode(self.handle, C.byref(desc), C.byref(stats)))
         return stats
+
+    def prepare_decode(self, desc):
+        """Does the first-use work a decode of `desc` would do (the verified divisions); see avifgpu_prepare_decode."""
+        self._check(self.lib.avifgpu_prepare_decode(self.handle, C.byref(desc)))
 
     def transfer(self, function, values, param=0.0):
         values = np.ascontiguousarray(values, dtype=np.float32)

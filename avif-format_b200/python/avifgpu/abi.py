@@ -8,7 +8,7 @@ import ctypes as C
 
 import numpy as np
 
-API_VERSION = 4
+API_VERSION = 5
 
 # avifgpu_status
 OK = 0

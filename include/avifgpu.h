@@ -50,7 +50,7 @@ extern "C" {
 #define AVIFGPU_EXPORT __attribute__((visibility("default")))
 #endif
 
-#define AVIFGPU_API_VERSION 4
+#define AVIFGPU_API_VERSION 5
 
 typedef enum avifgpu_status
 {
@@ -312,7 +312,24 @@ AVIFGPU_EXPORT int avifgpu_wait(avifgpu_context* ctx, int64_t ticket);
 /* ---- the hot path: device-pointer variants (no copies, no synchronisation) --------------------------- */
 
 /* Same contracts, but host_rows / planes are DEVICE pointers valid on the context's device and the work is
- * enqueued on `cuda_stream` (a cudaStream_t; NULL = the legacy default stream). */
+ * enqueued on `cuda_stream` (a cudaStream_t; NULL = the legacy default stream).
+ *
+ * CUDA graph capture.  Both calls may be recorded into a CUDA graph (cudaStreamBeginCapture ... cudaStreamEndCapture,
+ * or torch.cuda.graph), in any capture mode, global included.  While `cuda_stream` is capturing a call:
+ *   - enqueues kernel launches on `cuda_stream` and nothing else: no allocation, no synchronisation, no copy;
+ *   - uses only the first-use state the context already has: step tables, Gray16 LUTs and the verified fast forms
+ *     (divisions, premultiplication).  What is missing takes, for this call only, the path that needs no preparation
+ *     (the generic exact kernel, or the reference instruction sequence) -- bit-identical outputs, typically slower
+ *     kernels.  Nothing is cached, and the call's pixels do not count towards avifgpu_set_table_autobuild.
+ *     Prepare before capturing so that the graph holds the tuned kernels: avifgpu_prepare_encode (step tables, Gray16
+ *     LUTs), avifgpu_prepare_decode (HLG / PQ / green divisions), and for integer planar encodes with premultiplied
+ *     alpha one direct call outside the capture (the premultiply check);
+ *   - returns a launch failure without synchronising anything: ending the capture is the caller's business.
+ * The graph holds the pointers, strides, row block and description of the captured call: to convert another frame,
+ * copy it into the captured buffers and replay.  avifgpu_launch_count counts the captured kernels once, at capture, and
+ * not per replay.  The graph refers to the context's tables, which are never freed or moved before avifgpu_destroy:
+ * it stays valid, whatever the context prepares later, until then.  The legacy NULL stream cannot be captured; capture
+ * on a stream of your own. */
 AVIFGPU_EXPORT int avifgpu_encode_rows_device(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
                                               const void* device_rows, int64_t row_stride_bytes,
                                               int32_t y0, int32_t nrows, const avifgpu_planes* device_dst,
@@ -404,6 +421,11 @@ typedef struct avifgpu_curve_stats
  * avifgpu_set_table_autobuild). */
 AVIFGPU_EXPORT int avifgpu_prepare_encode(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
                                           avifgpu_curve_stats* out_stats);
+
+/* Does now the first-use work a decode of `desc` would do: the on-device checks behind the tuned float decode's HLG and
+ * PQ divisions and the YCbCr decodes' green-channel division (once per context and configuration).
+ * Optional, except before capturing a decode into a CUDA graph. */
+AVIFGPU_EXPORT int avifgpu_prepare_decode(avifgpu_context* ctx, const avifgpu_decode_desc* desc);
 
 /* Without avifgpu_prepare_encode() the encode calls convert with the exact kernel (glibc-identical powf per sample)
  * until `pixels` pixels of one configuration have gone through this context, and build the step tables then.

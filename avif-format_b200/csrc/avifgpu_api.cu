@@ -24,21 +24,6 @@
 
 namespace avifgpu
 {
-int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* stream);
-int LaunchDecodeGeneric(const DecodeParams& params, void* stream);
-int LaunchEncodeFast(const EncodeParams& params, int hostDepth, void* stream);   // 0 = not applicable
-int LaunchEncodeFastInteger(const EncodeParams& params, int hostDepth, void* stream); // 0 = not applicable
-int LaunchEncodeFastGray32(const EncodeParams& params, int hostDepth, void* stream);  // 0 = not applicable
-cudaError_t BuildGray16Lut(uint16_t* deviceLut, int smpte428, uint32_t maxCode, void* stream);
-long long VerifyHlgDivisions(void* stream);
-long long VerifyPqRatio(void* stream);
-long long VerifyFastPremultiply(uint32_t maxCode, void* stream);
-long long VerifyGreenDivision(const DecodeParams& params, void* stream);
-int LaunchDecodeFast(const DecodeParams& params, void* stream);                  // 0 = not applicable
-int LaunchDecodeFastInteger(const DecodeParams& params, void* stream);           // 0 = not applicable
-int LaunchDecodeFastTable(const DecodeParams& params, void* stream);             // 0 = not applicable
-int LaunchHlgOotf(int inverse, const float luma[3], float displayGamma, float peak, const float* in, float* out, size_t pixels, void* stream);
-
 namespace
 {
     thread_local int g_launchFailure = 0; // cudaError_t of the last failed launch on this thread, 0 = none
@@ -428,20 +413,6 @@ struct avifgpu_context
         }
         cudaGetLastError();
         lastError = std::string(what) + " failed: " + (code != 0 ? cudaGetErrorString(static_cast<cudaError_t>(code)) : avifgpu_status_string(status));
-        return status;
-    }
-
-    // Any failure in the middle of a host-pointer call: same draining, then the status.
-    int Abandon(int status)
-    {
-        for (cudaStream_t stream : streams)
-        {
-            if (stream)
-            {
-                cudaStreamSynchronize(stream);
-            }
-        }
-        cudaGetLastError();
         return status;
     }
 
@@ -914,7 +885,7 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_device(avifgpu_context* ctx, const avifgp
     p.rowCount = nrows;
     p.yPhase = y0 & p.ys;
     p.smCount = ctx->smCount;
-    DeviceGuard deviceGuardForTables(ctx->device);
+    DeviceGuard guard(ctx->device);
     bool capturing;
     if ((status = QueryCapture(ctx, cuda_stream, &capturing)) != AVIFGPU_OK)
     {
@@ -935,7 +906,6 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_device(avifgpu_context* ctx, const avifgp
         p.plane[k] = static_cast<const uint8_t*>(device_src->data[k]) + static_cast<int64_t>(y0 >> g.ys) * device_src->stride[k];
         p.planeStride[k] = device_src->stride[k];
     }
-    DeviceGuard guard(ctx->device);
     const int launched = LaunchDecode(p, cuda_stream);
     if (launched < 0)
     {

@@ -11,6 +11,9 @@
 
 #include <atomic>
 
+#include <driver_types.h>
+
+#include "../../include/avifgpu.h"
 #include "curve_tables.h"
 #include "pixel_math.cuh"
 
@@ -114,16 +117,107 @@ struct DecodeParams
     int32_t verifiedPqRatio;       // 1 once the context has verified the branch-free division inside PQToLinear on this device
 };
 
+// The block restricted to its sub-rectangle [x0, x0 + width) x [y0, y0 + rows), for the edge strips the tuned
+// launchers leave to the generic kernel.  Plane k moves by (y0 >> ys_k) rows and (x0 >> xs_k) sites of
+// samplesPerPixel_k samples, as EncodePlaneGeometry / DecodePlaneGeometry lay the planes out: only planes 1 and 2 are
+// sub-sampled (FillEncodeParams / FillDecodeParams leave xs = ys = 0 for every other layout), and only plane 0 of the
+// reference layout with three or more channels interleaves `channels` samples per pixel.  A null plane stays null.
+// Blocks carry no column phase, so x0 starts a chroma site (a multiple of 1 << xs); an encode block has no row phase
+// either, so y0 is a multiple of 1 << ys (tests/native/launch_window_check.cpp).
+inline EncodeParams EncodeWindow(const EncodeParams& p, int hostDepth, int x0, int y0, int width, int rows)
+{
+    EncodeParams w = p;
+    w.rows = static_cast<const uint8_t*>(p.rows) + static_cast<int64_t>(y0) * p.rowStride + static_cast<int64_t>(x0) * p.channels * (hostDepth / 8);
+    const int sampleBytes = p.imageDepth > 8 ? 2 : 1;
+    for (int k = 0; k < 4; ++k)
+    {
+        if (p.plane[k] == nullptr)
+        {
+            continue;
+        }
+        const bool chroma = k == 1 || k == 2;
+        const int samplesPerPixel = (!p.planar && k == 0 && p.channels >= 3) ? p.channels : 1;
+        w.plane[k] = static_cast<uint8_t*>(p.plane[k]) + static_cast<int64_t>(y0 >> (chroma ? p.ys : 0)) * p.planeStride[k] +
+                     static_cast<int64_t>(x0 >> (chroma ? p.xs : 0)) * samplesPerPixel * sampleBytes;
+    }
+    w.width = width;
+    w.rowCount = rows;
+    return w;
+}
+
+// The same for a decode block, whose first row may be the second of a 4:2:0 row pair (yPhase = 1): the chroma planes
+// move by the chroma rows between the two first rows, and the window's phase is that of its own first row, so y0 may
+// be odd.
+inline DecodeParams DecodeWindow(const DecodeParams& p, int x0, int y0, int width, int rows)
+{
+    DecodeParams w = p;
+    const int channels = (p.colorspace == AVIFGPU_COLORSPACE_MONOCHROME ? 1 : 3) + (p.hasAlpha ? 1 : 0);
+    w.rows = static_cast<uint8_t*>(p.rows) + static_cast<int64_t>(y0) * p.rowStride + static_cast<int64_t>(x0) * channels * (p.hostDepth / 8);
+    const int sampleBytes = p.bitDepth > 8 ? 2 : 1;
+    for (int k = 0; k < 4; ++k)
+    {
+        if (p.plane[k] == nullptr)
+        {
+            continue;
+        }
+        const bool chroma = k == 1 || k == 2;
+        const int planeRows = chroma ? (p.yPhase + y0) >> p.ys : y0;
+        w.plane[k] = static_cast<const uint8_t*>(p.plane[k]) + static_cast<int64_t>(planeRows) * p.planeStride[k] +
+                     static_cast<int64_t>(x0 >> (chroma ? p.xs : 0)) * sampleBytes;
+    }
+    w.width = width;
+    w.rowCount = rows;
+    w.yPhase = (p.yPhase + y0) & p.ys;
+    return w;
+}
+
+// True when `p` and every row `stride` bytes after it start on an `alignment`-byte boundary.
+inline bool Aligned(const void* p, int64_t stride, int alignment)
+{
+    return (reinterpret_cast<uintptr_t>(p) % alignment) == 0 && (stride % alignment) == 0;
+}
+
+// The SM count the tuned launchers size their grids by: the context's, or H100's 132 when it is unknown.
+inline int SmCountOrDefault(int32_t smCount)
+{
+    return smCount > 0 ? smCount : 132;
+}
+
 // A launcher that sees a CUDA error has already consumed it (cudaGetLastError clears the slot), so it leaves the code
 // here -- a thread-local slot in avifgpu_api.cu -- and returns AVIFGPU_ERR_CUDA; the API reports it from there instead
 // of asking CUDA a second time (which would answer cudaSuccess and turn a failed launch into AVIFGPU_OK).
 int ReportLaunchFailure(int cudaErrorCode);
 
 // Launchers implemented in kernels_*.cu.  They only enqueue work on `stream` and return the number of kernels
-// launched (>= 1) or a negative avifgpu_status.
+// launched (>= 1) or a negative avifgpu_status; the tuned ones (LaunchEncodeFast*, LaunchDecodeFast*) return 0 for a
+// configuration they do not cover.
 int LaunchEncode(const EncodeParams& params, int hostDepth, void* stream);
 int LaunchDecode(const DecodeParams& params, void* stream);
+int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* stream);
+int LaunchDecodeGeneric(const DecodeParams& params, void* stream);
+int LaunchEncodeFast(const EncodeParams& params, int hostDepth, void* stream);
+int LaunchEncodeFastInteger(const EncodeParams& params, int hostDepth, void* stream);
+int LaunchEncodeFastGray32(const EncodeParams& params, int hostDepth, void* stream);
+int LaunchDecodeFast(const DecodeParams& params, void* stream);
+int LaunchDecodeFastInteger(const DecodeParams& params, void* stream);
+int LaunchDecodeFastTable(const DecodeParams& params, void* stream);
 int LaunchTransfer(int function, float param, const float* in, float* out, size_t count, void* stream);
+int LaunchHlgOotf(int inverse, const float luma[3], float displayGamma, float peak, const float* in, float* out, size_t pixels, void* stream);
+
+// The end of every tuned launch site.  A tuned kernel converts the block's aligned interior [0, coveredWidth) x
+// [0, coveredRows); `tuned` is its launch status.  On success the generic kernel converts the right strip
+// [coveredWidth, width) x [0, rowCount), then the bottom strip [0, coveredWidth) x [coveredRows, rowCount); an empty
+// strip launches nothing.  Returns 1 + the strip launches, or a negative status.
+int CompleteEncode(cudaError_t tuned, const EncodeParams& p, int hostDepth, int coveredWidth, int coveredRows, void* stream);
+int CompleteDecode(cudaError_t tuned, const DecodeParams& p, int coveredWidth, int coveredRows, void* stream);
+
+cudaError_t BuildGray16Lut(uint16_t* deviceLut, int smpte428, uint32_t maxCode, void* stream);
+
+// Exhaustive device checks of the arithmetic shortcuts (kernels_fast_decode.cu, kernels_fast_int.cu).
+long long VerifyHlgDivisions(void* stream);
+long long VerifyPqRatio(void* stream);
+long long VerifyFastPremultiply(uint32_t maxCode, void* stream);
+long long VerifyGreenDivision(const DecodeParams& params, void* stream);
 
 } // namespace avifgpu
 

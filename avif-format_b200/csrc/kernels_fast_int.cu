@@ -658,11 +658,6 @@ cudaError_t LaunchGrayInt(const Rgb16Params& rp, int channels, int smCount, cuda
     return cudaGetLastError();
 }
 
-bool Aligned(const void* p, int64_t stride, int alignment)
-{
-    return (reinterpret_cast<uintptr_t>(p) % alignment) == 0 && (stride % alignment) == 0;
-}
-
 template <typename HostT, typename PlaneT, int CHANNELS, int PREMULTIPLY>
 cudaError_t LaunchRgbInt(const Rgb16Params& rp, int xs, int ys, int smCount, cudaStream_t stream)
 {
@@ -686,8 +681,6 @@ cudaError_t LaunchRgbIntChannels(const Rgb16Params& rp, int channels, bool premu
 }
 
 } // namespace
-
-int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* stream);
 
 // Runs the exhaustive comparison behind FastPremultiplyBiased for one bit depth; returns the number of disagreements
 // (0 = verified) or -1 on a CUDA error.  Synchronous.
@@ -722,7 +715,7 @@ int LaunchEncodeFastInteger(const EncodeParams& p, int hostDepth, void* streamHa
     {
         return 0;
     }
-    const int smCount = p.smCount > 0 ? p.smCount : 132;
+    const int smCount = SmCountOrDefault(p.smCount);
 
     if (hostDepth == 16 && p.imageDepth > 8 && p.channels == 1 && !p.planar)
     {
@@ -744,23 +737,7 @@ int LaunchEncodeFastInteger(const EncodeParams& p, int hostDepth, void* streamHa
         gp.rowCount = p.rowCount;
         gp.lut = p.gray16Lut;
         EncodeGray16LutKernel<<<smCount, kLutThreads, kLutEntries * 2, stream>>>(gp);
-        if (const cudaError_t launchError = cudaGetLastError())
-        {
-            return ReportLaunchFailure(static_cast<int>(launchError));
-        }
-        int launched = 1;
-        const int covered = gp.chunksPerRow * 8;
-        if (covered < p.width)
-        {
-            EncodeParams strip = p;
-            strip.rows = static_cast<const uint8_t*>(p.rows) + static_cast<int64_t>(covered) * 2;
-            strip.width = p.width - covered;
-            strip.plane[0] = static_cast<uint8_t*>(p.plane[0]) + static_cast<int64_t>(covered) * 2;
-            const int n = LaunchEncodeGeneric(strip, hostDepth, streamHandle);
-            if (n < 0) return n;
-            launched += n;
-        }
-        return launched;
+        return CompleteEncode(cudaGetLastError(), p, hostDepth, gp.chunksPerRow * 8, p.rowCount, streamHandle);
     }
 
     // Gray(+A) hosts in the reference layout (Y plane [0], alpha plane [3]); premultiplication and the Gray16 SMPTE 428
@@ -799,23 +776,7 @@ int LaunchEncodeFastInteger(const EncodeParams& p, int hostDepth, void* streamHa
         {
             e = planeBytes == 2 ? LaunchGrayInt<uint8_t, uint16_t>(rp, p.channels, smCount, stream) : LaunchGrayInt<uint8_t, uint8_t>(rp, p.channels, smCount, stream);
         }
-        if (e != cudaSuccess)
-        {
-            return ReportLaunchFailure(static_cast<int>(e));
-        }
-        int launched = 1;
-        if (width8 < p.width)
-        {
-            EncodeParams strip = p;
-            strip.rows = static_cast<const uint8_t*>(p.rows) + static_cast<int64_t>(width8) * p.channels * hostBytes;
-            strip.width = p.width - width8;
-            strip.plane[0] = static_cast<uint8_t*>(p.plane[0]) + static_cast<int64_t>(width8) * planeBytes;
-            if (p.channels == 2) strip.plane[3] = static_cast<uint8_t*>(p.plane[3]) + static_cast<int64_t>(width8) * planeBytes;
-            const int n = LaunchEncodeGeneric(strip, hostDepth, streamHandle);
-            if (n < 0) return n;
-            launched += n;
-        }
-        return launched;
+        return CompleteEncode(e, p, hostDepth, width8, p.rowCount, streamHandle);
     }
 
     // The biased-truncation trick needs non-negative intermediates: true for every matrix with kr, kg, kb >= 0
@@ -869,40 +830,7 @@ int LaunchEncodeFastInteger(const EncodeParams& p, int hostDepth, void* streamHa
             e = planeBytes == 2 ? LaunchRgbIntChannels<uint8_t, uint16_t>(rp, p.channels, p.premultiply != 0, p.xs, p.ys, smCount, stream)
                                 : LaunchRgbIntChannels<uint8_t, uint8_t>(rp, p.channels, p.premultiply != 0, p.xs, p.ys, smCount, stream);
         }
-        if (e != cudaSuccess)
-        {
-            return ReportLaunchFailure(static_cast<int>(e));
-        }
-        int launched = 1;
-        const int colBytes = p.channels * hostBytes;
-        if (width8 < p.width)
-        {
-            EncodeParams strip = p;
-            strip.rows = static_cast<const uint8_t*>(p.rows) + static_cast<int64_t>(width8) * colBytes;
-            strip.width = p.width - width8;
-            strip.plane[0] = static_cast<uint8_t*>(p.plane[0]) + static_cast<int64_t>(width8) * planeBytes;
-            strip.plane[1] = static_cast<uint8_t*>(p.plane[1]) + static_cast<int64_t>(width8 >> p.xs) * planeBytes;
-            strip.plane[2] = static_cast<uint8_t*>(p.plane[2]) + static_cast<int64_t>(width8 >> p.xs) * planeBytes;
-            if (p.channels == 4) strip.plane[3] = static_cast<uint8_t*>(p.plane[3]) + static_cast<int64_t>(width8) * planeBytes;
-            const int n = LaunchEncodeGeneric(strip, hostDepth, streamHandle);
-            if (n < 0) return n;
-            launched += n;
-        }
-        if (evenRows < p.rowCount)
-        {
-            EncodeParams strip = p;
-            strip.rows = static_cast<const uint8_t*>(p.rows) + static_cast<int64_t>(evenRows) * p.rowStride;
-            strip.rowCount = p.rowCount - evenRows;
-            strip.width = width8;
-            strip.plane[0] = static_cast<uint8_t*>(p.plane[0]) + static_cast<int64_t>(evenRows) * p.planeStride[0];
-            strip.plane[1] = static_cast<uint8_t*>(p.plane[1]) + static_cast<int64_t>(evenRows >> p.ys) * p.planeStride[1];
-            strip.plane[2] = static_cast<uint8_t*>(p.plane[2]) + static_cast<int64_t>(evenRows >> p.ys) * p.planeStride[2];
-            if (p.channels == 4) strip.plane[3] = static_cast<uint8_t*>(p.plane[3]) + static_cast<int64_t>(evenRows) * p.planeStride[3];
-            const int n = LaunchEncodeGeneric(strip, hostDepth, streamHandle);
-            if (n < 0) return n;
-            launched += n;
-        }
-        return launched;
+        return CompleteEncode(e, p, hostDepth, width8, evenRows, streamHandle);
     }
     return 0;
 }

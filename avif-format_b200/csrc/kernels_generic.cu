@@ -615,6 +615,37 @@ int LaunchDecodeGeneric(const DecodeParams& p, void* streamHandle)
     return launchError == cudaSuccess ? 1 : ReportLaunchFailure(static_cast<int>(launchError));
 }
 
+// The generic launchers return 0 for an empty strip.
+int CompleteEncode(cudaError_t tuned, const EncodeParams& p, int hostDepth, int coveredWidth, int coveredRows, void* stream)
+{
+    if (tuned != cudaSuccess)
+    {
+        return ReportLaunchFailure(static_cast<int>(tuned));
+    }
+    const int right = LaunchEncodeGeneric(EncodeWindow(p, hostDepth, coveredWidth, 0, p.width - coveredWidth, p.rowCount), hostDepth, stream);
+    if (right < 0)
+    {
+        return right;
+    }
+    const int bottom = LaunchEncodeGeneric(EncodeWindow(p, hostDepth, 0, coveredRows, coveredWidth, p.rowCount - coveredRows), hostDepth, stream);
+    return bottom < 0 ? bottom : 1 + right + bottom;
+}
+
+int CompleteDecode(cudaError_t tuned, const DecodeParams& p, int coveredWidth, int coveredRows, void* stream)
+{
+    if (tuned != cudaSuccess)
+    {
+        return ReportLaunchFailure(static_cast<int>(tuned));
+    }
+    const int right = LaunchDecodeGeneric(DecodeWindow(p, coveredWidth, 0, p.width - coveredWidth, p.rowCount), stream);
+    if (right < 0)
+    {
+        return right;
+    }
+    const int bottom = LaunchDecodeGeneric(DecodeWindow(p, 0, coveredRows, coveredWidth, p.rowCount - coveredRows), stream);
+    return bottom < 0 ? bottom : 1 + right + bottom;
+}
+
 int LaunchTransfer(int function, float param, const float* in, float* out, size_t count, void* streamHandle)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);

@@ -915,6 +915,210 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_device(avifgpu_context* ctx, const avifgp
     return AVIFGPU_OK;
 }
 
+AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const avifgpu_batch_image* images,
+                                               int32_t count, void* cuda_stream)
+{
+    if (ctx == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    if (desc == nullptr || count < 0 || (count > 0 && images == nullptr))
+    {
+        return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL description or image array");
+    }
+    // every image is validated before anything is enqueued
+    std::vector<EncodeParams> params(static_cast<size_t>(count));
+    int64_t pixels = 0;
+    for (int32_t i = 0; i < count; ++i)
+    {
+        const avifgpu_batch_image& image = images[i];
+        avifgpu_encode_desc d = *desc;
+        d.width = image.width;
+        d.height = image.height;
+        std::string error;
+        const int status = ValidateEncodeDesc(&d, &error);
+        if (status != AVIFGPU_OK)
+        {
+            return ctx->Fail(status, "image " + std::to_string(i) + ": " + error);
+        }
+        EncodeParams& p = params[i];
+        FillEncodeParams(d, &p);
+        if (d.width == 0 || d.height == 0)
+        {
+            p.width = 0;
+            p.rowCount = 0;
+            continue;
+        }
+        if (image.rows == nullptr)
+        {
+            return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "image " + std::to_string(i) + ": NULL rows");
+        }
+        p.rows = image.rows;
+        p.rowStride = image.row_stride_bytes;
+        p.rowCount = d.height;
+        for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
+        {
+            if (!EncodePlaneGeometry(d, k).present)
+            {
+                continue;
+            }
+            if (image.planes.data[k] == nullptr)
+            {
+                return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "image " + std::to_string(i) + ": missing destination plane");
+            }
+            p.plane[k] = image.planes.data[k];
+            p.planeStride[k] = image.planes.stride[k];
+        }
+        pixels += static_cast<int64_t>(d.width) * d.height;
+    }
+    if (pixels == 0)
+    {
+        return AVIFGPU_OK;
+    }
+    DeviceGuard guard(ctx->device);
+    bool capturing;
+    int status = QueryCapture(ctx, cuda_stream, &capturing);
+    if (status != AVIFGPU_OK)
+    {
+        return status;
+    }
+    EncodeParams firstUse;
+    FillEncodeParams(*desc, &firstUse);
+    ctx->FirstUseEncode(*desc, pixels, capturing, &firstUse);
+    for (EncodeParams& p : params)
+    {
+        p.smCount = ctx->smCount;
+        p.curveTable = firstUse.curveTable;
+        p.gray16Lut = firstUse.gray16Lut;
+        p.verifiedPremultiply = firstUse.verifiedPremultiply;
+    }
+    BatchPlan plan;
+    PlanEncodeBatch(params, desc->host_depth, &plan);
+    for (const BatchChunk& chunk : plan.chunks)
+    {
+        const int launched = LaunchEncodeBatchChunk(params[chunk.imageIndex[0]], desc->host_depth, chunk, cuda_stream);
+        if (launched < 0)
+        {
+            return ctx->LaunchFailed(launched, "batched encode kernel launch", capturing);
+        }
+        ctx->launches += launched;
+    }
+    for (const int32_t i : plan.fallback)
+    {
+        const int launched = LaunchEncode(params[i], desc->host_depth, cuda_stream);
+        if (launched < 0)
+        {
+            return ctx->LaunchFailed(launched, "encode kernel launch", capturing);
+        }
+        ctx->launches += launched;
+    }
+    return AVIFGPU_OK;
+}
+
+AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifgpu_decode_desc* desc, const avifgpu_batch_image* images,
+                                               int32_t count, void* cuda_stream)
+{
+    if (ctx == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    if (desc == nullptr || count < 0 || (count > 0 && images == nullptr))
+    {
+        return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL description or image array");
+    }
+    // every image is validated before anything is enqueued
+    std::vector<DecodeParams> params(static_cast<size_t>(count));
+    int32_t transfer = 0;
+    int64_t pixels = 0;
+    for (int32_t i = 0; i < count; ++i)
+    {
+        const avifgpu_batch_image& image = images[i];
+        avifgpu_decode_desc d = *desc;
+        d.width = image.width;
+        d.height = image.height;
+        std::string error;
+        const int status = ValidateDecodeDesc(&d, &transfer, &error);
+        if (status != AVIFGPU_OK)
+        {
+            return ctx->Fail(status, "image " + std::to_string(i) + ": " + error);
+        }
+        DecodeParams& p = params[i];
+        if (!FillDecodeParams(d, transfer, &p, &error))
+        {
+            return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "image " + std::to_string(i) + ": " + error);
+        }
+        if (d.width == 0 || d.height == 0)
+        {
+            p.width = 0;
+            p.rowCount = 0;
+            continue;
+        }
+        if (image.rows == nullptr)
+        {
+            return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "image " + std::to_string(i) + ": NULL rows");
+        }
+        p.rows = image.rows;
+        p.rowStride = image.row_stride_bytes;
+        p.rowCount = d.height;
+        p.yPhase = 0;
+        for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
+        {
+            if (!DecodePlaneGeometry(d, k).present)
+            {
+                continue;
+            }
+            if (image.planes.data[k] == nullptr)
+            {
+                return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "image " + std::to_string(i) + ": missing source plane");
+            }
+            p.plane[k] = image.planes.data[k];
+            p.planeStride[k] = image.planes.stride[k];
+        }
+        pixels += static_cast<int64_t>(d.width) * d.height;
+    }
+    if (pixels == 0)
+    {
+        return AVIFGPU_OK;
+    }
+    DeviceGuard guard(ctx->device);
+    bool capturing;
+    int status = QueryCapture(ctx, cuda_stream, &capturing);
+    if (status != AVIFGPU_OK)
+    {
+        return status;
+    }
+    DecodeParams firstUse = params[0];
+    ctx->FirstUseDecode(*desc, transfer, capturing, &firstUse);
+    for (DecodeParams& p : params)
+    {
+        p.smCount = ctx->smCount;
+        p.verifiedHlgDivisions = firstUse.verifiedHlgDivisions;
+        p.verifiedGreenDivision = firstUse.verifiedGreenDivision;
+        p.verifiedPqRatio = firstUse.verifiedPqRatio;
+    }
+    BatchPlan plan;
+    PlanDecodeBatch(params, &plan);
+    for (const BatchChunk& chunk : plan.chunks)
+    {
+        const int launched = LaunchDecodeBatchChunk(params[chunk.imageIndex[0]], chunk, cuda_stream);
+        if (launched < 0)
+        {
+            return ctx->LaunchFailed(launched, "batched decode kernel launch", capturing);
+        }
+        ctx->launches += launched;
+    }
+    for (const int32_t i : plan.fallback)
+    {
+        const int launched = LaunchDecode(params[i], cuda_stream);
+        if (launched < 0)
+        {
+            return ctx->LaunchFailed(launched, "decode kernel launch", capturing);
+        }
+        ctx->launches += launched;
+    }
+    return AVIFGPU_OK;
+}
+
 } // extern "C"
 
 // ---- host-pointer entry points (PCIe inside) ---------------------------------------------------------------------

@@ -432,4 +432,154 @@ bool FillDecodeParams(const avifgpu_decode_desc& d, int32_t transfer, DecodePara
     return true;
 }
 
+
+// The conditions LaunchEncodeFastInteger's planar branch checks, in its order.  The biased-truncation trick needs
+// non-negative intermediates: true for every matrix with kr, kg, kb >= 0 (all of H.273's); anything else takes the
+// generic kernel.
+Interior EncodeRgbIntInterior(const EncodeParams& p, int hostDepth)
+{
+    const Interior none = { 0, 0 };
+    if ((hostDepth != 16 && hostDepth != 8) || !p.planar || (p.channels != 3 && p.channels != 4) ||
+        (p.premultiply && !(p.channels == 4 && p.verifiedPremultiply)) || p.imageDepth > 12 ||
+        !(p.matrix.identity || (p.matrix.kr >= 0.0f && p.matrix.kg >= 0.0f && p.matrix.kb >= 0.0f && p.matrix.kr < 1.0f && p.matrix.kb < 1.0f)) ||
+        !ForwardMatrixStaysInRange(p.matrix, p.chromaOffset, static_cast<int>(p.maxCode)))
+    {
+        return none;
+    }
+    const int hostBytes = hostDepth / 8;
+    const int planeBytes = p.imageDepth > 8 ? 2 : 1;
+    const int rowAlign = (8 * p.channels * hostBytes) % 16 == 0 ? 16 : 8; // a thread's 8-pixel chunk: 128-bit or 64-bit loads
+    const int lumaAlign = 8 * planeBytes;
+    const int chromaAlign = (p.xs ? 4 : 8) * planeBytes;
+    if (p.width < 8 || !Aligned(p.rows, p.rowStride, rowAlign) || !Aligned(p.plane[0], p.planeStride[0], lumaAlign) ||
+        !Aligned(p.plane[1], p.planeStride[1], chromaAlign) || !Aligned(p.plane[2], p.planeStride[2], chromaAlign) ||
+        (p.channels == 4 && !Aligned(p.plane[3], p.planeStride[3], lumaAlign)))
+    {
+        return none;
+    }
+    const int evenRows = p.ys ? (p.rowCount & ~1) : p.rowCount;
+    if (evenRows < 1)
+    {
+        return none;
+    }
+    return Interior{ p.width & ~7, evenRows };
+}
+
+// The conditions LaunchDecodeFastInteger checks before it runs DecodeYccToRgbIntKernel, in its order.
+Interior DecodeYccIntInterior(const DecodeParams& p)
+{
+    const Interior none = { 0, 0 };
+    if ((p.hostDepth != 8 && p.hostDepth != 16) || p.bitDepth > 12 || (p.hasAlpha && p.premultiplied) || p.colorspace != AVIFGPU_COLORSPACE_YCBCR ||
+        p.yPhase != 0)
+    {
+        return none;
+    }
+    const int sampleBytes = p.hostDepth == 8 ? 1 : 2;
+    if ((sampleBytes == 1) != (p.bitDepth <= 8))
+    {
+        return none; // 8-bit hosts read 8-bit planes, 16-bit hosts read 16-bit planes (ReadHeifImage.cpp:83, 186)
+    }
+    const int channels = p.hasAlpha ? 4 : 3;
+    const int lumaAlign = 8 * sampleBytes;
+    const int chromaAlign = (p.xs ? 4 : 8) * sampleBytes;
+    const int rowAlign = channels == 4 ? 16 : 8 * sampleBytes; // RGB8: 64-bit stores, everything else 128-bit
+    if (!Aligned(p.plane[0], p.planeStride[0], lumaAlign) || !Aligned(p.plane[1], p.planeStride[1], chromaAlign) ||
+        !Aligned(p.plane[2], p.planeStride[2], chromaAlign) || (p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], lumaAlign)) ||
+        !Aligned(p.rows, p.rowStride, rowAlign))
+    {
+        return none;
+    }
+    const int width8 = p.width & ~7;
+    const int evenRows = p.ys ? (p.rowCount & ~1) : p.rowCount;
+    if (width8 < 8 || evenRows < 1)
+    {
+        return none;
+    }
+    return Interior{ width8, evenRows };
+}
+
+namespace
+{
+template <typename Params>
+BatchRecord RecordOf(const Params& w)
+{
+    BatchRecord r{};
+    r.rows = w.rows;
+    r.rowStride = w.rowStride;
+    for (int k = 0; k < 4; ++k)
+    {
+        r.plane[k] = const_cast<void*>(static_cast<const void*>(w.plane[k]));
+        r.planeStride[k] = w.planeStride[k];
+    }
+    r.width = w.width;
+    r.rowCount = w.rowCount;
+    return r;
+}
+
+// Both directions: `interiorOf` is the single-image predicate, `windowOf(p, x0, y0, width, rows)` the launchers' window
+// and `edgeUnits(p, width, rows)` the units of one.
+template <typename Params, typename InteriorOf, typename WindowOf, typename EdgeUnits>
+void PlanBatch(const std::vector<Params>& images, BatchPlan* plan, InteriorOf interiorOf, WindowOf windowOf, EdgeUnits edgeUnits)
+{
+    plan->chunks.clear();
+    plan->fallback.clear();
+    for (int32_t i = 0; i < static_cast<int32_t>(images.size()); ++i)
+    {
+        const Params& p = images[i];
+        if (p.width <= 0 || p.rowCount <= 0)
+        {
+            continue;
+        }
+        const Interior inner = interiorOf(p);
+        if (inner.width == 0)
+        {
+            plan->fallback.push_back(i);
+            continue;
+        }
+        if (plan->chunks.empty() || plan->chunks.back().images == kBatchChunkImages)
+        {
+            plan->chunks.emplace_back();
+        }
+        BatchChunk& c = plan->chunks.back();
+        BatchRecord& r = c.interior[c.images];
+        r = RecordOf(windowOf(p, 0, 0, inner.width, inner.rows));
+        r.firstUnit = c.interiorUnits;
+        c.interiorUnits += BatchInteriorUnits(inner.width, inner.rows, p.ys);
+        c.imageIndex[c.images++] = i;
+        // the strips CompleteEncode / CompleteDecode hand to the generic kernel, in their order: right, then bottom
+        const int windowX[2] = { inner.width, 0 }, windowY[2] = { 0, inner.rows };
+        const int windowWidth[2] = { p.width - inner.width, inner.width }, windowRows[2] = { p.rowCount, p.rowCount - inner.rows };
+        for (int k = 0; k < 2; ++k)
+        {
+            if (windowWidth[k] <= 0 || windowRows[k] <= 0)
+            {
+                continue;
+            }
+            BatchRecord& w = c.window[c.windows];
+            w = RecordOf(windowOf(p, windowX[k], windowY[k], windowWidth[k], windowRows[k]));
+            w.firstUnit = c.windowUnits;
+            c.windowUnits += edgeUnits(p, windowWidth[k], windowRows[k]);
+            c.windowImage[c.windows++] = i;
+        }
+    }
+}
+} // namespace
+
+void PlanEncodeBatch(const std::vector<EncodeParams>& images, int hostDepth, BatchPlan* plan)
+{
+    PlanBatch(
+        images, plan, [&](const EncodeParams& p) { return EncodeRgbIntInterior(p, hostDepth); },
+        [&](const EncodeParams& p, int x0, int y0, int width, int rows) { return EncodeWindow(p, hostDepth, x0, y0, width, rows); },
+        [](const EncodeParams& p, int width, int rows) { return BatchEdgeUnits(width, rows, p.xs, p.ys); });
+}
+
+// An image starts at row 0 and its bottom window at an even row, so every decode window has yPhase 0.
+void PlanDecodeBatch(const std::vector<DecodeParams>& images, BatchPlan* plan)
+{
+    PlanBatch(
+        images, plan, [](const DecodeParams& p) { return DecodeYccIntInterior(p); },
+        [](const DecodeParams& p, int x0, int y0, int width, int rows) { return DecodeWindow(p, x0, y0, width, rows); },
+        [](const DecodeParams&, int width, int rows) { return BatchEdgeUnits(width, rows, 0, 0); }); // one thread per pixel
+}
+
 } // namespace avifgpu

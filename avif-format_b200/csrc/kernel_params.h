@@ -10,6 +10,7 @@
 #include <stdint.h>
 
 #include <atomic>
+#include <vector>
 
 #include <driver_types.h>
 
@@ -183,6 +184,79 @@ inline int SmCountOrDefault(int32_t smCount)
     return smCount > 0 ? smCount : 132;
 }
 
+// The aligned interior [0, width) x [0, rows) the tuned integer planar encode kernel (EncodeRgbIntPlanarKernel)
+// converts for this block, or {0, 0} when a direct call of the block takes another route: 8/16-bit RGB(A) hosts into
+// planar YCbCr of at most 12 bits, no alpha, straight alpha or a verified premultiply, a matrix the biased truncation
+// handles, 8-pixel-aligned buffers and at least 8 x (1 << ys) pixels.  width is a multiple of 8, rows of 1 << ys.
+struct Interior
+{
+    int32_t width;
+    int32_t rows;
+};
+Interior EncodeRgbIntInterior(const EncodeParams& p, int hostDepth);
+// The same for the tuned integer YCbCr decode kernel (DecodeYccToRgbIntKernel): 8/16-bit hosts reading 8-bit / 10-12-bit
+// YCbCr (+ straight alpha), a block starting on a 4:2:0 row pair, aligned buffers, at least 8 x (1 << ys) pixels.
+Interior DecodeYccIntInterior(const DecodeParams& p);
+
+// ---- batches of whole images (avifgpu_encode_batch_device, avifgpu_decode_batch_device) -----------------------------------------------------------
+//
+// What differs between the images of a batched launch; the launch carries these records by value as a kernel parameter
+// (no allocation, no copy, legal while capturing), so a chunk holds at most kBatchChunkImages images.  A launch walks one
+// unit space made by concatenating its records' units: record i owns [firstUnit_i, firstUnit_{i+1}).
+struct BatchRecord
+{
+    const void* rows;       // host-layout rows (encode source, decode destination) at the record's first row
+    int64_t rowStride;
+    void* plane[4];         // the same row in each plane (encode destination, decode source), as Encode/DecodeWindow place it
+    int64_t planeStride[4];
+    int32_t width;          // pixels
+    int32_t rowCount;
+    int64_t firstUnit;
+};
+
+constexpr int kBatchChunkImages = 64;
+constexpr int kBatchUnitPixels = 256; // interior unit: 256 pixels of one row (row pair for 4:2:0), one warp
+constexpr int kBatchEdgeThreads = 256; // edge unit: one CTA-sized run of chroma sites (encode) or pixels (decode) of one row (pair)
+
+// Units of an interior of `width` x `rows` pixels, and of an edge window.
+inline int64_t BatchInteriorUnits(int width, int rows, int ys)
+{
+    return static_cast<int64_t>((width + kBatchUnitPixels - 1) / kBatchUnitPixels) * ((rows + ys) >> ys);
+}
+inline int64_t BatchEdgeUnits(int width, int rows, int xs, int ys)
+{
+    return static_cast<int64_t>((((width + xs) >> xs) + kBatchEdgeThreads - 1) / kBatchEdgeThreads) * ((rows + ys) >> ys);
+}
+
+// One chunk: at most two launches -- the batched tuned kernel over every image's interior, then the batched generic
+// kernel over every image's right strip and odd last 4:2:0 row (none when no image has one).
+struct BatchChunk
+{
+    int32_t images = 0;                       // interiors in this chunk
+    int32_t imageIndex[kBatchChunkImages];    // their positions in the caller's array, increasing
+    BatchRecord interior[kBatchChunkImages];
+    int64_t interiorUnits = 0;
+    int32_t windows = 0;
+    int32_t windowImage[2 * kBatchChunkImages]; // position in the caller's array of each window's image
+    BatchRecord window[2 * kBatchChunkImages];
+    int64_t windowUnits = 0;
+};
+
+struct BatchPlan
+{
+    std::vector<BatchChunk> chunks;
+    std::vector<int32_t> fallback; // positions of the images that take one direct call each (LaunchEncode), in order
+};
+
+// Splits whole-image blocks (one EncodeParams per image; images with no pixels are skipped) into chunks of the images
+// EncodeRgbIntInterior takes, in order, and direct calls for the rest.
+void PlanEncodeBatch(const std::vector<EncodeParams>& images, int hostDepth, BatchPlan* plan);
+// The same for decode blocks, with DecodeYccIntInterior.
+void PlanDecodeBatch(const std::vector<DecodeParams>& images, BatchPlan* plan);
+
+// Launches of one chunk: 1 + (1 when it has edge windows).
+inline int BatchChunkLaunches(const BatchChunk& chunk) { return 1 + (chunk.windows > 0 ? 1 : 0); }
+
 // A launcher that sees a CUDA error has already consumed it (cudaGetLastError clears the slot), so it leaves the code
 // here -- a thread-local slot in avifgpu_api.cu -- and returns AVIFGPU_ERR_CUDA; the API reports it from there instead
 // of asking CUDA a second time (which would answer cudaSuccess and turn a failed launch into AVIFGPU_OK).
@@ -210,6 +284,11 @@ int LaunchHlgOotf(int inverse, const float luma[3], float displayGamma, float pe
 // strip launches nothing.  Returns 1 + the strip launches, or a negative status.
 int CompleteEncode(cudaError_t tuned, const EncodeParams& p, int hostDepth, int coveredWidth, int coveredRows, void* stream);
 int CompleteDecode(cudaError_t tuned, const DecodeParams& p, int coveredWidth, int coveredRows, void* stream);
+
+// The launches of one planned chunk (kernels_batch.cu); `shared` is the block of any of its images (every field but
+// the pointers, strides and sizes is the same for all of them).  Returns BatchChunkLaunches(chunk) or a negative status.
+int LaunchEncodeBatchChunk(const EncodeParams& shared, int hostDepth, const BatchChunk& chunk, void* stream);
+int LaunchDecodeBatchChunk(const DecodeParams& shared, const BatchChunk& chunk, void* stream);
 
 cudaError_t BuildGray16Lut(uint16_t* deviceLut, int smpte428, uint32_t maxCode, void* stream);
 

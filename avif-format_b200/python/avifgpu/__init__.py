@@ -68,6 +68,10 @@ def library():
         [ctx_p, C.POINTER(abi.EncodeDesc), C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(abi.Planes), C.c_void_p])
     sig("avifgpu_decode_rows_device", C.c_int,
         [ctx_p, C.POINTER(abi.DecodeDesc), C.POINTER(abi.Planes), C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p])
+    sig("avifgpu_encode_batch_device", C.c_int,
+        [ctx_p, C.POINTER(abi.EncodeDesc), C.POINTER(abi.BatchImage), C.c_int32, C.c_void_p])
+    sig("avifgpu_decode_batch_device", C.c_int,
+        [ctx_p, C.POINTER(abi.DecodeDesc), C.POINTER(abi.BatchImage), C.c_int32, C.c_void_p])
     sig("avifgpu_transfer_f32", C.c_int, [ctx_p, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_size_t])
     sig("avifgpu_prepare_encode", C.c_int, [ctx_p, C.POINTER(abi.EncodeDesc), C.POINTER(abi.CurveStats)])
     sig("avifgpu_prepare_decode", C.c_int, [ctx_p, C.POINTER(abi.DecodeDesc)])
@@ -126,7 +130,7 @@ EXPORTED_SYMBOLS = [
     "avifgpu_encode_host_col_bytes", "avifgpu_decode_host_col_bytes", "avifgpu_encode_plane_geometry",
     "avifgpu_decode_plane_geometry", "avifgpu_get_yuv_coefficients", "avifgpu_get_hlg_luma_coefficients",
     "avifgpu_build_yuv_tables", "avifgpu_encode_rows", "avifgpu_decode_rows", "avifgpu_encode_rows_device",
-    "avifgpu_decode_rows_device", "avifgpu_transfer_f32", "avifgpu_prepare_encode", "avifgpu_set_table_autobuild",
+    "avifgpu_decode_rows_device", "avifgpu_encode_batch_device", "avifgpu_decode_batch_device", "avifgpu_transfer_f32", "avifgpu_prepare_encode", "avifgpu_set_table_autobuild",
     "avifgpu_hlg_ootf_f32", "avifgpu_prepare_decode",
     "avifgpu_encode_rows_async", "avifgpu_decode_rows_async", "avifgpu_wait",
     "avifgpu_shard_group_create", "avifgpu_shard_group_destroy", "avifgpu_shard_group_size", "avifgpu_shard_group_context",
@@ -299,6 +303,14 @@ class Context:
         self._check(self.lib.avifgpu_encode_rows_device(self.handle, C.byref(desc), rows_ptr, row_stride, y0, nrows,
                                                         C.byref(planes_struct), stream))
 
+    def encode_batch_device(self, desc, images, stream=0):
+        """avifgpu_encode_batch_device: `images` is a ctypes array of abi.BatchImage (see batch_images_from_tensors)."""
+        self._check(self.lib.avifgpu_encode_batch_device(self.handle, C.byref(desc), images, len(images), stream))
+
+    def decode_batch_device(self, desc, images, stream=0):
+        """avifgpu_decode_batch_device: `images` is a ctypes array of abi.BatchImage (planes = source, rows = destination)."""
+        self._check(self.lib.avifgpu_decode_batch_device(self.handle, C.byref(desc), images, len(images), stream))
+
     def decode_device(self, desc, planes_struct, rows_ptr, row_stride, y0=0, nrows=None, stream=0):
         nrows = desc.height - y0 if nrows is None else nrows
         self._check(self.lib.avifgpu_decode_rows_device(self.handle, C.byref(desc), C.byref(planes_struct), y0, nrows,
@@ -417,3 +429,19 @@ def planes_from_tensors(tensors):
             planes.data[i] = t.data_ptr()
             planes.stride[i] = t.stride(0) * t.element_size()
     return planes
+
+
+def batch_images_from_tensors(images):
+    """A ctypes array of abi.BatchImage for [(width, height, rows, planes)]: `rows` a 2-D torch CUDA tensor of host-layout
+    rows (or None), `planes` a list of 2-D torch CUDA tensors or None, as for planes_from_tensors.  Encode reads the rows
+    and writes the planes, decode the other way round."""
+    out = (abi.BatchImage * len(images))()
+    for i, (width, height, rows, planes) in enumerate(images):
+        out[i].width = width
+        out[i].height = height
+        if rows is not None:
+            assert rows.dim() == 2 and rows.stride(1) == 1
+            out[i].rows = rows.data_ptr()
+            out[i].row_stride_bytes = rows.stride(0) * rows.element_size()
+        out[i].planes = planes_from_tensors(planes)
+    return out

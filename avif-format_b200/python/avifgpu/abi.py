@@ -8,7 +8,7 @@ import ctypes as C
 
 import numpy as np
 
-API_VERSION = 5
+API_VERSION = 6
 
 # avifgpu_status
 OK = 0
@@ -64,6 +64,17 @@ class Planes(C.Structure):
     _fields_ = [
         ("data", C.c_void_p * MAX_PLANES),
         ("stride", C.c_int64 * MAX_PLANES),
+    ]
+
+
+class BatchImage(C.Structure):
+    """avifgpu_batch_image: one whole image of a batch call (device pointers)."""
+    _fields_ = [
+        ("width", C.c_int32),
+        ("height", C.c_int32),
+        ("rows", C.c_void_p),
+        ("row_stride_bytes", C.c_int64),
+        ("planes", Planes),
     ]
 
 

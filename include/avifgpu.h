@@ -50,7 +50,7 @@ extern "C" {
 #define AVIFGPU_EXPORT __attribute__((visibility("default")))
 #endif
 
-#define AVIFGPU_API_VERSION 5
+#define AVIFGPU_API_VERSION 6
 
 typedef enum avifgpu_status
 {
@@ -339,6 +339,49 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_device(avifgpu_context* ctx, const avifgp
                                               const avifgpu_planes* device_src, int32_t y0, int32_t nrows,
                                               void* device_rows, int64_t row_stride_bytes,
                                               void* cuda_stream);
+
+/* ---- the hot path: batches of small device-resident images ------------------------------------------------ */
+
+/* One image of a batch: a whole image of the batch's description with its own size and buffers (device memory).
+ *   encode: rows = the source host-layout rows, planes = the destination planes;
+ *   decode: planes = the source planes, rows = the destination host-layout rows. */
+typedef struct avifgpu_batch_image
+{
+    int32_t width;
+    int32_t height;
+    void* rows;
+    int64_t row_stride_bytes;
+    avifgpu_planes planes;
+} avifgpu_batch_image;
+
+/*
+ * Converts `count` whole images with one encode description, many per kernel launch: for small images (thumbnails, image
+ * sets) a launch per image costs more than the image's own memory traffic.
+ *   - All images share `desc`; its width and height are replaced by each image's own.
+ *   - Each image is converted whole, like avifgpu_encode_rows_device with y0 = 0 and nrows = height.
+ *   - The result equals `count` such calls, one per image, in order, on `cuda_stream`, bit for bit.
+ *   - Every image is validated as `desc` with its own size, and its rows and planes are checked for NULL, before
+ *     anything is enqueued: one bad image fails the whole call (AVIFGPU_ERR_BAD_PARAM or AVIFGPU_ERR_UNSUPPORTED)
+ *     and nothing is launched.  count == 0 is AVIFGPU_OK with no launch; images of width or height 0 are skipped.
+ *   - The outputs of different images must not overlap.
+ *   - Like the device calls above it does not synchronise, may be captured into a CUDA graph under the same rules,
+ *     and avifgpu_launch_count counts what it launched.  The first-use work (premultiply check, Gray16 LUT, step
+ *     tables) is done once per call, outside a capture, for the batch's pixels.
+ * Images the tuned integer planar kernel takes in a direct call (8/16-bit RGB(A) hosts into planar YCbCr, aligned
+ * buffers, width >= 8) are converted in chunks of up to 64 images, at most two launches per chunk: one for every
+ * image's aligned interior, one for every image's right strip and odd last 4:2:0 row.  Every other image takes one
+ * direct call, after the chunks.
+ */
+AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
+                                               const avifgpu_batch_image* images, int32_t count, void* cuda_stream);
+
+/* The same for decodes: like `count` calls of avifgpu_decode_rows_device with y0 = 0 and nrows = height, one per image, in
+ * order.  Images the tuned integer YCbCr decode takes in a direct call (8/16-bit hosts reading YCbCr 8/10/12-bit,
+ * straight or no alpha, aligned buffers, width >= 8) go through chunks of up to 64 images, at most two launches per
+ * chunk; every other image takes one direct call, after the chunks.  The first-use work (the verified divisions) is
+ * done once per call, outside a capture. */
+AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
+                                               const avifgpu_batch_image* images, int32_t count, void* cuda_stream);
 
 /* ---- the hot path across several GPUs of one box (SURVEY.md 8e) ------------------------------------------------ */
 

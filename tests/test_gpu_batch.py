@@ -10,6 +10,7 @@ import pytest
 
 import cases
 from avifgpu import abi
+from test_gpu_multipass import pick
 
 pytestmark = pytest.mark.gpu
 
@@ -34,7 +35,7 @@ def padded(n):
 class Image:
     """One image's seeded host rows and sentinel-padded planes, as byte tensors on the GPU."""
 
-    def __init__(self, desc, w, h, seed, misalign=0):
+    def __init__(self, desc, w, h, seed, misalign=0, beyond=False):
         import torch
         self.w, self.h = w, h
         d = self.desc = batch_desc(desc, w, h)
@@ -42,7 +43,7 @@ class Image:
         if d.host_depth == 32:
             self.host = cases.float_host_rows(rng, h, w, d.host_channels)
         else:
-            self.host = cases.int_host_rows(rng, h, w, d.host_channels, d.host_depth)
+            self.host = cases.int_host_rows(rng, h, w, d.host_channels, d.host_depth, beyond=beyond)
         row_bytes = w * d.host_channels * d.host_depth // 8
         backing = torch.zeros((max(h, 1), padded(row_bytes) + misalign), dtype=torch.uint8, device="cuda")
         self.rows = backing[:, misalign:misalign + row_bytes]
@@ -87,7 +88,7 @@ def run_batch(ctx, desc, images, stream=0):
     ctx.encode_batch_device(desc, avifgpu.batch_images_from_tensors([im.record() for im in images]), stream=stream)
 
 
-def assert_same_as_direct(ctx, images, checker=None):
+def assert_same_as_direct(ctx, images, checker=None, threads=1):
     import torch
     for im in images:
         reference = im.fresh_planes()
@@ -100,7 +101,7 @@ def assert_same_as_direct(ctx, images, checker=None):
             assert np.array_equal(a, b), (im.w, im.h, k)
             assert (a[:, got.shape[1]:] == SENTINEL).all(), ("padding overwritten", im.w, im.h, k)
         if checker is not None and im.w and im.h:
-            expected = checker.encode(im.desc, im.host)
+            expected = checker.encode(im.desc, im.host, threads=threads)
             for k, got in enumerate(im.planes):
                 if got is not None:
                     codes = got.cpu().numpy().view(abi.code_dtype(im.desc.image_bit_depth))
@@ -277,12 +278,12 @@ def test_captured_batch_replays_like_direct_calls(ctx):
 class DecImage:
     """One image's seeded source planes and sentinel-padded destination rows, as byte tensors on the GPU."""
 
-    def __init__(self, desc, w, h, seed, misalign=0):
+    def __init__(self, desc, w, h, seed, misalign=0, overshoot=False):
         import torch
         self.w, self.h = w, h
         d = self.desc = abi.DecodeDesc.from_buffer_copy(desc)
         d.width, d.height = w, h
-        self.codes = cases.code_planes(cases.rng_for(f"dbatch_{seed}_{w}x{h}"), d)
+        self.codes = cases.code_planes(cases.rng_for(f"dbatch_{seed}_{w}x{h}"), d, overshoot=overshoot)
         self.planes = []
         for c in self.codes:
             if c is None:
@@ -313,7 +314,7 @@ def run_decode_batch(ctx, desc, images, stream=0):
     ctx.decode_batch_device(desc, avifgpu.batch_images_from_tensors([im.record() for im in images]), stream=stream)
 
 
-def assert_decode_same_as_direct(ctx, images, checker=None):
+def assert_decode_same_as_direct(ctx, images, checker=None, threads=1):
     import torch
     for im in images:
         reference = im.alloc()
@@ -323,7 +324,7 @@ def assert_decode_same_as_direct(ctx, images, checker=None):
         assert np.array_equal(a, b), (im.w, im.h)
         assert (a[:, im.row_bytes:] == SENTINEL).all(), ("padding overwritten", im.w, im.h)
         if checker is not None and im.w and im.h:
-            expected = checker.decode(im.desc, im.codes)
+            expected = checker.decode(im.desc, im.codes, threads=threads)
             got = im.rows.cpu().numpy().view(abi.host_dtype(im.desc.host_depth))
             assert np.array_equal(got, expected), ("checker", im.w, im.h)
 
@@ -346,7 +347,7 @@ DECODE = [
 def test_decode_batch_equals_direct_calls_and_checker(ctx, checker, port, name, desc):
     images = [DecImage(desc, w, h, f"{name}_{i}") for i, (w, h) in enumerate(SIZES)]
     run_decode_batch(ctx, desc, images)
-    assert_decode_same_as_direct(ctx, images, checker if checker.kind == "reference" else port)
+    assert_decode_same_as_direct(ctx, images, pick(checker, port, True))
 
 
 @pytest.mark.parametrize("n", [1, 8, 64])

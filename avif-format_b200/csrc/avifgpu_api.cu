@@ -3,6 +3,7 @@
 // converts pixels launches a CUDA kernel or fails.
 #include "../../include/avifgpu.h"
 
+#include "batch_indirect.h"
 #include "curve_tables.h"
 #include "host_params.h"
 #include "kernel_params.h"
@@ -1116,6 +1117,153 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifg
         }
         ctx->launches += launched;
     }
+    return AVIFGPU_OK;
+}
+
+AVIFGPU_EXPORT int avifgpu_batch_workspace_bytes(int32_t max_count, size_t* out_bytes)
+{
+    if (out_bytes == nullptr || max_count < 1 || max_count > kIndirectMaxImages)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    *out_bytes = IndirectWorkspaceLayout(max_count).bytes;
+    return AVIFGPU_OK;
+}
+
+} // extern "C"
+
+namespace
+{
+    // The host checks both device-described calls make before anything is launched.
+    int CheckIndirect(avifgpu_context* ctx, const void* images, const int32_t* count, int32_t maxCount, const void* workspace, size_t workspaceBytes)
+    {
+        if (images == nullptr || count == nullptr || workspace == nullptr)
+        {
+            return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL device image array, count or workspace");
+        }
+        if (maxCount < 1 || maxCount > kIndirectMaxImages)
+        {
+            return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "max_count must be 1..4096");
+        }
+        if (workspaceBytes < IndirectWorkspaceLayout(maxCount).bytes)
+        {
+            return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "workspace smaller than avifgpu_batch_workspace_bytes(max_count)");
+        }
+        return AVIFGPU_OK;
+    }
+} // namespace
+
+extern "C" {
+
+AVIFGPU_EXPORT int avifgpu_encode_batch_indirect(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const avifgpu_batch_image* device_images,
+                                                 const int32_t* device_count, int32_t max_count, void* device_workspace, size_t workspace_bytes,
+                                                 int32_t* device_status, void* cuda_stream)
+{
+    if (ctx == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    if (desc == nullptr)
+    {
+        return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL description");
+    }
+    avifgpu_encode_desc d = *desc; // the images carry the sizes
+    d.width = 0;
+    d.height = 0;
+    std::string error;
+    int status = ValidateEncodeDesc(&d, &error);
+    if (status != AVIFGPU_OK)
+    {
+        return ctx->Fail(status, error);
+    }
+    if ((status = CheckIndirect(ctx, device_images, device_count, max_count, device_workspace, workspace_bytes)) != AVIFGPU_OK)
+    {
+        return status;
+    }
+    if ((d.host_depth != 8 && d.host_depth != 16) || d.layout != AVIFGPU_LAYOUT_PLANAR_YCBCR)
+    {
+        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "device-described batches encode 8- or 16-bit RGB(A) hosts into planar YCbCr");
+    }
+    EncodeParams shared;
+    FillEncodeParams(d, &shared);
+    int planeMask = 0;
+    for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
+    {
+        planeMask |= EncodePlaneGeometry(d, k).present ? 1 << k : 0;
+    }
+    DeviceGuard guard(ctx->device);
+    bool capturing;
+    if ((status = QueryCapture(ctx, cuda_stream, &capturing)) != AVIFGPU_OK)
+    {
+        return status;
+    }
+    shared.smCount = ctx->smCount;
+    ctx->FirstUseEncode(d, 0, capturing, &shared);
+    const int launched = LaunchEncodeIndirect(shared, d.host_depth, EncodeRgbIntTuned(shared, d.host_depth), planeMask, device_images, device_count,
+                                              max_count, device_workspace, device_status, cuda_stream);
+    if (launched < 0)
+    {
+        return ctx->LaunchFailed(launched, "device-described batch encode launch", capturing);
+    }
+    ctx->launches += launched;
+    return AVIFGPU_OK;
+}
+
+AVIFGPU_EXPORT int avifgpu_decode_batch_indirect(avifgpu_context* ctx, const avifgpu_decode_desc* desc, const avifgpu_batch_image* device_images,
+                                                 const int32_t* device_count, int32_t max_count, void* device_workspace, size_t workspace_bytes,
+                                                 int32_t* device_status, void* cuda_stream)
+{
+    if (ctx == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    if (desc == nullptr)
+    {
+        return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL description");
+    }
+    avifgpu_decode_desc d = *desc;
+    d.width = 0;
+    d.height = 0;
+    std::string error;
+    int32_t transfer = 0;
+    int status = ValidateDecodeDesc(&d, &transfer, &error);
+    if (status != AVIFGPU_OK)
+    {
+        return ctx->Fail(status, error);
+    }
+    if ((status = CheckIndirect(ctx, device_images, device_count, max_count, device_workspace, workspace_bytes)) != AVIFGPU_OK)
+    {
+        return status;
+    }
+    if ((d.host_depth != 8 && d.host_depth != 16) || d.colorspace != AVIFGPU_COLORSPACE_YCBCR || d.alpha_state == AVIFGPU_ALPHA_PREMULTIPLIED)
+    {
+        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "device-described batches decode YCbCr with no or straight alpha into 8- or 16-bit hosts");
+    }
+    DecodeParams shared;
+    if (!FillDecodeParams(d, transfer, &shared, &error))
+    {
+        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, error);
+    }
+    int planeMask = 0;
+    for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
+    {
+        planeMask |= DecodePlaneGeometry(d, k).present ? 1 << k : 0;
+    }
+    DeviceGuard guard(ctx->device);
+    bool capturing;
+    if ((status = QueryCapture(ctx, cuda_stream, &capturing)) != AVIFGPU_OK)
+    {
+        return status;
+    }
+    shared.smCount = ctx->smCount;
+    ctx->FirstUseDecode(d, transfer, capturing, &shared);
+    const int launched = LaunchDecodeIndirect(shared, DecodeYccIntTuned(shared), planeMask, device_images, device_count, max_count, device_workspace,
+                                              device_status, cuda_stream);
+    if (launched < 0)
+    {
+        return ctx->LaunchFailed(launched, "device-described batch decode launch", capturing);
+    }
+    ctx->launches += launched;
     return AVIFGPU_OK;
 }
 

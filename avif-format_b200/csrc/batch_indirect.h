@@ -1,0 +1,205 @@
+// batch_indirect.h -- the device-described batches of avifgpu_encode_batch_indirect / avifgpu_decode_batch_indirect.
+//
+// The image records, their count and the workspace live in device memory and are read when the work runs, so one call
+// (or one captured graph of it) converts whatever the buffers hold at that moment.  A call is three launches:
+//   1. the plan kernel (one CTA) routes every image with the per-image step below -- the same functions PlanEncodeBatch /
+//      PlanDecodeBatch call -- and writes, per image, one interior record and up to two window records, the exclusive
+//      prefix sums of their units and the two totals into the workspace;
+//   2. the interior kernel walks the interior units with the tuned integer kernel's per-unit code;
+//   3. the edge kernel walks the window units with the generic kernel's per-site / per-pixel code.
+// Plain C++ (AVIFGPU_HD): tests/native/indirect_plan_check.cpp compiles the per-image step with the host compiler.
+#ifndef AVIF_BATCH_INDIRECT_H
+#define AVIF_BATCH_INDIRECT_H
+
+#include <stddef.h>
+#include <stdint.h>
+
+#include "../../include/avifgpu.h"
+#include "kernel_params.h"
+
+namespace avifgpu
+{
+
+constexpr int kIndirectMaxImages = 4096;
+
+// The workspace of a call of at most maxCount images: a header, then the first units of the interiors (maxCount) and
+// of the windows (2 * maxCount, image i owning 2i and 2i + 1), then the records in the same order.  A record that owns
+// no unit (an empty or rejected image, a missing strip) has the first unit of the next, so the last record whose first
+// unit is at most u owns unit u.
+struct IndirectHeader
+{
+    int64_t interiorUnits;
+    int64_t windowUnits;
+    int32_t count; // images planned: *device_count, or 0 when it was out of range
+    int32_t reserved;
+};
+
+struct IndirectLayout
+{
+    size_t interiorFirst, windowFirst, interior, window, bytes; // byte offsets, and the total
+};
+
+AVIFGPU_HD inline size_t IndirectAlign(size_t bytes) { return (bytes + 255) / 256 * 256; }
+
+AVIFGPU_HD inline IndirectLayout IndirectWorkspaceLayout(int maxCount)
+{
+    const size_t n = static_cast<size_t>(maxCount);
+    IndirectLayout l;
+    l.interiorFirst = IndirectAlign(sizeof(IndirectHeader));
+    l.windowFirst = l.interiorFirst + IndirectAlign(sizeof(int64_t) * n);
+    l.interior = l.windowFirst + IndirectAlign(sizeof(int64_t) * 2 * n);
+    l.window = l.interior + IndirectAlign(sizeof(BatchRecord) * n);
+    l.bytes = l.window + IndirectAlign(sizeof(BatchRecord) * 2 * n);
+    return l;
+}
+
+// The last of `count` records whose first unit is at most `unit` -- the record that owns it -- searching from `record`,
+// whose first unit is at most `unit` already (a worker passes the record of its previous unit: units only increase).
+AVIFGPU_HD inline int FindRecord(const int64_t* first, int count, int record, long long unit)
+{
+    if (record + 1 >= count || unit < first[record + 1])
+    {
+        return record;
+    }
+    int lo = record + 1, hi = count - 1;
+    while (lo < hi)
+    {
+        const int mid = (lo + hi + 1) >> 1;
+        if (first[mid] <= unit)
+        {
+            lo = mid;
+        }
+        else
+        {
+            hi = mid - 1;
+        }
+    }
+    return lo;
+}
+
+// One image's part of the plan: its status, its interior record (width 0: none) and its windows, with their units.
+struct IndirectImagePlan
+{
+    int32_t status;
+    int32_t windows;
+    BatchRecord interior;
+    int64_t interiorUnits;
+    BatchRecord window[2];
+    int64_t windowUnits[2];
+};
+
+// Puts the record's size, rows and the planes of `planeMask` (bit k: the description has plane k) into `p`, with the
+// host-described calls' checks: AVIFGPU_ERR_BAD_PARAM for a negative size, or for a non-empty image with NULL rows or a
+// NULL plane the description has.
+template <typename Params>
+AVIFGPU_HD inline int AdoptBatchImage(Params& p, int planeMask, const avifgpu_batch_image& image)
+{
+    if (image.width < 0 || image.height < 0)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    p.width = image.width;
+    p.rowCount = image.height;
+    if (image.width == 0 || image.height == 0)
+    {
+        return AVIFGPU_OK;
+    }
+    if (image.rows == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    p.rows = image.rows;
+    p.rowStride = image.row_stride_bytes;
+    for (int k = 0; k < 4; ++k)
+    {
+        p.plane[k] = nullptr;
+        p.planeStride[k] = 0;
+        if ((planeMask >> k) & 1)
+        {
+            if (image.planes.data[k] == nullptr)
+            {
+                return AVIFGPU_ERR_BAD_PARAM;
+            }
+            p.plane[k] = image.planes.data[k];
+            p.planeStride[k] = image.planes.stride[k];
+        }
+    }
+    return AVIFGPU_OK;
+}
+
+// The per-image step of the plan.  `shared` is the description's block (FillEncodeParams), `tuned` EncodeRgbIntTuned of
+// it.  An image the tuned kernel takes in a direct call gets its interior and the strips CompleteEncode would hand to
+// the generic kernel; any other non-empty image becomes one whole-image window, which is what the generic kernel
+// converts in a direct call.
+AVIFGPU_HD inline IndirectImagePlan PlanIndirectEncodeImage(const EncodeParams& shared, int hostDepth, bool tuned, int planeMask,
+                                                            const avifgpu_batch_image& image)
+{
+    IndirectImagePlan plan{};
+    EncodeParams p = shared;
+    plan.status = AdoptBatchImage(p, planeMask, image);
+    if (plan.status != AVIFGPU_OK || p.width == 0 || p.rowCount == 0)
+    {
+        return plan;
+    }
+    const Interior inner = tuned ? EncodeRgbIntBlockInterior(p, hostDepth) : Interior{ 0, 0 };
+    if (inner.width == 0)
+    {
+        plan.window[0] = RecordOf(EncodeWindow(p, hostDepth, 0, 0, p.width, p.rowCount));
+        plan.windowUnits[0] = BatchEdgeUnits(p.width, p.rowCount, p.xs, p.ys);
+        plan.windows = 1;
+        return plan;
+    }
+    plan.interior = RecordOf(EncodeWindow(p, hostDepth, 0, 0, inner.width, inner.rows));
+    plan.interiorUnits = BatchInteriorUnits(inner.width, inner.rows, p.ys);
+    Strip strip[2];
+    plan.windows = InteriorStrips(p.width, p.rowCount, inner, strip);
+    for (int k = 0; k < plan.windows; ++k)
+    {
+        plan.window[k] = RecordOf(EncodeWindow(p, hostDepth, strip[k].x0, strip[k].y0, strip[k].width, strip[k].rows));
+        plan.windowUnits[k] = BatchEdgeUnits(strip[k].width, strip[k].rows, p.xs, p.ys);
+    }
+    return plan;
+}
+
+// The same for decodes (`tuned` = DecodeYccIntTuned); edge units are runs of pixels of one row.
+AVIFGPU_HD inline IndirectImagePlan PlanIndirectDecodeImage(const DecodeParams& shared, bool tuned, int planeMask, const avifgpu_batch_image& image)
+{
+    IndirectImagePlan plan{};
+    DecodeParams p = shared;
+    plan.status = AdoptBatchImage(p, planeMask, image);
+    if (plan.status != AVIFGPU_OK || p.width == 0 || p.rowCount == 0)
+    {
+        return plan;
+    }
+    p.yPhase = 0;
+    const Interior inner = tuned ? DecodeYccIntBlockInterior(p) : Interior{ 0, 0 };
+    if (inner.width == 0)
+    {
+        plan.window[0] = RecordOf(DecodeWindow(p, 0, 0, p.width, p.rowCount));
+        plan.windowUnits[0] = BatchEdgeUnits(p.width, p.rowCount, 0, 0);
+        plan.windows = 1;
+        return plan;
+    }
+    plan.interior = RecordOf(DecodeWindow(p, 0, 0, inner.width, inner.rows));
+    plan.interiorUnits = BatchInteriorUnits(inner.width, inner.rows, p.ys);
+    Strip strip[2];
+    plan.windows = InteriorStrips(p.width, p.rowCount, inner, strip);
+    for (int k = 0; k < plan.windows; ++k)
+    {
+        plan.window[k] = RecordOf(DecodeWindow(p, strip[k].x0, strip[k].y0, strip[k].width, strip[k].rows));
+        plan.windowUnits[k] = BatchEdgeUnits(strip[k].width, strip[k].rows, 0, 0);
+    }
+    return plan;
+}
+
+// The launchers (kernels_batch_indirect.cu): the plan, interior and edge kernels of one call on `stream`.  `shared` is the
+// description's block with the context's first-use state; `tuned` its description half of the routing.  Return 3 (the
+// launches) or a negative status.
+int LaunchEncodeIndirect(const EncodeParams& shared, int hostDepth, bool tuned, int planeMask, const avifgpu_batch_image* images,
+                         const int32_t* count, int maxCount, void* workspace, int32_t* status, void* stream);
+int LaunchDecodeIndirect(const DecodeParams& shared, bool tuned, int planeMask, const avifgpu_batch_image* images, const int32_t* count,
+                         int maxCount, void* workspace, int32_t* status, void* stream);
+
+} // namespace avifgpu
+
+#endif

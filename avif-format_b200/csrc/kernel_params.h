@@ -18,6 +18,15 @@
 #include "curve_tables.h"
 #include "pixel_math.cuh"
 
+// The routing and window arithmetic below is plain C++ that the plan kernel of the device-described batch calls
+// (kernels_batch_indirect.cu) runs on the device too; the attribute is empty for the host compiler (host_params.cpp,
+// tests/native).
+#if defined(__CUDACC__)
+#define AVIFGPU_HD __host__ __device__
+#else
+#define AVIFGPU_HD
+#endif
+
 namespace avifgpu
 {
 
@@ -125,7 +134,7 @@ struct DecodeParams
 // reference layout with three or more channels interleaves `channels` samples per pixel.  A null plane stays null.
 // Blocks carry no column phase, so x0 starts a chroma site (a multiple of 1 << xs); an encode block has no row phase
 // either, so y0 is a multiple of 1 << ys (tests/native/launch_window_check.cpp).
-inline EncodeParams EncodeWindow(const EncodeParams& p, int hostDepth, int x0, int y0, int width, int rows)
+AVIFGPU_HD inline EncodeParams EncodeWindow(const EncodeParams& p, int hostDepth, int x0, int y0, int width, int rows)
 {
     EncodeParams w = p;
     w.rows = static_cast<const uint8_t*>(p.rows) + static_cast<int64_t>(y0) * p.rowStride + static_cast<int64_t>(x0) * p.channels * (hostDepth / 8);
@@ -149,7 +158,7 @@ inline EncodeParams EncodeWindow(const EncodeParams& p, int hostDepth, int x0, i
 // The same for a decode block, whose first row may be the second of a 4:2:0 row pair (yPhase = 1): the chroma planes
 // move by the chroma rows between the two first rows, and the window's phase is that of its own first row, so y0 may
 // be odd.
-inline DecodeParams DecodeWindow(const DecodeParams& p, int x0, int y0, int width, int rows)
+AVIFGPU_HD inline DecodeParams DecodeWindow(const DecodeParams& p, int x0, int y0, int width, int rows)
 {
     DecodeParams w = p;
     const int channels = (p.colorspace == AVIFGPU_COLORSPACE_MONOCHROME ? 1 : 3) + (p.hasAlpha ? 1 : 0);
@@ -173,7 +182,7 @@ inline DecodeParams DecodeWindow(const DecodeParams& p, int x0, int y0, int widt
 }
 
 // True when `p` and every row `stride` bytes after it start on an `alignment`-byte boundary.
-inline bool Aligned(const void* p, int64_t stride, int alignment)
+AVIFGPU_HD inline bool Aligned(const void* p, int64_t stride, int alignment)
 {
     return (reinterpret_cast<uintptr_t>(p) % alignment) == 0 && (stride % alignment) == 0;
 }
@@ -193,10 +202,80 @@ struct Interior
     int32_t width;
     int32_t rows;
 };
-Interior EncodeRgbIntInterior(const EncodeParams& p, int hostDepth);
+// EncodeRgbIntInterior in two halves: the description's (host depth, layout, channels, premultiply, depth, matrix --
+// the same for every block of one description, host only) and the block's (buffer alignment, at least 8 pixels and one
+// 4:2:0 row pair).
+bool EncodeRgbIntTuned(const EncodeParams& p, int hostDepth);
+AVIFGPU_HD inline Interior EncodeRgbIntBlockInterior(const EncodeParams& p, int hostDepth)
+{
+    const Interior none = { 0, 0 };
+    const int hostBytes = hostDepth / 8;
+    const int planeBytes = p.imageDepth > 8 ? 2 : 1;
+    const int rowAlign = (8 * p.channels * hostBytes) % 16 == 0 ? 16 : 8; // a thread's 8-pixel chunk: 128-bit or 64-bit loads
+    const int lumaAlign = 8 * planeBytes;
+    const int chromaAlign = (p.xs ? 4 : 8) * planeBytes;
+    if (p.width < 8 || !Aligned(p.rows, p.rowStride, rowAlign) || !Aligned(p.plane[0], p.planeStride[0], lumaAlign) ||
+        !Aligned(p.plane[1], p.planeStride[1], chromaAlign) || !Aligned(p.plane[2], p.planeStride[2], chromaAlign) ||
+        (p.channels == 4 && !Aligned(p.plane[3], p.planeStride[3], lumaAlign)))
+    {
+        return none;
+    }
+    const int evenRows = p.ys ? (p.rowCount & ~1) : p.rowCount;
+    if (evenRows < 1)
+    {
+        return none;
+    }
+    return Interior{ p.width & ~7, evenRows };
+}
+Interior EncodeRgbIntInterior(const EncodeParams& p, int hostDepth); // EncodeRgbIntTuned ? EncodeRgbIntBlockInterior : none
+
 // The same for the tuned integer YCbCr decode kernel (DecodeYccToRgbIntKernel): 8/16-bit hosts reading 8-bit / 10-12-bit
 // YCbCr (+ straight alpha), a block starting on a 4:2:0 row pair, aligned buffers, at least 8 x (1 << ys) pixels.
-Interior DecodeYccIntInterior(const DecodeParams& p);
+bool DecodeYccIntTuned(const DecodeParams& p);
+AVIFGPU_HD inline Interior DecodeYccIntBlockInterior(const DecodeParams& p)
+{
+    const Interior none = { 0, 0 };
+    const int sampleBytes = p.hostDepth == 8 ? 1 : 2;
+    const int channels = p.hasAlpha ? 4 : 3;
+    const int lumaAlign = 8 * sampleBytes;
+    const int chromaAlign = (p.xs ? 4 : 8) * sampleBytes;
+    const int rowAlign = channels == 4 ? 16 : 8 * sampleBytes; // RGB8: 64-bit stores, everything else 128-bit
+    if (!Aligned(p.plane[0], p.planeStride[0], lumaAlign) || !Aligned(p.plane[1], p.planeStride[1], chromaAlign) ||
+        !Aligned(p.plane[2], p.planeStride[2], chromaAlign) || (p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], lumaAlign)) ||
+        !Aligned(p.rows, p.rowStride, rowAlign))
+    {
+        return none;
+    }
+    const int width8 = p.width & ~7;
+    const int evenRows = p.ys ? (p.rowCount & ~1) : p.rowCount;
+    if (width8 < 8 || evenRows < 1)
+    {
+        return none;
+    }
+    return Interior{ width8, evenRows };
+}
+Interior DecodeYccIntInterior(const DecodeParams& p); // DecodeYccIntTuned ? DecodeYccIntBlockInterior : none
+
+// The strips CompleteEncode / CompleteDecode hand to the generic kernel around a block's interior, in their order: the
+// right strip [inner.width, width) x [0, rows), then the bottom strip [0, inner.width) x [inner.rows, rows).  Returns how
+// many of the two are non-empty; those come first in `strip`.
+struct Strip
+{
+    int32_t x0, y0, width, rows;
+};
+AVIFGPU_HD inline int InteriorStrips(int width, int rows, Interior inner, Strip strip[2])
+{
+    const Strip candidate[2] = { { inner.width, 0, width - inner.width, rows }, { 0, inner.rows, inner.width, rows - inner.rows } };
+    int count = 0;
+    for (int k = 0; k < 2; ++k)
+    {
+        if (candidate[k].width > 0 && candidate[k].rows > 0)
+        {
+            strip[count++] = candidate[k];
+        }
+    }
+    return count;
+}
 
 // ---- batches of whole images (avifgpu_encode_batch_device, avifgpu_decode_batch_device) -----------------------------------------------------------
 //
@@ -219,13 +298,30 @@ constexpr int kBatchUnitPixels = 256; // interior unit: 256 pixels of one row (r
 constexpr int kBatchEdgeThreads = 256; // edge unit: one CTA-sized run of chroma sites (encode) or pixels (decode) of one row (pair)
 
 // Units of an interior of `width` x `rows` pixels, and of an edge window.
-inline int64_t BatchInteriorUnits(int width, int rows, int ys)
+AVIFGPU_HD inline int64_t BatchInteriorUnits(int width, int rows, int ys)
 {
     return static_cast<int64_t>((width + kBatchUnitPixels - 1) / kBatchUnitPixels) * ((rows + ys) >> ys);
 }
-inline int64_t BatchEdgeUnits(int width, int rows, int xs, int ys)
+AVIFGPU_HD inline int64_t BatchEdgeUnits(int width, int rows, int xs, int ys)
 {
     return static_cast<int64_t>((((width + xs) >> xs) + kBatchEdgeThreads - 1) / kBatchEdgeThreads) * ((rows + ys) >> ys);
+}
+
+// The record of a block (an EncodeWindow / DecodeWindow), first unit 0.
+template <typename Params>
+AVIFGPU_HD inline BatchRecord RecordOf(const Params& w)
+{
+    BatchRecord r{};
+    r.rows = w.rows;
+    r.rowStride = w.rowStride;
+    for (int k = 0; k < 4; ++k)
+    {
+        r.plane[k] = const_cast<void*>(static_cast<const void*>(w.plane[k]));
+        r.planeStride[k] = w.planeStride[k];
+    }
+    r.width = w.width;
+    r.rowCount = w.rowCount;
+    return r;
 }
 
 // One chunk: at most two launches -- the batched tuned kernel over every image's interior, then the batched generic

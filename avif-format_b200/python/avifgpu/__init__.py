@@ -72,6 +72,9 @@ def library():
         [ctx_p, C.POINTER(abi.EncodeDesc), C.POINTER(abi.BatchImage), C.c_int32, C.c_void_p])
     sig("avifgpu_decode_batch_device", C.c_int,
         [ctx_p, C.POINTER(abi.DecodeDesc), C.POINTER(abi.BatchImage), C.c_int32, C.c_void_p])
+    sig("avifgpu_batch_workspace_bytes", C.c_int, [C.c_int32, C.POINTER(C.c_size_t)])
+    for name, desc_type in (("avifgpu_encode_batch_indirect", abi.EncodeDesc), ("avifgpu_decode_batch_indirect", abi.DecodeDesc)):
+        sig(name, C.c_int, [ctx_p, C.POINTER(desc_type), C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p])
     sig("avifgpu_transfer_f32", C.c_int, [ctx_p, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_size_t])
     sig("avifgpu_prepare_encode", C.c_int, [ctx_p, C.POINTER(abi.EncodeDesc), C.POINTER(abi.CurveStats)])
     sig("avifgpu_prepare_decode", C.c_int, [ctx_p, C.POINTER(abi.DecodeDesc)])
@@ -130,7 +133,8 @@ EXPORTED_SYMBOLS = [
     "avifgpu_encode_host_col_bytes", "avifgpu_decode_host_col_bytes", "avifgpu_encode_plane_geometry",
     "avifgpu_decode_plane_geometry", "avifgpu_get_yuv_coefficients", "avifgpu_get_hlg_luma_coefficients",
     "avifgpu_build_yuv_tables", "avifgpu_encode_rows", "avifgpu_decode_rows", "avifgpu_encode_rows_device",
-    "avifgpu_decode_rows_device", "avifgpu_encode_batch_device", "avifgpu_decode_batch_device", "avifgpu_transfer_f32", "avifgpu_prepare_encode", "avifgpu_set_table_autobuild",
+    "avifgpu_decode_rows_device", "avifgpu_encode_batch_device", "avifgpu_decode_batch_device",
+    "avifgpu_batch_workspace_bytes", "avifgpu_encode_batch_indirect", "avifgpu_decode_batch_indirect", "avifgpu_transfer_f32", "avifgpu_prepare_encode", "avifgpu_set_table_autobuild",
     "avifgpu_hlg_ootf_f32", "avifgpu_prepare_decode",
     "avifgpu_encode_rows_async", "avifgpu_decode_rows_async", "avifgpu_wait",
     "avifgpu_shard_group_create", "avifgpu_shard_group_destroy", "avifgpu_shard_group_size", "avifgpu_shard_group_context",
@@ -311,6 +315,17 @@ class Context:
         """avifgpu_decode_batch_device: `images` is a ctypes array of abi.BatchImage (planes = source, rows = destination)."""
         self._check(self.lib.avifgpu_decode_batch_device(self.handle, C.byref(desc), images, len(images), stream))
 
+    def encode_batch_indirect(self, desc, images, count, max_count, workspace, status=None, stream=0):
+        """avifgpu_encode_batch_indirect: `images` (records, see pack_batch_images), `count` (one int32), `workspace` and
+        `status` (max_count int32, or None) are CUDA tensors, read when the work runs on `stream`."""
+        self._check(self.lib.avifgpu_encode_batch_indirect(self.handle, C.byref(desc), *_indirect_args(images, count, max_count, workspace, status),
+                                                           stream))
+
+    def decode_batch_indirect(self, desc, images, count, max_count, workspace, status=None, stream=0):
+        """avifgpu_decode_batch_indirect: as encode_batch_indirect (planes = source, rows = destination)."""
+        self._check(self.lib.avifgpu_decode_batch_indirect(self.handle, C.byref(desc), *_indirect_args(images, count, max_count, workspace, status),
+                                                           stream))
+
     def decode_device(self, desc, planes_struct, rows_ptr, row_stride, y0=0, nrows=None, stream=0):
         nrows = desc.height - y0 if nrows is None else nrows
         self._check(self.lib.avifgpu_decode_rows_device(self.handle, C.byref(desc), C.byref(planes_struct), y0, nrows,
@@ -445,3 +460,41 @@ def batch_images_from_tensors(images):
             out[i].row_stride_bytes = rows.stride(0) * rows.element_size()
         out[i].planes = planes_from_tensors(planes)
     return out
+
+
+def batch_workspace_bytes(max_count):
+    """avifgpu_batch_workspace_bytes: the device workspace a device-described batch of up to max_count images needs."""
+    out = C.c_size_t()
+    status = library().avifgpu_batch_workspace_bytes(max_count, C.byref(out))
+    if status != 0:
+        raise AvifGpuError(status, f"avifgpu_batch_workspace_bytes({max_count})")
+    return out.value
+
+
+def pack_batch_images(images, capacity=None, out=None):
+    """The records of batch_images_from_tensors(images) -- or `images` itself when it already is a ctypes array of
+    abi.BatchImage -- as a CUDA uint8 tensor of capacity x sizeof(BatchImage) bytes (records past len(images) zeroed), for
+    the device-described batch calls.  With `out` (such a tensor) the records are written into it instead, in stream
+    order on the current stream."""
+    import torch
+    capacity = len(images) if capacity is None else capacity
+    assert len(images) <= capacity
+    records = images if isinstance(images, C.Array) else batch_images_from_tensors(images)
+    host = (abi.BatchImage * capacity)()
+    C.memmove(host, records, len(images) * C.sizeof(abi.BatchImage))
+    data = torch.frombuffer(bytearray(bytes(host)), dtype=torch.uint8).reshape(capacity, C.sizeof(abi.BatchImage))
+    if out is None:
+        return data.cuda()
+    assert out.dtype == torch.uint8 and out.is_cuda and out.shape == data.shape
+    out.copy_(data)
+    return out
+
+
+def _indirect_args(images, count, max_count, workspace, status):
+    import torch
+    assert images.is_cuda and count.is_cuda and count.dtype == torch.int32 and workspace.is_cuda
+    assert images.numel() >= max_count * C.sizeof(abi.BatchImage)
+    if status is not None:
+        assert status.is_cuda and status.dtype == torch.int32 and status.numel() >= max_count
+    return (images.data_ptr(), count.data_ptr(), max_count, workspace.data_ptr(), workspace.numel() * workspace.element_size(),
+            None if status is None else status.data_ptr())

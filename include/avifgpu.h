@@ -50,7 +50,7 @@ extern "C" {
 #define AVIFGPU_EXPORT __attribute__((visibility("default")))
 #endif
 
-#define AVIFGPU_API_VERSION 6
+#define AVIFGPU_API_VERSION 7
 
 typedef enum avifgpu_status
 {
@@ -382,6 +382,54 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
  * done once per call, outside a capture. */
 AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
                                                const avifgpu_batch_image* images, int32_t count, void* cuda_stream);
+
+/* ---- the hot path: batches described in device memory ---------------------------------------------------------- */
+
+/* Device workspace bytes a device-described batch of up to max_count images needs (1 <= max_count <= 4096).
+ * Pure host arithmetic. */
+AVIFGPU_EXPORT int avifgpu_batch_workspace_bytes(int32_t max_count, size_t* out_bytes);
+
+/*
+ * A batch whose image list and count are device memory, read when the work runs: one CUDA graph captured once converts
+ * a different image set on every replay, and images made by earlier GPU work (a resize, a decoder writing into a pool)
+ * need no copy to the host and no synchronisation.
+ *   - Device inputs.  device_images (max_count avifgpu_batch_image records), *device_count and device_workspace are
+ *     device memory, read on `cuda_stream` when the work runs, not when the call is made: write them earlier on the same
+ *     stream, or in work ordered before it.  desc->width and desc->height are ignored.
+ *   - Host checks, before any launch (each returns its status and launches nothing): ctx, desc, device_images,
+ *     device_count or device_workspace NULL; desc invalid (validated as for the other calls, its size ignored);
+ *     max_count outside [1, 4096]; workspace_bytes below avifgpu_batch_workspace_bytes(max_count).
+ *   - Supported descriptions: encode, 8- or 16-bit RGB(A) hosts into planar YCbCr, any alpha state; decode, 8- or 16-bit
+ *     hosts reading YCbCr with no or straight alpha.  Anything else is AVIFGPU_ERR_UNSUPPORTED, with no launch.
+ *   - Device-side checks.  With n = *device_count: n < 0 or n > max_count converts nothing and sets all max_count
+ *     entries of device_status to AVIFGPU_ERR_BAD_PARAM.  Otherwise image i < n gets device_status[i] = 0, or
+ *     AVIFGPU_ERR_BAD_PARAM when its width or height is negative, or when it is non-empty and its rows or a plane the
+ *     description has is NULL (the host-described calls' checks); a rejected image is skipped and its outputs are not
+ *     touched.  Images of width or height 0 are accepted and write nothing.  device_status may be NULL.
+ *   - Outputs: every accepted image equals one *_rows_device call of the whole image, bit for bit.  The outputs of
+ *     different images must not overlap.
+ *   - Launches: exactly three per call, whatever the batch holds, n = 0 included (plan, interiors, edges);
+ *     avifgpu_launch_count rises by 3.
+ *   - Capture: the call may be captured under the device calls' rules.  The graph holds the description and the
+ *     addresses of the records, count, workspace and status array, not their contents: a replay converts whatever those
+ *     buffers hold at that moment.
+ *   - First-use work: an encode makes the premultiply check outside a capture; call avifgpu_prepare_decode before
+ *     capturing a decode.  An encode captured before the check sends every image through the edge kernel: the same
+ *     output bit for bit, a slower kernel.
+ *   - Workspace: one workspace must not serve two calls that can be in flight at the same time.  The library allocates
+ *     nothing for this call.
+ * Images the tuned integer kernels take in a direct call have their aligned interior converted by the interior kernel,
+ * their right strip and odd last 4:2:0 row by the edge kernel; every other image is one whole-image window of the edge
+ * kernel, which runs the generic kernels' own per-site / per-pixel code.
+ */
+AVIFGPU_EXPORT int avifgpu_encode_batch_indirect(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
+                                                 const avifgpu_batch_image* device_images, const int32_t* device_count,
+                                                 int32_t max_count, void* device_workspace, size_t workspace_bytes,
+                                                 int32_t* device_status, void* cuda_stream);
+AVIFGPU_EXPORT int avifgpu_decode_batch_indirect(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
+                                                 const avifgpu_batch_image* device_images, const int32_t* device_count,
+                                                 int32_t max_count, void* device_workspace, size_t workspace_bytes,
+                                                 int32_t* device_status, void* cuda_stream);
 
 /* ---- the hot path across several GPUs of one box (SURVEY.md 8e) ------------------------------------------------ */
 

@@ -3,7 +3,7 @@
 // converts pixels launches a CUDA kernel or fails.
 #include "../../include/avifgpu.h"
 
-#include "batch_indirect.h"
+#include "batch_plan.h"
 #include "curve_tables.h"
 #include "host_params.h"
 #include "kernel_params.h"
@@ -927,13 +927,14 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
     {
         return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL description or image array");
     }
-    // every image is validated before anything is enqueued
-    std::vector<EncodeParams> params(static_cast<size_t>(count));
+    // every image is validated before anything is enqueued: the description at the image's size, then its buffers
+    avifgpu_encode_desc d = *desc;
+    EncodeParams shared;
+    int planeMask = 0;
     int64_t pixels = 0;
     for (int32_t i = 0; i < count; ++i)
     {
         const avifgpu_batch_image& image = images[i];
-        avifgpu_encode_desc d = *desc;
         d.width = image.width;
         d.height = image.height;
         std::string error;
@@ -942,35 +943,20 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
         {
             return ctx->Fail(status, "image " + std::to_string(i) + ": " + error);
         }
-        EncodeParams& p = params[i];
-        FillEncodeParams(d, &p);
-        if (d.width == 0 || d.height == 0)
+        if (i == 0)
         {
-            p.width = 0;
-            p.rowCount = 0;
-            continue;
-        }
-        if (image.rows == nullptr)
-        {
-            return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "image " + std::to_string(i) + ": NULL rows");
-        }
-        p.rows = image.rows;
-        p.rowStride = image.row_stride_bytes;
-        p.rowCount = d.height;
-        for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
-        {
-            if (!EncodePlaneGeometry(d, k).present)
+            FillEncodeParams(d, &shared);
+            for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
             {
-                continue;
+                planeMask |= EncodePlaneGeometry(d, k).present ? 1 << k : 0;
             }
-            if (image.planes.data[k] == nullptr)
-            {
-                return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "image " + std::to_string(i) + ": missing destination plane");
-            }
-            p.plane[k] = image.planes.data[k];
-            p.planeStride[k] = image.planes.stride[k];
         }
-        pixels += static_cast<int64_t>(d.width) * d.height;
+        EncodeParams p = shared;
+        if (AdoptBatchImage(p, planeMask, image) != AVIFGPU_OK)
+        {
+            return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "image " + std::to_string(i) + (image.rows == nullptr ? ": NULL rows" : ": missing destination plane"));
+        }
+        pixels += static_cast<int64_t>(image.width) * image.height;
     }
     if (pixels == 0)
     {
@@ -983,21 +969,13 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
     {
         return status;
     }
-    EncodeParams firstUse;
-    FillEncodeParams(*desc, &firstUse);
-    ctx->FirstUseEncode(*desc, pixels, capturing, &firstUse);
-    for (EncodeParams& p : params)
-    {
-        p.smCount = ctx->smCount;
-        p.curveTable = firstUse.curveTable;
-        p.gray16Lut = firstUse.gray16Lut;
-        p.verifiedPremultiply = firstUse.verifiedPremultiply;
-    }
+    shared.smCount = ctx->smCount;
+    ctx->FirstUseEncode(*desc, pixels, capturing, &shared);
     BatchPlan plan;
-    PlanEncodeBatch(params, desc->host_depth, &plan);
+    PlanEncodeBatch(shared, desc->host_depth, planeMask, images, count, &plan);
     for (const BatchChunk& chunk : plan.chunks)
     {
-        const int launched = LaunchEncodeBatchChunk(params[chunk.imageIndex[0]], desc->host_depth, chunk, cuda_stream);
+        const int launched = LaunchEncodeBatchChunk(shared, desc->host_depth, chunk, cuda_stream);
         if (launched < 0)
         {
             return ctx->LaunchFailed(launched, "batched encode kernel launch", capturing);
@@ -1006,7 +984,9 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
     }
     for (const int32_t i : plan.fallback)
     {
-        const int launched = LaunchEncode(params[i], desc->host_depth, cuda_stream);
+        EncodeParams p = shared;
+        AdoptBatchImage(p, planeMask, images[i]);
+        const int launched = LaunchEncode(p, desc->host_depth, cuda_stream);
         if (launched < 0)
         {
             return ctx->LaunchFailed(launched, "encode kernel launch", capturing);
@@ -1027,14 +1007,15 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifg
     {
         return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL description or image array");
     }
-    // every image is validated before anything is enqueued
-    std::vector<DecodeParams> params(static_cast<size_t>(count));
+    // every image is validated before anything is enqueued: the description at the image's size, then its buffers
+    avifgpu_decode_desc d = *desc;
+    DecodeParams shared;
     int32_t transfer = 0;
+    int planeMask = 0;
     int64_t pixels = 0;
     for (int32_t i = 0; i < count; ++i)
     {
         const avifgpu_batch_image& image = images[i];
-        avifgpu_decode_desc d = *desc;
         d.width = image.width;
         d.height = image.height;
         std::string error;
@@ -1043,39 +1024,23 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifg
         {
             return ctx->Fail(status, "image " + std::to_string(i) + ": " + error);
         }
-        DecodeParams& p = params[i];
-        if (!FillDecodeParams(d, transfer, &p, &error))
+        if (i == 0)
         {
-            return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "image " + std::to_string(i) + ": " + error);
-        }
-        if (d.width == 0 || d.height == 0)
-        {
-            p.width = 0;
-            p.rowCount = 0;
-            continue;
-        }
-        if (image.rows == nullptr)
-        {
-            return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "image " + std::to_string(i) + ": NULL rows");
-        }
-        p.rows = image.rows;
-        p.rowStride = image.row_stride_bytes;
-        p.rowCount = d.height;
-        p.yPhase = 0;
-        for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
-        {
-            if (!DecodePlaneGeometry(d, k).present)
+            if (!FillDecodeParams(d, transfer, &shared, &error))
             {
-                continue;
+                return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "image 0: " + error);
             }
-            if (image.planes.data[k] == nullptr)
+            for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
             {
-                return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "image " + std::to_string(i) + ": missing source plane");
+                planeMask |= DecodePlaneGeometry(d, k).present ? 1 << k : 0;
             }
-            p.plane[k] = image.planes.data[k];
-            p.planeStride[k] = image.planes.stride[k];
         }
-        pixels += static_cast<int64_t>(d.width) * d.height;
+        DecodeParams p = shared;
+        if (AdoptBatchImage(p, planeMask, image) != AVIFGPU_OK)
+        {
+            return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "image " + std::to_string(i) + (image.rows == nullptr ? ": NULL rows" : ": missing source plane"));
+        }
+        pixels += static_cast<int64_t>(image.width) * image.height;
     }
     if (pixels == 0)
     {
@@ -1088,20 +1053,13 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifg
     {
         return status;
     }
-    DecodeParams firstUse = params[0];
-    ctx->FirstUseDecode(*desc, transfer, capturing, &firstUse);
-    for (DecodeParams& p : params)
-    {
-        p.smCount = ctx->smCount;
-        p.verifiedHlgDivisions = firstUse.verifiedHlgDivisions;
-        p.verifiedGreenDivision = firstUse.verifiedGreenDivision;
-        p.verifiedPqRatio = firstUse.verifiedPqRatio;
-    }
+    shared.smCount = ctx->smCount;
+    ctx->FirstUseDecode(*desc, transfer, capturing, &shared);
     BatchPlan plan;
-    PlanDecodeBatch(params, &plan);
+    PlanDecodeBatch(shared, planeMask, images, count, &plan);
     for (const BatchChunk& chunk : plan.chunks)
     {
-        const int launched = LaunchDecodeBatchChunk(params[chunk.imageIndex[0]], chunk, cuda_stream);
+        const int launched = LaunchDecodeBatchChunk(shared, chunk, cuda_stream);
         if (launched < 0)
         {
             return ctx->LaunchFailed(launched, "batched decode kernel launch", capturing);
@@ -1110,7 +1068,9 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifg
     }
     for (const int32_t i : plan.fallback)
     {
-        const int launched = LaunchDecode(params[i], cuda_stream);
+        DecodeParams p = shared;
+        AdoptBatchImage(p, planeMask, images[i]);
+        const int launched = LaunchDecode(p, cuda_stream);
         if (launched < 0)
         {
             return ctx->LaunchFailed(launched, "decode kernel launch", capturing);

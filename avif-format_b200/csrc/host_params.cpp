@@ -3,6 +3,8 @@
 // reference's do.
 #include "host_params.h"
 
+#include "batch_plan.h"
+
 #include <cstring>
 
 namespace avifgpu
@@ -469,65 +471,57 @@ Interior DecodeYccIntInterior(const DecodeParams& p)
 
 namespace
 {
-// Both directions: `interiorOf` is the single-image predicate, `windowOf(p, x0, y0, width, rows)` the launchers' window
-// and `edgeUnits(p, width, rows)` the units of one.
-template <typename Params, typename InteriorOf, typename WindowOf, typename EdgeUnits>
-void PlanBatch(const std::vector<Params>& images, BatchPlan* plan, InteriorOf interiorOf, WindowOf windowOf, EdgeUnits edgeUnits)
+// Adds image i's plan to `plan`: its interior and windows to the last chunk (a new one when that is full), or the image to
+// the direct calls when it is non-empty and has no interior.
+void AddToBatch(const BatchImagePlan& image, int32_t i, BatchPlan* plan)
 {
-    plan->chunks.clear();
-    plan->fallback.clear();
-    for (int32_t i = 0; i < static_cast<int32_t>(images.size()); ++i)
+    if (image.interior.width == 0)
     {
-        const Params& p = images[i];
-        if (p.width <= 0 || p.rowCount <= 0)
-        {
-            continue;
-        }
-        const Interior inner = interiorOf(p);
-        if (inner.width == 0)
+        if (image.windows > 0)
         {
             plan->fallback.push_back(i);
-            continue;
         }
-        if (plan->chunks.empty() || plan->chunks.back().images == kBatchChunkImages)
-        {
-            plan->chunks.emplace_back();
-        }
-        BatchChunk& c = plan->chunks.back();
-        BatchRecord& r = c.interior[c.images];
-        r = RecordOf(windowOf(p, 0, 0, inner.width, inner.rows));
-        r.firstUnit = c.interiorUnits;
-        c.interiorUnits += BatchInteriorUnits(inner.width, inner.rows, p.ys);
-        c.imageIndex[c.images++] = i;
-        Strip strip[2];
-        const int strips = InteriorStrips(p.width, p.rowCount, inner, strip);
-        for (int k = 0; k < strips; ++k)
-        {
-            BatchRecord& w = c.window[c.windows];
-            w = RecordOf(windowOf(p, strip[k].x0, strip[k].y0, strip[k].width, strip[k].rows));
-            w.firstUnit = c.windowUnits;
-            c.windowUnits += edgeUnits(p, strip[k].width, strip[k].rows);
-            c.windowImage[c.windows++] = i;
-        }
+        return;
+    }
+    if (plan->chunks.empty() || plan->chunks.back().images == kBatchChunkImages)
+    {
+        plan->chunks.emplace_back();
+    }
+    BatchChunk& c = plan->chunks.back();
+    c.interior[c.images] = image.interior;
+    c.interior[c.images].firstUnit = c.interiorUnits;
+    c.interiorUnits += image.interiorUnits;
+    c.imageIndex[c.images++] = i;
+    for (int k = 0; k < image.windows; ++k)
+    {
+        c.window[c.windows] = image.window[k];
+        c.window[c.windows].firstUnit = c.windowUnits;
+        c.windowUnits += image.windowUnits[k];
+        c.windowImage[c.windows++] = i;
     }
 }
 } // namespace
 
-void PlanEncodeBatch(const std::vector<EncodeParams>& images, int hostDepth, BatchPlan* plan)
+void PlanEncodeBatch(const EncodeParams& shared, int hostDepth, int planeMask, const avifgpu_batch_image* images, int32_t count, BatchPlan* plan)
 {
-    PlanBatch(
-        images, plan, [&](const EncodeParams& p) { return EncodeRgbIntInterior(p, hostDepth); },
-        [&](const EncodeParams& p, int x0, int y0, int width, int rows) { return EncodeWindow(p, hostDepth, x0, y0, width, rows); },
-        [](const EncodeParams& p, int width, int rows) { return BatchEdgeUnits(width, rows, p.xs, p.ys); });
+    plan->chunks.clear();
+    plan->fallback.clear();
+    const bool tuned = EncodeRgbIntTuned(shared, hostDepth);
+    for (int32_t i = 0; i < count; ++i)
+    {
+        AddToBatch(PlanBatchEncodeImage(shared, hostDepth, tuned, planeMask, images[i]), i, plan);
+    }
 }
 
-// An image starts at row 0 and its bottom window at an even row, so every decode window has yPhase 0.
-void PlanDecodeBatch(const std::vector<DecodeParams>& images, BatchPlan* plan)
+void PlanDecodeBatch(const DecodeParams& shared, int planeMask, const avifgpu_batch_image* images, int32_t count, BatchPlan* plan)
 {
-    PlanBatch(
-        images, plan, [](const DecodeParams& p) { return DecodeYccIntInterior(p); },
-        [](const DecodeParams& p, int x0, int y0, int width, int rows) { return DecodeWindow(p, x0, y0, width, rows); },
-        [](const DecodeParams&, int width, int rows) { return BatchEdgeUnits(width, rows, 0, 0); }); // one thread per pixel
+    plan->chunks.clear();
+    plan->fallback.clear();
+    const bool tuned = DecodeYccIntTuned(shared);
+    for (int32_t i = 0; i < count; ++i)
+    {
+        AddToBatch(PlanBatchDecodeImage(shared, tuned, planeMask, images[i]), i, plan);
+    }
 }
 
 } // namespace avifgpu

@@ -415,6 +415,7 @@ __device__ __forceinline__ void EncodeRgbIntGroup(const Rgb16Params& p, const fl
 // ---- planar YCbCr -> RGB(A) 8/16-bit hosts -------------------------------------------------------------------------
 
 constexpr int kUnitPixels = 256; // per row: 32 lanes x 8 pixels
+constexpr int kYccBlocksPerSm = 3; // DecodeYccToRgbIntKernel's and its batched forms' occupancy, and their grid caps per SM
 
 struct IntDecodeParams
 {
@@ -430,6 +431,26 @@ struct IntDecodeParams
     InverseMatrix matrix;
     int32_t verifiedGreenDivision;
 };
+
+// The fields every unit of `p`'s image shares; the launchers add pointers, strides and sizes.
+inline IntDecodeParams IntDecodeShared(const DecodeParams& p)
+{
+    IntDecodeParams fp{};
+    fp.bitDepth = p.bitDepth;
+    fp.maxCode = p.maxCode;
+    fp.range = p.range;
+    fp.matrix = p.matrix;
+    fp.verifiedGreenDivision = p.verifiedGreenDivision;
+    return fp;
+}
+
+// The dynamic shared memory StageYccTables fills: the Y and UV tables, plus the alpha table of 16-bit hosts with alpha.
+// At most 40 KB, under the default 48 KB limit.
+inline size_t YccTableBytes(int bitDepth, bool alphaTable)
+{
+    const size_t entries = static_cast<size_t>(1) << bitDepth;
+    return 2 * sizeof(float) * entries + (alphaTable ? sizeof(uint16_t) * entries : 0);
+}
 
 // Eight (four) consecutive samples of a plane as they sit in memory, and their expansion into 32-bit codes.
 template <typename SampleT>

@@ -18,8 +18,8 @@
 #include "curve_tables.h"
 #include "pixel_math.cuh"
 
-// The routing and window arithmetic below is plain C++ that the plan kernel of the device-described batch calls
-// (kernels_batch_indirect.cu) runs on the device too; the attribute is empty for the host compiler (host_params.cpp,
+// The routing and window arithmetic below is plain C++ that the plan kernel of the device-described batch
+// (kernels_batch.cu) runs on the device too; the attribute is empty for the host compiler (host_params.cpp,
 // tests/native).
 #if defined(__CUDACC__)
 #define AVIFGPU_HD __host__ __device__
@@ -344,12 +344,6 @@ struct BatchPlan
     std::vector<int32_t> fallback; // positions of the images that take one direct call each (LaunchEncode), in order
 };
 
-// Splits whole-image blocks (one EncodeParams per image; images with no pixels are skipped) into chunks of the images
-// EncodeRgbIntInterior takes, in order, and direct calls for the rest.
-void PlanEncodeBatch(const std::vector<EncodeParams>& images, int hostDepth, BatchPlan* plan);
-// The same for decode blocks, with DecodeYccIntInterior.
-void PlanDecodeBatch(const std::vector<DecodeParams>& images, BatchPlan* plan);
-
 // Launches of one chunk: 1 + (1 when it has edge windows).
 inline int BatchChunkLaunches(const BatchChunk& chunk) { return 1 + (chunk.windows > 0 ? 1 : 0); }
 
@@ -381,8 +375,8 @@ int LaunchHlgOotf(int inverse, const float luma[3], float displayGamma, float pe
 int CompleteEncode(cudaError_t tuned, const EncodeParams& p, int hostDepth, int coveredWidth, int coveredRows, void* stream);
 int CompleteDecode(cudaError_t tuned, const DecodeParams& p, int coveredWidth, int coveredRows, void* stream);
 
-// The launches of one planned chunk (kernels_batch.cu); `shared` is the block of any of its images (every field but
-// the pointers, strides and sizes is the same for all of them).  Returns BatchChunkLaunches(chunk) or a negative status.
+// The launches of one planned chunk (PlanEncodeBatch / PlanDecodeBatch, batch_plan.h; kernels_batch.cu); `shared` is the
+// description's block (its pointers, strides and sizes are unused).  Returns BatchChunkLaunches(chunk) or a negative status.
 int LaunchEncodeBatchChunk(const EncodeParams& shared, int hostDepth, const BatchChunk& chunk, void* stream);
 int LaunchDecodeBatchChunk(const DecodeParams& shared, const BatchChunk& chunk, void* stream);
 

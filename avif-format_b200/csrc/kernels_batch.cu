@@ -1,18 +1,27 @@
-// kernels_batch.cu -- many small images per launch for avifgpu_encode_batch_device and avifgpu_decode_batch_device.
-// A 512 x 512 image is 2 MB of traffic, well under a microsecond of HBM time, so one launch per image is bound by the launch and the grid's ramp and
-// drain.  Here one launch walks the units of every image of a chunk:
+// kernels_batch.cu -- many small images per launch, for both batch APIs.  A 512 x 512 image is 2 MB of traffic, well
+// under a microsecond of HBM time, so one launch per image is bound by the launch and the grid's ramp and drain.  Here
+// one launch walks the units of every image of a batch:
 //
-//   EncodeRgbIntBatchKernel    the aligned interiors, with EncodeRgbIntGroup (int_units.cuh) -- the single-image tuned
-//                              kernel's own group code; a warp takes one unit (256 pixels of one row or 4:2:0 row pair,
-//                              8 per lane) at a time, persistent over the chunk's concatenated unit space;
-//   EncodePlanarBatchKernel    the right strips and odd last 4:2:0 rows, with EncodePlanarSite (generic_units.cuh) -- the
-//                              generic kernel's own site code; a CTA takes one run of 256 chroma sites at a time;
+//   EncodeRgbIntBatchKernel       the aligned interiors, with EncodeRgbIntGroup (int_units.cuh) -- the single-image
+//                                 tuned kernel's own group code; a warp takes one unit (256 pixels of one row or 4:2:0 row
+//                                 pair, 8 per lane) at a time, persistent over the concatenated unit space;
+//   EncodePlanarBatchKernel       the windows -- right strips, odd last 4:2:0 rows, and whole images the tuned kernel does
+//                                 not take -- with EncodePlanarSite (generic_units.cuh), the generic kernel's own site
+//                                 code; a CTA takes one run of 256 chroma sites at a time;
 //   DecodeYccToRgbIntBatchKernel  the decode interiors, with LoadYccUnit / ExpandYccUnit / StoreYccUnit (int_units.cuh);
-//                              the unorm -> float tables are staged once per CTA for the whole chunk (one description);
-//   DecodeBatchKernel          the decode edge strips, with DecodeChunkPixel (generic_units.cuh).
+//                                 the unorm -> float tables are staged once per CTA for the whole batch (one description);
+//   DecodeBatchKernel             the decode windows, with DecodeChunkPixel (generic_units.cuh).
 //
-// A worker's units increase, so it finds each unit's record by walking forward through the records' first units: once per
-// unit and warp- (CTA-) uniform, never per pixel.  The per-image records travel in the kernel parameter (__grid_constant__).
+// Each is a template on where its records come from:
+//   ChunkSource      a host-described chunk (PlanEncodeBatch / PlanDecodeBatch): the records and their unit total travel
+//                    in the kernel parameter (__grid_constant__) and the grid is sized to the units.  A worker's units
+//                    increase, so it finds each unit's record by walking forward through the records' first units.
+//   WorkspaceSource  a device-described batch: PlanIndirectKernel writes the records, their first units and the totals
+//                    into the workspace when the work runs.  The host does not know how much work there is, so the grid
+//                    is the chunk launchers' cap and a CTA with no unit returns before it stages anything; a worker finds
+//                    its unit's record with a binary search (FindRecord), starting after the record of its previous unit.
+// Either way the search is once per unit and warp- (CTA-) uniform, never per pixel.
+#include "batch_plan.h"
 #include "generic_units.cuh"
 #include "int_units.cuh"
 #include "kernel_params.h"
@@ -27,45 +36,7 @@ namespace
 {
 
 constexpr int kWarps = kRgbThreads / 32;
-
-struct RgbIntBatchParams
-{
-    Rgb16Params shared; // pointers, strides and sizes unused
-    int32_t count;
-    int64_t units;
-    BatchRecord image[kBatchChunkImages];
-};
-
-struct PlanarBatchParams
-{
-    EncodeParams shared; // pointers, strides and sizes unused
-    int32_t count;
-    int64_t units;
-    BatchRecord window[2 * kBatchChunkImages];
-};
-
-constexpr int kDecodeBlocksPerSm = 3; // DecodeYccToRgbIntKernel's occupancy (kernels_fast_decode_int.cu)
-
-struct YccIntBatchParams
-{
-    IntDecodeParams shared; // pointers, strides and sizes unused
-    int32_t count;
-    int64_t units;
-    BatchRecord image[kBatchChunkImages];
-};
-
-struct DecodeEdgeBatchParams
-{
-    DecodeParams shared; // pointers, strides and sizes unused
-    int32_t count;
-    int64_t units;
-    BatchRecord window[2 * kBatchChunkImages];
-};
-
-// CUDA 12.1+ on Volta and later: at most 32764 bytes of kernel parameters.
-static_assert(sizeof(RgbIntBatchParams) <= 32764 && sizeof(PlanarBatchParams) <= 32764 && sizeof(YccIntBatchParams) <= 32764 &&
-                  sizeof(DecodeEdgeBatchParams) <= 32764,
-              "a chunk must fit one kernel parameter block");
+constexpr int kPlanThreads = 1024;
 
 // The record that owns `unit`, walking forward from `record` (units only increase along a worker's walk).
 template <int N>
@@ -78,19 +49,240 @@ __device__ __forceinline__ int RecordOfUnit(const BatchRecord (&records)[N], int
     return record;
 }
 
-template <typename HostT, typename PlaneT, int CHANNELS, int XS, int YS, int PREMULTIPLY>
-__global__ void __launch_bounds__(kRgbThreads) EncodeRgbIntBatchKernel(const __grid_constant__ RgbIntBatchParams b)
+// The records of one host-described chunk, by value.  `shared` carries the description (its pointers, strides and sizes
+// are unused); N is kBatchChunkImages interiors or twice as many windows.
+template <typename Shared, int N>
+struct ChunkSource
 {
+    Shared shared;
+    int32_t count;
+    int64_t units;
+    BatchRecord record[N];
+
+    struct Walk
+    {
+        const ChunkSource& s;
+        __device__ __forceinline__ explicit Walk(const ChunkSource& source) : s(source) {}
+        __device__ __forceinline__ long long Units() const { return s.units; }
+        __device__ __forceinline__ bool Idle(long long) const { return false; } // the grid is sized to the units
+        __device__ __forceinline__ int Count() const { return s.count; }
+        __device__ __forceinline__ int Find(int, int record, long long unit) const { return RecordOfUnit(s.record, s.count, record, unit); }
+        __device__ __forceinline__ const BatchRecord& Record(int record) const { return s.record[record]; }
+    };
+};
+
+// The workspace seen by the kernels.
+struct IndirectView
+{
+    IndirectHeader* header;
+    int64_t* interiorFirst;
+    int64_t* windowFirst;
+    BatchRecord* interior;
+    BatchRecord* window;
+
+    __device__ __forceinline__ IndirectView(void* workspace, int maxCount)
+    {
+        uint8_t* base = static_cast<uint8_t*>(workspace);
+        const IndirectLayout l = IndirectWorkspaceLayout(maxCount);
+        header = reinterpret_cast<IndirectHeader*>(base);
+        interiorFirst = reinterpret_cast<int64_t*>(base + l.interiorFirst);
+        windowFirst = reinterpret_cast<int64_t*>(base + l.windowFirst);
+        interior = reinterpret_cast<BatchRecord*>(base + l.interior);
+        window = reinterpret_cast<BatchRecord*>(base + l.window);
+    }
+};
+
+// The interior (WINDOWS = 0) or window records of a device-described batch, in its workspace.
+template <typename Shared, int WINDOWS>
+struct WorkspaceSource
+{
+    Shared shared;
+    void* workspace;
+    int32_t maxCount;
+
+    struct Walk
+    {
+        IndirectView w;
+        long long units;
+        __device__ __forceinline__ explicit Walk(const WorkspaceSource& source)
+            : w(source.workspace, source.maxCount), units(WINDOWS ? w.header->windowUnits : w.header->interiorUnits)
+        {
+        }
+        __device__ __forceinline__ long long Units() const { return units; }
+        __device__ __forceinline__ bool Idle(long long firstUnit) const { return firstUnit >= units; } // no unit for this CTA
+        __device__ __forceinline__ int Count() const { return WINDOWS ? 2 * w.header->count : w.header->count; }
+        __device__ __forceinline__ int Find(int count, int record, long long unit) const
+        {
+            return FindRecord(WINDOWS ? w.windowFirst : w.interiorFirst, count, record, unit);
+        }
+        __device__ __forceinline__ const BatchRecord& Record(int record) const { return (WINDOWS ? w.window : w.interior)[record]; }
+    };
+};
+
+using RgbIntChunk = ChunkSource<Rgb16Params, kBatchChunkImages>;
+using PlanarChunk = ChunkSource<EncodeParams, 2 * kBatchChunkImages>;
+using YccIntChunk = ChunkSource<IntDecodeParams, kBatchChunkImages>;
+using DecodeEdgeChunk = ChunkSource<DecodeParams, 2 * kBatchChunkImages>;
+
+// CUDA 12.1+ on Volta and later: at most 32764 bytes of kernel parameters.
+static_assert(sizeof(RgbIntChunk) <= 32764 && sizeof(PlanarChunk) <= 32764 && sizeof(YccIntChunk) <= 32764 && sizeof(DecodeEdgeChunk) <= 32764,
+              "a chunk must fit one kernel parameter block");
+
+// Block-wide exclusive scan of a pair of counts over kPlanThreads threads; every thread gets the block's totals too.
+__device__ __forceinline__ void ScanPair(long long a, long long b, long long& beforeA, long long& beforeB, long long& totalA, long long& totalB)
+{
+    __shared__ long long warpA[kPlanThreads / 32], warpB[kPlanThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    long long sumA = a, sumB = b;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1)
+    {
+        const long long upA = __shfl_up_sync(0xffffffffu, sumA, d);
+        const long long upB = __shfl_up_sync(0xffffffffu, sumB, d);
+        if (lane >= d)
+        {
+            sumA += upA;
+            sumB += upB;
+        }
+    }
+    if (lane == 31)
+    {
+        warpA[warp] = sumA;
+        warpB[warp] = sumB;
+    }
+    __syncthreads();
+    if (warp == 0)
+    {
+        long long wA = warpA[lane], wB = warpB[lane]; // kPlanThreads / 32 == 32 warps
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1)
+        {
+            const long long upA = __shfl_up_sync(0xffffffffu, wA, d);
+            const long long upB = __shfl_up_sync(0xffffffffu, wB, d);
+            if (lane >= d)
+            {
+                wA += upA;
+                wB += upB;
+            }
+        }
+        warpA[lane] = wA;
+        warpB[lane] = wB;
+    }
+    __syncthreads();
+    beforeA = (warp ? warpA[warp - 1] : 0) + sumA - a;
+    beforeB = (warp ? warpB[warp - 1] : 0) + sumB - b;
+    totalA = warpA[kPlanThreads / 32 - 1];
+    totalB = warpB[kPlanThreads / 32 - 1];
+    __syncthreads(); // the next tile rewrites warpA / warpB
+}
+static_assert(kPlanThreads == 32 * 32, "ScanPair scans one value per warp in one warp");
+
+struct EncodePlanner
+{
+    EncodeParams shared;
+    int32_t hostDepth;
+    int32_t tuned;
+    int32_t planeMask;
+    __device__ __forceinline__ BatchImagePlan operator()(const avifgpu_batch_image& image) const
+    {
+        return PlanBatchEncodeImage(shared, hostDepth, tuned != 0, planeMask, image);
+    }
+};
+
+struct DecodePlanner
+{
+    DecodeParams shared;
+    int32_t tuned;
+    int32_t planeMask;
+    __device__ __forceinline__ BatchImagePlan operator()(const avifgpu_batch_image& image) const
+    {
+        return PlanBatchDecodeImage(shared, tuned != 0, planeMask, image);
+    }
+};
+
+// Tiles of kPlanThreads images; the running sums carry across tiles.
+template <typename Planner>
+__global__ void __launch_bounds__(kPlanThreads) PlanIndirectKernel(const __grid_constant__ Planner planner, const avifgpu_batch_image* __restrict__ images,
+                                                                   const int32_t* __restrict__ countPointer, int maxCount, void* workspace,
+                                                                   int32_t* __restrict__ status)
+{
+    const IndirectView w(workspace, maxCount);
+    const int n = *countPointer;
+    if (n < 0 || n > maxCount)
+    {
+        for (int i = threadIdx.x; status != nullptr && i < maxCount; i += blockDim.x)
+        {
+            status[i] = AVIFGPU_ERR_BAD_PARAM;
+        }
+        if (threadIdx.x == 0)
+        {
+            *w.header = IndirectHeader{ 0, 0, 0, 0 };
+        }
+        return;
+    }
+    long long interiorCarry = 0, windowCarry = 0;
+    for (int base = 0; base < n; base += kPlanThreads)
+    {
+        const int i = base + static_cast<int>(threadIdx.x);
+        long long interiorUnits = 0, windowUnits[2] = { 0, 0 };
+        if (i < n)
+        {
+            // the records go out now, their first units after the scan: only the unit counts stay in registers
+            const BatchImagePlan plan = planner(images[i]);
+            if (status != nullptr)
+            {
+                status[i] = plan.status;
+            }
+            w.interior[i] = plan.interior;
+            w.window[2 * i] = plan.window[0];
+            w.window[2 * i + 1] = plan.window[1];
+            interiorUnits = plan.interiorUnits;
+            windowUnits[0] = plan.windowUnits[0];
+            windowUnits[1] = plan.windowUnits[1];
+        }
+        long long interiorBefore, windowBefore, interiorTotal, windowTotal;
+        ScanPair(interiorUnits, windowUnits[0] + windowUnits[1], interiorBefore, windowBefore, interiorTotal, windowTotal);
+        if (i < n)
+        {
+            const long long first = interiorCarry + interiorBefore;
+            w.interiorFirst[i] = first;
+            w.interior[i].firstUnit = first;
+            long long windowFirst = windowCarry + windowBefore;
+            for (int k = 0; k < 2; ++k)
+            {
+                w.windowFirst[2 * i + k] = windowFirst;
+                w.window[2 * i + k].firstUnit = windowFirst;
+                windowFirst += windowUnits[k];
+            }
+        }
+        interiorCarry += interiorTotal;
+        windowCarry += windowTotal;
+    }
+    if (threadIdx.x == 0)
+    {
+        *w.header = IndirectHeader{ interiorCarry, windowCarry, n, 0 };
+    }
+}
+
+template <typename Source, typename HostT, typename PlaneT, int CHANNELS, int XS, int YS, int PREMULTIPLY>
+__global__ void __launch_bounds__(kRgbThreads) EncodeRgbIntBatchKernel(const __grid_constant__ Source s)
+{
+    const typename Source::Walk walk(s);
+    if (walk.Idle(static_cast<long long>(blockIdx.x) * kWarps))
+    {
+        return;
+    }
+    const int count = walk.Count();
     __shared__ float hostLut[(sizeof(HostT) == 1 && sizeof(PlaneT) == 2) ? 256 : 1];
-    StageHostLut<HostT, PlaneT>(hostLut, b.shared.maxCode);
+    StageHostLut<HostT, PlaneT>(hostLut, s.shared.maxCode);
     const int lane = threadIdx.x & 31;
     const long long warpCount = static_cast<long long>(gridDim.x) * kWarps;
     int record = 0;
-    for (long long unit = static_cast<long long>(blockIdx.x) * kWarps + (threadIdx.x >> 5); unit < b.units; unit += warpCount)
+    for (long long unit = static_cast<long long>(blockIdx.x) * kWarps + (threadIdx.x >> 5); unit < walk.Units(); unit += warpCount)
     {
-        record = RecordOfUnit(b.image, b.count, record, unit);
-        const BatchRecord& r = b.image[record];
-        Rgb16Params p = b.shared;
+        record = walk.Find(count, record, unit);
+        const BatchRecord& r = walk.Record(record);
+        Rgb16Params p = s.shared;
         p.rows = static_cast<const uint8_t*>(r.rows);
         p.rowStride = r.rowStride;
         for (int k = 0; k < 4; ++k)
@@ -111,18 +303,24 @@ __global__ void __launch_bounds__(kRgbThreads) EncodeRgbIntBatchKernel(const __g
     }
 }
 
-template <typename HostT>
-__global__ void __launch_bounds__(kBatchEdgeThreads) EncodePlanarBatchKernel(const __grid_constant__ PlanarBatchParams b)
+template <typename Source, typename HostT>
+__global__ void __launch_bounds__(kBatchEdgeThreads) EncodePlanarBatchKernel(const __grid_constant__ Source s)
 {
+    const typename Source::Walk walk(s);
+    if (walk.Idle(blockIdx.x))
+    {
+        return;
+    }
+    const int count = walk.Count();
     __shared__ uint64_t libmStorage[96];
     const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
     __syncthreads();
     int record = 0;
-    for (long long unit = blockIdx.x; unit < b.units; unit += gridDim.x)
+    for (long long unit = blockIdx.x; unit < walk.Units(); unit += gridDim.x)
     {
-        record = RecordOfUnit(b.window, b.count, record, unit);
-        const BatchRecord& r = b.window[record];
-        EncodeParams p = b.shared;
+        record = walk.Find(count, record, unit);
+        const BatchRecord& r = walk.Record(record);
+        EncodeParams p = s.shared;
         p.rows = r.rows;
         p.rowStride = r.rowStride;
         for (int k = 0; k < 4; ++k)
@@ -136,22 +334,28 @@ __global__ void __launch_bounds__(kBatchEdgeThreads) EncodePlanarBatchKernel(con
     }
 }
 
-template <typename SampleT, int XS, int YS, int ALPHA>
-__global__ void __launch_bounds__(kRgbThreads, kDecodeBlocksPerSm) DecodeYccToRgbIntBatchKernel(const __grid_constant__ YccIntBatchParams b)
+template <typename Source, typename SampleT, int XS, int YS, int ALPHA>
+__global__ void __launch_bounds__(kRgbThreads, kYccBlocksPerSm) DecodeYccToRgbIntBatchKernel(const __grid_constant__ Source s)
 {
+    const typename Source::Walk walk(s);
+    if (walk.Idle(static_cast<long long>(blockIdx.x) * kWarps))
+    {
+        return;
+    }
+    const int count = walk.Count();
     constexpr int kRows = YS ? 2 : 1;
     extern __shared__ __align__(16) uint8_t sharedBytes[];
-    const YccTables tables = StageYccTables<SampleT, ALPHA>(sharedBytes, b.shared);
+    const YccTables tables = StageYccTables<SampleT, ALPHA>(sharedBytes, s.shared);
     __syncthreads();
-    const YccFactors factors = MakeYccFactors<SampleT>(b.shared.matrix);
+    const YccFactors factors = MakeYccFactors<SampleT>(s.shared.matrix);
     const int lane = threadIdx.x & 31;
     const long long warpCount = static_cast<long long>(gridDim.x) * kWarps;
     int record = 0;
-    for (long long unit = static_cast<long long>(blockIdx.x) * kWarps + (threadIdx.x >> 5); unit < b.units; unit += warpCount)
+    for (long long unit = static_cast<long long>(blockIdx.x) * kWarps + (threadIdx.x >> 5); unit < walk.Units(); unit += warpCount)
     {
-        record = RecordOfUnit(b.image, b.count, record, unit);
-        const BatchRecord& r = b.image[record];
-        IntDecodeParams p = b.shared;
+        record = walk.Find(count, record, unit);
+        const BatchRecord& r = walk.Record(record);
+        IntDecodeParams p = s.shared;
         for (int k = 0; k < 4; ++k)
         {
             p.plane[k] = static_cast<const uint8_t*>(r.plane[k]);
@@ -178,18 +382,24 @@ __global__ void __launch_bounds__(kRgbThreads, kDecodeBlocksPerSm) DecodeYccToRg
     }
 }
 
-template <typename PlaneT, typename HostT>
-__global__ void __launch_bounds__(kBatchEdgeThreads) DecodeBatchKernel(const __grid_constant__ DecodeEdgeBatchParams b)
+template <typename Source, typename PlaneT, typename HostT>
+__global__ void __launch_bounds__(kBatchEdgeThreads) DecodeBatchKernel(const __grid_constant__ Source s)
 {
+    const typename Source::Walk walk(s);
+    if (walk.Idle(blockIdx.x))
+    {
+        return;
+    }
+    const int count = walk.Count();
     __shared__ uint64_t libmStorage[96];
     const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
     __syncthreads();
     int record = 0;
-    for (long long unit = blockIdx.x; unit < b.units; unit += gridDim.x)
+    for (long long unit = blockIdx.x; unit < walk.Units(); unit += gridDim.x)
     {
-        record = RecordOfUnit(b.window, b.count, record, unit);
-        const BatchRecord& r = b.window[record];
-        DecodeParams p = b.shared;
+        record = walk.Find(count, record, unit);
+        const BatchRecord& r = walk.Record(record);
+        DecodeParams p = s.shared;
         for (int k = 0; k < 4; ++k)
         {
             p.plane[k] = r.plane[k];
@@ -199,17 +409,107 @@ __global__ void __launch_bounds__(kBatchEdgeThreads) DecodeBatchKernel(const __g
         p.rowStride = r.rowStride;
         p.width = r.width;
         p.rowCount = r.rowCount;
-        p.yPhase = 0; // PlanDecodeBatch: every window starts on a 4:2:0 row pair
+        p.yPhase = 0; // every window starts on a 4:2:0 row pair
         DecodeChunkPixel<PlaneT, HostT, kBatchEdgeThreads>(p, t, static_cast<unsigned>(unit - r.firstUnit));
     }
 }
 
-template <typename SampleT, int ALPHA>
-void LaunchYccIntBatch(const YccIntBatchParams& b, int xs, int ys, unsigned grid, size_t shared, cudaStream_t stream)
+// ---- the dispatch ladders, one per kernel, for either source ------------------------------------------------------------
+
+template <typename Source, typename HostT, typename PlaneT, int CHANNELS, int PREMULTIPLY>
+void LaunchRgbIntChroma(const Source& s, int xs, int ys, unsigned grid, cudaStream_t stream)
 {
-    if (xs == 1 && ys == 1) DecodeYccToRgbIntBatchKernel<SampleT, 1, 1, ALPHA><<<grid, kRgbThreads, shared, stream>>>(b);
-    else if (xs == 1) DecodeYccToRgbIntBatchKernel<SampleT, 1, 0, ALPHA><<<grid, kRgbThreads, shared, stream>>>(b);
-    else DecodeYccToRgbIntBatchKernel<SampleT, 0, 0, ALPHA><<<grid, kRgbThreads, shared, stream>>>(b);
+    if (xs == 1 && ys == 1) EncodeRgbIntBatchKernel<Source, HostT, PlaneT, CHANNELS, 1, 1, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(s);
+    else if (xs == 1) EncodeRgbIntBatchKernel<Source, HostT, PlaneT, CHANNELS, 1, 0, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(s);
+    else EncodeRgbIntBatchKernel<Source, HostT, PlaneT, CHANNELS, 0, 0, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(s);
+}
+
+template <typename Source, typename HostT, typename PlaneT>
+void LaunchRgbIntChannels(const Source& s, const EncodeParams& d, unsigned grid, cudaStream_t stream)
+{
+    if (d.channels == 4 && d.premultiply) LaunchRgbIntChroma<Source, HostT, PlaneT, 4, 1>(s, d.xs, d.ys, grid, stream);
+    else if (d.channels == 4) LaunchRgbIntChroma<Source, HostT, PlaneT, 4, 0>(s, d.xs, d.ys, grid, stream);
+    else LaunchRgbIntChroma<Source, HostT, PlaneT, 3, 0>(s, d.xs, d.ys, grid, stream);
+}
+
+// The interior kernel of description `d`: host depth x plane depth x channels / premultiply x chroma.
+template <typename Source>
+void LaunchRgbInt(const Source& s, const EncodeParams& d, int hostDepth, unsigned grid, cudaStream_t stream)
+{
+    const bool wide = d.imageDepth > 8;
+    if (hostDepth == 16)
+    {
+        if (wide) LaunchRgbIntChannels<Source, uint16_t, uint16_t>(s, d, grid, stream);
+        else LaunchRgbIntChannels<Source, uint16_t, uint8_t>(s, d, grid, stream);
+    }
+    else
+    {
+        if (wide) LaunchRgbIntChannels<Source, uint8_t, uint16_t>(s, d, grid, stream);
+        else LaunchRgbIntChannels<Source, uint8_t, uint8_t>(s, d, grid, stream);
+    }
+}
+
+template <typename Source>
+void LaunchPlanar(const Source& s, int hostDepth, unsigned grid, cudaStream_t stream)
+{
+    if (hostDepth == 16) EncodePlanarBatchKernel<Source, uint16_t><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
+    else EncodePlanarBatchKernel<Source, uint8_t><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
+}
+
+template <typename Source, typename SampleT, int ALPHA>
+void LaunchYccIntChroma(const Source& s, int xs, int ys, unsigned grid, size_t bytes, cudaStream_t stream)
+{
+    if (xs == 1 && ys == 1) DecodeYccToRgbIntBatchKernel<Source, SampleT, 1, 1, ALPHA><<<grid, kRgbThreads, bytes, stream>>>(s);
+    else if (xs == 1) DecodeYccToRgbIntBatchKernel<Source, SampleT, 1, 0, ALPHA><<<grid, kRgbThreads, bytes, stream>>>(s);
+    else DecodeYccToRgbIntBatchKernel<Source, SampleT, 0, 0, ALPHA><<<grid, kRgbThreads, bytes, stream>>>(s);
+}
+
+// The interior kernel of description `d` (host depth x alpha x chroma), with `bytes` of staged tables.
+template <typename Source>
+void LaunchYccInt(const Source& s, const DecodeParams& d, unsigned grid, size_t bytes, cudaStream_t stream)
+{
+    if (d.hostDepth == 8)
+    {
+        if (d.hasAlpha) LaunchYccIntChroma<Source, uint8_t, 1>(s, d.xs, d.ys, grid, bytes, stream);
+        else LaunchYccIntChroma<Source, uint8_t, 0>(s, d.xs, d.ys, grid, bytes, stream);
+    }
+    else
+    {
+        if (d.hasAlpha) LaunchYccIntChroma<Source, uint16_t, 1>(s, d.xs, d.ys, grid, bytes, stream);
+        else LaunchYccIntChroma<Source, uint16_t, 0>(s, d.xs, d.ys, grid, bytes, stream);
+    }
+}
+
+template <typename Source>
+void LaunchDecodeEdge(const Source& s, int hostDepth, unsigned grid, cudaStream_t stream)
+{
+    if (hostDepth == 16) DecodeBatchKernel<Source, uint16_t, uint16_t><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
+    else DecodeBatchKernel<Source, uint8_t, uint8_t><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
+}
+
+// DecodeYccToRgbIntKernel's tables for description `d`.
+size_t YccTableBytesOf(const DecodeParams& d) { return YccTableBytes(d.bitDepth, d.hasAlpha && d.hostDepth != 8); }
+
+// The edge kernels' description: integer hosts have no transfer curve.
+EncodeParams PlanarShared(const EncodeParams& shared)
+{
+    EncodeParams edge = shared;
+    edge.useCurveView = 0;
+    return edge;
+}
+
+template <typename Chunk>
+Chunk ChunkOf(const decltype(Chunk::shared)& shared, const BatchRecord* records, int count, int64_t units)
+{
+    Chunk b{};
+    b.shared = shared;
+    b.count = count;
+    b.units = units;
+    for (int i = 0; i < count; ++i)
+    {
+        b.record[i] = records[i];
+    }
+    return b;
 }
 
 unsigned GridFor(long long blocks, long long cap)
@@ -217,20 +517,11 @@ unsigned GridFor(long long blocks, long long cap)
     return static_cast<unsigned>(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
-template <typename HostT, typename PlaneT, int CHANNELS, int PREMULTIPLY>
-void LaunchRgbIntBatch(const RgbIntBatchParams& b, int xs, int ys, unsigned grid, cudaStream_t stream)
+// `launches` if the launches before it succeeded, else the failure's status.
+int Launched(int launches)
 {
-    if (xs == 1 && ys == 1) EncodeRgbIntBatchKernel<HostT, PlaneT, CHANNELS, 1, 1, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(b);
-    else if (xs == 1) EncodeRgbIntBatchKernel<HostT, PlaneT, CHANNELS, 1, 0, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(b);
-    else EncodeRgbIntBatchKernel<HostT, PlaneT, CHANNELS, 0, 0, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(b);
-}
-
-template <typename HostT, typename PlaneT>
-void LaunchRgbIntBatchChannels(const RgbIntBatchParams& b, int channels, bool premultiply, int xs, int ys, unsigned grid, cudaStream_t stream)
-{
-    if (channels == 4 && premultiply) LaunchRgbIntBatch<HostT, PlaneT, 4, 1>(b, xs, ys, grid, stream);
-    else if (channels == 4) LaunchRgbIntBatch<HostT, PlaneT, 4, 0>(b, xs, ys, grid, stream);
-    else LaunchRgbIntBatch<HostT, PlaneT, 3, 0>(b, xs, ys, grid, stream);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? launches : ReportLaunchFailure(static_cast<int>(e));
 }
 
 } // namespace
@@ -238,110 +529,82 @@ void LaunchRgbIntBatchChannels(const RgbIntBatchParams& b, int channels, bool pr
 int LaunchEncodeBatchChunk(const EncodeParams& shared, int hostDepth, const BatchChunk& chunk, void* streamHandle)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
-    const int smCount = SmCountOrDefault(shared.smCount);
+    const long long cap = static_cast<long long>(SmCountOrDefault(shared.smCount)) * 16; // the single-image kernel's cap of 16 CTAs per SM
+    // one warp per unit
+    LaunchRgbInt(ChunkOf<RgbIntChunk>(RgbIntShared(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared, hostDepth,
+                 GridFor((chunk.interiorUnits + kWarps - 1) / kWarps, cap), stream);
+    const int interior = Launched(1);
+    if (interior < 0 || chunk.windows == 0)
     {
-        RgbIntBatchParams b{};
-        b.shared = RgbIntShared(shared);
-        b.count = chunk.images;
-        b.units = chunk.interiorUnits;
-        for (int i = 0; i < chunk.images; ++i)
-        {
-            b.image[i] = chunk.interior[i];
-        }
-        // one warp per unit; the single-image kernel's cap of 16 CTAs per SM
-        const unsigned grid = GridFor((chunk.interiorUnits + kWarps - 1) / kWarps, static_cast<long long>(smCount) * 16);
-        const bool wide = shared.imageDepth > 8;
-        if (hostDepth == 16)
-        {
-            if (wide) LaunchRgbIntBatchChannels<uint16_t, uint16_t>(b, shared.channels, shared.premultiply != 0, shared.xs, shared.ys, grid, stream);
-            else LaunchRgbIntBatchChannels<uint16_t, uint8_t>(b, shared.channels, shared.premultiply != 0, shared.xs, shared.ys, grid, stream);
-        }
-        else
-        {
-            if (wide) LaunchRgbIntBatchChannels<uint8_t, uint16_t>(b, shared.channels, shared.premultiply != 0, shared.xs, shared.ys, grid, stream);
-            else LaunchRgbIntBatchChannels<uint8_t, uint8_t>(b, shared.channels, shared.premultiply != 0, shared.xs, shared.ys, grid, stream);
-        }
-        const cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess)
-        {
-            return ReportLaunchFailure(static_cast<int>(e));
-        }
+        return interior;
     }
-    if (chunk.windows == 0)
-    {
-        return BatchChunkLaunches(chunk);
-    }
-    PlanarBatchParams b{};
-    b.shared = shared;
-    b.shared.useCurveView = 0; // integer hosts: no transfer curve
-    b.count = chunk.windows;
-    b.units = chunk.windowUnits;
-    for (int i = 0; i < chunk.windows; ++i)
-    {
-        b.window[i] = chunk.window[i];
-    }
-    const unsigned grid = GridFor(chunk.windowUnits, static_cast<long long>(smCount) * 16);
-    if (hostDepth == 16) EncodePlanarBatchKernel<uint16_t><<<grid, kBatchEdgeThreads, 0, stream>>>(b);
-    else EncodePlanarBatchKernel<uint8_t><<<grid, kBatchEdgeThreads, 0, stream>>>(b);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? BatchChunkLaunches(chunk) : ReportLaunchFailure(static_cast<int>(e));
+    LaunchPlanar(ChunkOf<PlanarChunk>(PlanarShared(shared), chunk.window, chunk.windows, chunk.windowUnits), hostDepth, GridFor(chunk.windowUnits, cap), stream);
+    return Launched(2);
 }
 
 int LaunchDecodeBatchChunk(const DecodeParams& shared, const BatchChunk& chunk, void* streamHandle)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
     const int smCount = SmCountOrDefault(shared.smCount);
+    LaunchYccInt(ChunkOf<YccIntChunk>(IntDecodeShared(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared,
+                 GridFor((chunk.interiorUnits + kWarps - 1) / kWarps, static_cast<long long>(smCount) * kYccBlocksPerSm), YccTableBytesOf(shared), stream);
+    const int interior = Launched(1);
+    if (interior < 0 || chunk.windows == 0)
     {
-        YccIntBatchParams b{};
-        b.shared.bitDepth = shared.bitDepth;
-        b.shared.maxCode = shared.maxCode;
-        b.shared.range = shared.range;
-        b.shared.matrix = shared.matrix;
-        b.shared.verifiedGreenDivision = shared.verifiedGreenDivision;
-        b.count = chunk.images;
-        b.units = chunk.interiorUnits;
-        for (int i = 0; i < chunk.images; ++i)
-        {
-            b.image[i] = chunk.interior[i];
-        }
-        // DecodeYccToRgbIntKernel's tables (at most 40 KB: no opt-in beyond the default 48 KB) and grid cap
-        const size_t entries = static_cast<size_t>(1) << shared.bitDepth;
-        const bool host8 = shared.hostDepth == 8;
-        const size_t bytes = 2 * sizeof(float) * entries + ((shared.hasAlpha && !host8) ? sizeof(uint16_t) * entries : 0);
-        const unsigned grid = GridFor((chunk.interiorUnits + kWarps - 1) / kWarps, static_cast<long long>(smCount) * kDecodeBlocksPerSm);
-        if (host8)
-        {
-            if (shared.hasAlpha) LaunchYccIntBatch<uint8_t, 1>(b, shared.xs, shared.ys, grid, bytes, stream);
-            else LaunchYccIntBatch<uint8_t, 0>(b, shared.xs, shared.ys, grid, bytes, stream);
-        }
-        else
-        {
-            if (shared.hasAlpha) LaunchYccIntBatch<uint16_t, 1>(b, shared.xs, shared.ys, grid, bytes, stream);
-            else LaunchYccIntBatch<uint16_t, 0>(b, shared.xs, shared.ys, grid, bytes, stream);
-        }
-        const cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess)
-        {
-            return ReportLaunchFailure(static_cast<int>(e));
-        }
+        return interior;
     }
-    if (chunk.windows == 0)
+    LaunchDecodeEdge(ChunkOf<DecodeEdgeChunk>(shared, chunk.window, chunk.windows, chunk.windowUnits), shared.hostDepth,
+                     GridFor(chunk.windowUnits, static_cast<long long>(smCount) * 16), stream);
+    return Launched(2);
+}
+
+int LaunchEncodeIndirect(const EncodeParams& shared, int hostDepth, bool tuned, int planeMask, const avifgpu_batch_image* images,
+                         const int32_t* count, int maxCount, void* workspace, int32_t* status, void* streamHandle)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
+    const unsigned cap = static_cast<unsigned>(SmCountOrDefault(shared.smCount)) * 16; // the chunk launchers' caps
+    EncodePlanner planner{};
+    planner.shared = shared;
+    planner.hostDepth = hostDepth;
+    planner.tuned = tuned ? 1 : 0;
+    planner.planeMask = planeMask;
+    PlanIndirectKernel<EncodePlanner><<<1, kPlanThreads, 0, stream>>>(planner, images, count, maxCount, workspace, status);
+    if (Launched(1) < 0)
     {
-        return BatchChunkLaunches(chunk);
+        return AVIFGPU_ERR_CUDA;
     }
-    DecodeEdgeBatchParams b{};
-    b.shared = shared;
-    b.count = chunk.windows;
-    b.units = chunk.windowUnits;
-    for (int i = 0; i < chunk.windows; ++i)
+    LaunchRgbInt(WorkspaceSource<Rgb16Params, 0>{ RgbIntShared(shared), workspace, maxCount }, shared, hostDepth, cap, stream);
+    if (Launched(1) < 0)
     {
-        b.window[i] = chunk.window[i];
+        return AVIFGPU_ERR_CUDA;
     }
-    const unsigned grid = GridFor(chunk.windowUnits, static_cast<long long>(smCount) * 16);
-    if (shared.hostDepth == 16) DecodeBatchKernel<uint16_t, uint16_t><<<grid, kBatchEdgeThreads, 0, stream>>>(b);
-    else DecodeBatchKernel<uint8_t, uint8_t><<<grid, kBatchEdgeThreads, 0, stream>>>(b);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? BatchChunkLaunches(chunk) : ReportLaunchFailure(static_cast<int>(e));
+    LaunchPlanar(WorkspaceSource<EncodeParams, 1>{ PlanarShared(shared), workspace, maxCount }, hostDepth, cap, stream);
+    return Launched(3);
+}
+
+int LaunchDecodeIndirect(const DecodeParams& shared, bool tuned, int planeMask, const avifgpu_batch_image* images, const int32_t* count,
+                         int maxCount, void* workspace, int32_t* status, void* streamHandle)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
+    const int smCount = SmCountOrDefault(shared.smCount);
+    DecodePlanner planner{};
+    planner.shared = shared;
+    planner.tuned = tuned ? 1 : 0;
+    planner.planeMask = planeMask;
+    PlanIndirectKernel<DecodePlanner><<<1, kPlanThreads, 0, stream>>>(planner, images, count, maxCount, workspace, status);
+    if (Launched(1) < 0)
+    {
+        return AVIFGPU_ERR_CUDA;
+    }
+    // A description the tuned kernel does not take plans no interior unit: its grid returns before staging, so it gets no tables.
+    LaunchYccInt(WorkspaceSource<IntDecodeParams, 0>{ IntDecodeShared(shared), workspace, maxCount }, shared,
+                 static_cast<unsigned>(smCount * kYccBlocksPerSm), tuned ? YccTableBytesOf(shared) : 0, stream);
+    if (Launched(1) < 0)
+    {
+        return AVIFGPU_ERR_CUDA;
+    }
+    LaunchDecodeEdge(WorkspaceSource<DecodeParams, 1>{ shared, workspace, maxCount }, shared.hostDepth, static_cast<unsigned>(smCount * 16), stream);
+    return Launched(3);
 }
 
 } // namespace avifgpu

@@ -30,10 +30,9 @@ namespace
 
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
-constexpr int kBlocksPerSm = 3;
 
 template <typename SampleT, int XS, int YS, int ALPHA>
-__global__ void __launch_bounds__(kThreads, kBlocksPerSm) DecodeYccToRgbIntKernel(const IntDecodeParams p)
+__global__ void __launch_bounds__(kThreads, kYccBlocksPerSm) DecodeYccToRgbIntKernel(const IntDecodeParams p)
 {
     constexpr int kRows = YS ? 2 : 1;
     extern __shared__ __align__(16) uint8_t sharedBytes[];
@@ -99,8 +98,7 @@ __global__ void __launch_bounds__(kThreads, kBlocksPerSm) DecodeYccToRgbIntKerne
 template <typename SampleT, int XS, int YS, int ALPHA>
 cudaError_t LaunchOne(const IntDecodeParams& fp, int smCount, cudaStream_t stream)
 {
-    const size_t entries = static_cast<size_t>(1) << fp.bitDepth;
-    const size_t shared = 2 * sizeof(float) * entries + ((ALPHA && sizeof(SampleT) == 2) ? sizeof(uint16_t) * entries : 0);
+    const size_t shared = YccTableBytes(fp.bitDepth, ALPHA && sizeof(SampleT) == 2);
     static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
     {
         const cudaError_t e = AllowDynamicShared(DecodeYccToRgbIntKernel<SampleT, XS, YS, ALPHA>, 64 * 1024, configuredDevices);
@@ -112,7 +110,7 @@ cudaError_t LaunchOne(const IntDecodeParams& fp, int smCount, cudaStream_t strea
     constexpr int rowsPerUnit = YS ? 2 : 1;
     const long long units = static_cast<long long>((fp.width + kUnitPixels - 1) / kUnitPixels) * ((fp.rowCount + rowsPerUnit - 1) / rowsPerUnit);
     long long blocks = (units + kWarps - 1) / kWarps;
-    const long long resident = static_cast<long long>(smCount) * kBlocksPerSm;
+    const long long resident = static_cast<long long>(smCount) * kYccBlocksPerSm;
     if (blocks > resident)
     {
         blocks = resident;
@@ -402,7 +400,7 @@ int LaunchDecodeFastInteger(const DecodeParams& p, void* streamHandle)
     const int sampleBytes = p.hostDepth == 8 ? 1 : 2;
     const int width8 = inner.width;
     const int evenRows = inner.rows;
-    IntDecodeParams fp{};
+    IntDecodeParams fp = IntDecodeShared(p);
     for (int k = 0; k < 4; ++k)
     {
         fp.plane[k] = static_cast<const uint8_t*>(p.plane[k]);
@@ -412,11 +410,6 @@ int LaunchDecodeFastInteger(const DecodeParams& p, void* streamHandle)
     fp.rowStride = p.rowStride;
     fp.width = width8;
     fp.rowCount = evenRows;
-    fp.bitDepth = p.bitDepth;
-    fp.maxCode = p.maxCode;
-    fp.range = p.range;
-    fp.matrix = p.matrix;
-    fp.verifiedGreenDivision = p.verifiedGreenDivision;
 
     const int smCount = SmCountOrDefault(p.smCount);
     cudaError_t e;

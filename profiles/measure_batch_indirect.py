@@ -54,7 +54,7 @@ def kernel_split(run, calls=50):
         torch.cuda.synchronize()
     out = {}
     for event in prof.key_averages():
-        if "Indirect" in event.key:
+        if "PlanIndirect" in event.key or "WorkspaceSource" in event.key:
             name = ("plan" if "PlanIndirect" in event.key else "interior" if ("RgbInt" in event.key or "YccToRgbInt" in event.key) else "edge")
             out[name] = out.get(name, 0.0) + event.device_time_total / calls
     return out

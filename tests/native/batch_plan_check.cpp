@@ -1,5 +1,5 @@
-// tests/native/batch_plan_check.cpp -- host-side check of PlanEncodeBatch (csrc/host_params.cpp), the planner behind
-// avifgpu_encode_batch_device.  For every valid encode description and seeded random batches of 1 to 300 images of mixed
+// tests/native/batch_plan_check.cpp -- host-side check of PlanEncodeBatch (csrc/host_params.cpp, csrc/batch_plan.h), the
+// planner behind avifgpu_encode_batch_device.  For every valid encode description and seeded random batches of 1 to 300 images of mixed
 // sizes (1 x 1, widths below 8, odd widths and heights) on fake planes, some of them misaligned:
 //   - every pixel and every chroma site of every image is covered exactly once, by an interior, an edge window or a
 //     direct call, read back from the records' rows and plane pointers;
@@ -9,6 +9,7 @@
 //   - a chunk's kernel parameters fit the 32764-byte limit.
 // Decode batches (PlanDecodeBatch) get the pixel coverage, routing and launch checks too.
 // Prints "encode descriptions=N batches=M images=K" and "decode descriptions=N images=K"; exit code 1 on any failure.
+#include "batch_plan.h"
 #include "host_params.h"
 
 #include <cstdio>
@@ -38,6 +39,23 @@ struct FakeImage
     int colBytes;
     PlaneGeometry g[4];
 };
+
+// The batch record of an image's own block.
+template <typename Params>
+avifgpu_batch_image BatchImageOf(const Params& p)
+{
+    avifgpu_batch_image image{};
+    image.width = p.width;
+    image.height = p.rowCount;
+    image.rows = const_cast<void*>(static_cast<const void*>(p.rows));
+    image.row_stride_bytes = p.rowStride;
+    for (int k = 0; k < 4; ++k)
+    {
+        image.planes.data[k] = const_cast<void*>(static_cast<const void*>(p.plane[k]));
+        image.planes.stride[k] = p.planeStride[k];
+    }
+    return image;
+}
 
 // Marks the pixels of the record [x, x + width) x [y, y + rows) of `image`, from its rows pointer.
 void Cover(std::vector<int>& count, const FakeImage& im, const BatchRecord& r, int description, int batch)
@@ -103,13 +121,21 @@ int main()
                                     continue;
                                 }
                                 ++descriptions;
+                                int planeMask = 0;
+                                for (int k = 0; k < 4; ++k)
+                                {
+                                    planeMask |= EncodePlaneGeometry(d, k).present ? 1 << k : 0;
+                                }
                                 for (int verified : { 0, 1 })
                                 {
+                                    EncodeParams shared;
+                                    FillEncodeParams(d, &shared);
+                                    shared.verifiedPremultiply = verified;
                                     for (int trial = 0; trial < 3; ++trial)
                                     {
                                         const int n = 1 + static_cast<int>(rng() % (trial == 2 ? 300 : 20));
                                         std::vector<FakeImage> fake(n);
-                                        std::vector<EncodeParams> params(n);
+                                        std::vector<avifgpu_batch_image> batch(n);
                                         for (int i = 0; i < n; ++i)
                                         {
                                             avifgpu_encode_desc di = d;
@@ -137,10 +163,10 @@ int main()
                                                 im.p.plane[k] = reinterpret_cast<void*>(im.planeBase[k]);
                                                 im.p.planeStride[k] = static_cast<int64_t>(im.g[k].widthSamples) * im.g[k].bytesPerSample + 128;
                                             }
-                                            params[i] = im.p;
+                                            batch[i] = BatchImageOf(im.p);
                                         }
                                         BatchPlan plan;
-                                        PlanEncodeBatch(params, hostDepth, &plan);
+                                        PlanEncodeBatch(shared, hostDepth, planeMask, batch.data(), n, &plan);
                                         ++batches;
                                         images += n;
                                         std::vector<std::vector<int>> count(n);
@@ -246,6 +272,11 @@ int main()
                         continue;
                     }
                     ++decodeDescriptions;
+                    int planeMask = 0;
+                    for (int k = 0; k < 4; ++k)
+                    {
+                        planeMask |= DecodePlaneGeometry(d, k).present ? 1 << k : 0;
+                    }
                     for (int trial = 0; trial < 3; ++trial)
                     {
                         const int n = 1 + static_cast<int>(rng() % (trial == 2 ? 300 : 20));
@@ -273,8 +304,13 @@ int main()
                                 }
                             }
                         }
+                        std::vector<avifgpu_batch_image> batch(n);
+                        for (int i = 0; i < n; ++i)
+                        {
+                            batch[i] = BatchImageOf(params[i]);
+                        }
                         BatchPlan plan;
-                        PlanDecodeBatch(params, &plan);
+                        PlanDecodeBatch(probe, planeMask, batch.data(), n, &plan);
                         decodeImages += n;
                         std::vector<std::vector<int>> count(n);
                         std::vector<int> batched(n, 0);

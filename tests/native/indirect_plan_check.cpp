@@ -1,17 +1,19 @@
-// tests/native/indirect_plan_check.cpp -- host-side check of the plan behind avifgpu_encode_batch_indirect /
-// avifgpu_decode_batch_indirect (csrc/batch_indirect.h), compiled with the host compiler from the same __host__ __device__
-// functions the plan kernel runs.  For every supported encode and decode description (with and without the verified
-// premultiply) and seeded random image sets of sizes 0 to 600, negative sizes, NULL rows, NULL planes and misaligned
-// pointers and strides, on fake padded planes:
+// tests/native/indirect_plan_check.cpp -- host-side check of the per-image planning step both batch APIs share
+// (PlanBatchEncodeImage / PlanBatchDecodeImage, csrc/batch_plan.h) and of the device-described batch's workspace, compiled
+// with the host compiler from the same __host__ __device__ functions the plan kernel runs.  For every supported encode
+// and decode description (with and without the verified premultiply) and seeded random image sets of sizes 0 to 600,
+// negative sizes, NULL rows, NULL planes and misaligned pointers and strides, on fake padded planes:
 //   - a rejected image (negative size; non-empty with NULL rows or a NULL plane the description has) gets BAD_PARAM and
 //     no record, an empty image OK and no record;
-//   - the interior records and windows, and their units, equal PlanEncodeBatch / PlanDecodeBatch's for the same images
-//     with chunking ignored, in image order;
-//   - an image the planners send to a direct call becomes exactly one whole-image window;
+//   - every pixel of an accepted image is covered exactly once by its interior and windows, judged from the records'
+//     rows pointers, and each record's luma and chroma planes sit at its first pixel and chroma site;
+//   - an image has an interior exactly when EncodeRgbIntInterior / DecodeYccIntInterior of its own block (built here as a
+//     direct call builds it) takes it, that interior is the predicate's rectangle, and its windows are the strips around
+//     it; any other image is exactly one whole-image window; every unit count matches its record;
 //   - with the records laid out at the exclusive prefix sums of their units (IndirectWorkspaceLayout), FindRecord finds
 //     the owner of every unit from any earlier starting record.
 // Prints "encode descriptions=N images=K" and "decode descriptions=N images=K"; exit code 1 on any failure.
-#include "batch_indirect.h"
+#include "batch_plan.h"
 #include "host_params.h"
 
 #include <cstdio>
@@ -36,7 +38,7 @@ void Fail(const char* what, int description, int image)
 
 bool SameRecord(const BatchRecord& a, const BatchRecord& b)
 {
-    // every field but the first unit, which restarts in each chunk of the host-described planners
+    // every field but the first unit, which the plan sets after its scan
     BatchRecord x = a, y = b;
     x.firstUnit = y.firstUnit = 0;
     return std::memcmp(&x, &y, sizeof(x)) == 0;
@@ -88,41 +90,85 @@ std::vector<avifgpu_batch_image> RandomImages(std::mt19937& rng, int n, int colB
     return images;
 }
 
-struct Reference
+// Checks the plan `q` of an accepted, non-empty image against its own block `p` and `inner`, the single-image predicate's
+// interior of that block.  A window has units of (1 << edgeXs) x (1 << edgeYs) pixels.
+template <typename Params>
+void CheckImagePlan(const char* direction, const BatchImagePlan& q, const Params& p, Interior inner, int colBytes, int sampleBytes, int edgeXs,
+                    int edgeYs, int description, int image)
 {
-    std::vector<int> interiorOf;   // per image: index into `interior`, or -1
-    std::vector<BatchRecord> interior;
-    std::vector<std::vector<BatchRecord>> windows; // per image
-    std::vector<int> fallback;     // per image: 1 when a direct call converts it
-};
-
-Reference Flatten(const BatchPlan& plan, int n)
-{
-    Reference r;
-    r.interiorOf.assign(n, -1);
-    r.windows.assign(n, {});
-    r.fallback.assign(n, 0);
-    for (const BatchChunk& c : plan.chunks)
+    char what[96];
+    const auto fail = [&](const char* check)
     {
-        for (int j = 0; j < c.images; ++j)
+        std::snprintf(what, sizeof(what), "%s %s", direction, check);
+        Fail(what, description, image);
+    };
+    // the records, as rectangles of the image read back from their rows pointers
+    BatchRecord records[3];
+    int count = 0;
+    if (inner.width > 0)
+    {
+        if (q.interior.width != inner.width || q.interior.rowCount != inner.rows || q.interior.rows != p.rows ||
+            q.interiorUnits != BatchInteriorUnits(inner.width, inner.rows, p.ys))
+            fail("interior");
+        if (q.interior.width == 0)
         {
-            r.interiorOf[c.imageIndex[j]] = static_cast<int>(r.interior.size());
-            r.interior.push_back(c.interior[j]);
+            fail("image the predicate batches has no interior");
+            return;
         }
-        for (int j = 0; j < c.windows; ++j)
+        records[count++] = q.interior;
+        const int strips = (inner.width < p.width ? 1 : 0) + (inner.rows < p.rowCount ? 1 : 0);
+        if (q.windows != strips)
         {
-            r.windows[c.windowImage[j]].push_back(c.window[j]);
+            fail("window count");
+            return;
         }
     }
-    for (const int32_t i : plan.fallback)
+    else if (q.interior.width != 0 || q.interiorUnits != 0 || q.windows != 1 || !SameRecord(q.window[0], RecordOf(p)) ||
+             q.windowUnits[0] != BatchEdgeUnits(p.width, p.rowCount, edgeXs, edgeYs) || q.windowUnits[1] != 0)
     {
-        r.fallback[i] = 1;
+        fail("fallback is not one whole-image window");
+        return;
     }
-    return r;
+    for (int k = 0; k < q.windows; ++k)
+    {
+        if (q.windowUnits[k] != BatchEdgeUnits(q.window[k].width, q.window[k].rowCount, edgeXs, edgeYs)) fail("window");
+        records[count++] = q.window[k];
+    }
+    if (q.windows < 2 && q.windowUnits[1] != 0) fail("missing window has units");
+    int x0[3], y0[3];
+    int64_t area = 0;
+    for (int j = 0; j < count; ++j)
+    {
+        const BatchRecord& r = records[j];
+        const int64_t offset = static_cast<int64_t>(reinterpret_cast<uintptr_t>(r.rows) - reinterpret_cast<uintptr_t>(p.rows));
+        y0[j] = static_cast<int>(offset / p.rowStride);
+        x0[j] = static_cast<int>(offset % p.rowStride) / colBytes;
+        if (offset < 0 || (offset % p.rowStride) % colBytes || r.width <= 0 || r.rowCount <= 0 || x0[j] + r.width > p.width ||
+            y0[j] + r.rowCount > p.rowCount)
+        {
+            fail("record outside its image");
+            return;
+        }
+        area += static_cast<int64_t>(r.width) * r.rowCount;
+        const uintptr_t luma = reinterpret_cast<uintptr_t>(p.plane[0]) + static_cast<uintptr_t>(y0[j] * p.planeStride[0] + x0[j] * sampleBytes);
+        const uintptr_t chroma = reinterpret_cast<uintptr_t>(p.plane[1]) +
+                                 static_cast<uintptr_t>((y0[j] >> p.ys) * p.planeStride[1] + (x0[j] >> p.xs) * sampleBytes);
+        if (reinterpret_cast<uintptr_t>(r.plane[0]) != luma || reinterpret_cast<uintptr_t>(r.plane[1]) != chroma || (x0[j] & ((1 << p.xs) - 1)) ||
+            (y0[j] & ((1 << p.ys) - 1)))
+            fail("planes of a record");
+        for (int i = 0; i < j; ++i)
+        {
+            const bool apart = x0[i] + records[i].width <= x0[j] || x0[j] + r.width <= x0[i] || y0[i] + records[i].rowCount <= y0[j] ||
+                               y0[j] + r.rowCount <= y0[i];
+            if (!apart) fail("records overlap");
+        }
+    }
+    // disjoint rectangles inside the image whose areas add up to it cover every pixel exactly once
+    if (area != static_cast<int64_t>(p.width) * p.rowCount) fail("pixel not covered exactly once");
 }
 
 // The plan kernel's output for `plans`, laid out serially, and FindRecord against a linear search over every unit.
-void CheckLayoutAndSearch(std::mt19937& rng, const std::vector<IndirectImagePlan>& plans, int description)
+void CheckLayoutAndSearch(std::mt19937& rng, const std::vector<BatchImagePlan>& plans, int description)
 {
     const int n = static_cast<int>(plans.size());
     std::vector<int64_t> interiorFirst(n), windowFirst(2 * static_cast<size_t>(n));
@@ -215,80 +261,37 @@ int main()
                                 const std::vector<avifgpu_batch_image> batch =
                                     RandomImages(rng, n, EncodeHostColBytes(d), planeMask, planeXs, depth > 8 ? 2 : 1, &rejected);
                                 images += n;
-                                std::vector<IndirectImagePlan> plans(n);
-                                std::vector<EncodeParams> params(n);
+                                std::vector<BatchImagePlan> plans(n);
                                 for (int i = 0; i < n; ++i)
                                 {
-                                    plans[i] = PlanIndirectEncodeImage(shared, hostDepth, tuned, planeMask, batch[i]);
-                                    // what the host-described call builds for the same image (host checks passed)
-                                    avifgpu_encode_desc di = d;
-                                    di.width = rejected[i] ? 0 : batch[i].width;
-                                    di.height = rejected[i] ? 0 : batch[i].height;
-                                    EncodeParams& p = params[i];
-                                    FillEncodeParams(di, &p);
-                                    p.verifiedPremultiply = verified;
-                                    if (!rejected[i] && di.width > 0 && di.height > 0)
-                                    {
-                                        p.rows = batch[i].rows;
-                                        p.rowStride = batch[i].row_stride_bytes;
-                                        p.rowCount = di.height;
-                                        for (int k = 0; k < 4; ++k)
-                                        {
-                                            if ((planeMask >> k) & 1)
-                                            {
-                                                p.plane[k] = batch[i].planes.data[k];
-                                                p.planeStride[k] = batch[i].planes.stride[k];
-                                            }
-                                        }
-                                    }
-                                    else
-                                    {
-                                        p.width = p.rowCount = 0;
-                                    }
-                                }
-                                BatchPlan plan;
-                                PlanEncodeBatch(params, hostDepth, &plan);
-                                const Reference ref = Flatten(plan, n);
-                                for (int i = 0; i < n; ++i)
-                                {
-                                    const IndirectImagePlan& q = plans[i];
-                                    const int expectStatus = rejected[i] ? AVIFGPU_ERR_BAD_PARAM : AVIFGPU_OK;
-                                    if (q.status != expectStatus) Fail("encode status", descriptions, i);
-                                    if (params[i].width == 0)
+                                    const BatchImagePlan& q = plans[i] = PlanBatchEncodeImage(shared, hostDepth, tuned, planeMask, batch[i]);
+                                    if (q.status != (rejected[i] ? AVIFGPU_ERR_BAD_PARAM : AVIFGPU_OK)) Fail("encode status", descriptions, i);
+                                    if (rejected[i] || batch[i].width == 0 || batch[i].height == 0)
                                     {
                                         if (q.windows != 0 || q.interiorUnits != 0 || q.windowUnits[0] != 0 || q.windowUnits[1] != 0 || q.interior.width != 0)
                                             Fail("encode records of a rejected or empty image", descriptions, i);
                                         continue;
                                     }
-                                    if (ref.fallback[i])
+                                    // the image's own block, as the direct call of it builds it
+                                    avifgpu_encode_desc di = d;
+                                    di.width = batch[i].width;
+                                    di.height = batch[i].height;
+                                    EncodeParams p;
+                                    FillEncodeParams(di, &p);
+                                    p.verifiedPremultiply = verified;
+                                    p.rows = batch[i].rows;
+                                    p.rowStride = batch[i].row_stride_bytes;
+                                    p.rowCount = di.height;
+                                    for (int k = 0; k < 4; ++k)
                                     {
-                                        const EncodeParams& p = params[i];
-                                        if (q.interiorUnits != 0 || q.windows != 1 || !SameRecord(q.window[0], RecordOf(p)) ||
-                                            q.windowUnits[0] != BatchEdgeUnits(p.width, p.rowCount, p.xs, p.ys) || q.windowUnits[1] != 0)
-                                            Fail("encode fallback is not one whole-image window", descriptions, i);
-                                        continue;
+                                        if ((planeMask >> k) & 1)
+                                        {
+                                            p.plane[k] = batch[i].planes.data[k];
+                                            p.planeStride[k] = batch[i].planes.stride[k];
+                                        }
                                     }
-                                    if (ref.interiorOf[i] < 0)
-                                    {
-                                        Fail("encode image the planner batches has no interior", descriptions, i);
-                                        continue;
-                                    }
-                                    const BatchRecord& r = ref.interior[ref.interiorOf[i]];
-                                    if (!SameRecord(q.interior, r) ||
-                                        q.interiorUnits != BatchInteriorUnits(r.width, r.rowCount, params[i].ys))
-                                        Fail("encode interior", descriptions, i);
-                                    if (q.windows != static_cast<int>(ref.windows[i].size()))
-                                    {
-                                        Fail("encode window count", descriptions, i);
-                                        continue;
-                                    }
-                                    for (int k = 0; k < q.windows; ++k)
-                                    {
-                                        const BatchRecord& wr = ref.windows[i][k];
-                                        if (!SameRecord(q.window[k], wr) || q.windowUnits[k] != BatchEdgeUnits(wr.width, wr.rowCount, params[i].xs, params[i].ys))
-                                            Fail("encode window", descriptions, i);
-                                    }
-                                    if (q.windows < 2 && q.windowUnits[1] != 0) Fail("encode missing window has units", descriptions, i);
+                                    CheckImagePlan("encode", q, p, EncodeRgbIntInterior(p, hostDepth), EncodeHostColBytes(d), depth > 8 ? 2 : 1, p.xs, p.ys,
+                                                   descriptions, i);
                                 }
                                 CheckLayoutAndSearch(rng, plans, descriptions);
                             }
@@ -332,76 +335,34 @@ int main()
                         std::vector<int> rejected;
                         const std::vector<avifgpu_batch_image> batch = RandomImages(rng, n, DecodeHostColBytes(d), planeMask, planeXs, bitDepth > 8 ? 2 : 1, &rejected);
                         decodeImages += n;
-                        std::vector<IndirectImagePlan> plans(n);
-                        std::vector<DecodeParams> params(n);
+                        std::vector<BatchImagePlan> plans(n);
                         for (int i = 0; i < n; ++i)
                         {
-                            plans[i] = PlanIndirectDecodeImage(shared, tuned, planeMask, batch[i]);
-                            avifgpu_decode_desc di = d;
-                            di.width = rejected[i] ? 0 : batch[i].width;
-                            di.height = rejected[i] ? 0 : batch[i].height;
-                            DecodeParams& p = params[i];
-                            FillDecodeParams(di, transfer, &p, nullptr);
-                            if (!rejected[i] && di.width > 0 && di.height > 0)
-                            {
-                                p.rows = batch[i].rows;
-                                p.rowStride = batch[i].row_stride_bytes;
-                                p.rowCount = di.height;
-                                for (int k = 0; k < 4; ++k)
-                                {
-                                    if ((planeMask >> k) & 1)
-                                    {
-                                        p.plane[k] = batch[i].planes.data[k];
-                                        p.planeStride[k] = batch[i].planes.stride[k];
-                                    }
-                                }
-                            }
-                            else
-                            {
-                                p.width = p.rowCount = 0;
-                            }
-                        }
-                        BatchPlan plan;
-                        PlanDecodeBatch(params, &plan);
-                        const Reference ref = Flatten(plan, n);
-                        for (int i = 0; i < n; ++i)
-                        {
-                            const IndirectImagePlan& q = plans[i];
+                            const BatchImagePlan& q = plans[i] = PlanBatchDecodeImage(shared, tuned, planeMask, batch[i]);
                             if (q.status != (rejected[i] ? AVIFGPU_ERR_BAD_PARAM : AVIFGPU_OK)) Fail("decode status", decodeDescriptions, i);
-                            if (params[i].width == 0)
+                            if (rejected[i] || batch[i].width == 0 || batch[i].height == 0)
                             {
                                 if (q.windows != 0 || q.interiorUnits != 0 || q.windowUnits[0] != 0 || q.windowUnits[1] != 0 || q.interior.width != 0)
                                     Fail("decode records of a rejected or empty image", decodeDescriptions, i);
                                 continue;
                             }
-                            if (ref.fallback[i])
+                            avifgpu_decode_desc di = d;
+                            di.width = batch[i].width;
+                            di.height = batch[i].height;
+                            DecodeParams p;
+                            FillDecodeParams(di, transfer, &p, nullptr);
+                            p.rows = batch[i].rows;
+                            p.rowStride = batch[i].row_stride_bytes;
+                            p.rowCount = di.height;
+                            for (int k = 0; k < 4; ++k)
                             {
-                                const DecodeParams& p = params[i];
-                                if (q.interiorUnits != 0 || q.windows != 1 || !SameRecord(q.window[0], RecordOf(p)) ||
-                                    q.windowUnits[0] != BatchEdgeUnits(p.width, p.rowCount, 0, 0) || q.windowUnits[1] != 0)
-                                    Fail("decode fallback is not one whole-image window", decodeDescriptions, i);
-                                continue;
+                                if ((planeMask >> k) & 1)
+                                {
+                                    p.plane[k] = batch[i].planes.data[k];
+                                    p.planeStride[k] = batch[i].planes.stride[k];
+                                }
                             }
-                            if (ref.interiorOf[i] < 0)
-                            {
-                                Fail("decode image the planner batches has no interior", decodeDescriptions, i);
-                                continue;
-                            }
-                            const BatchRecord& r = ref.interior[ref.interiorOf[i]];
-                            if (!SameRecord(q.interior, r) || q.interiorUnits != BatchInteriorUnits(r.width, r.rowCount, params[i].ys))
-                                Fail("decode interior", decodeDescriptions, i);
-                            if (q.windows != static_cast<int>(ref.windows[i].size()))
-                            {
-                                Fail("decode window count", decodeDescriptions, i);
-                                continue;
-                            }
-                            for (int k = 0; k < q.windows; ++k)
-                            {
-                                const BatchRecord& wr = ref.windows[i][k];
-                                if (!SameRecord(q.window[k], wr) || q.windowUnits[k] != BatchEdgeUnits(wr.width, wr.rowCount, 0, 0))
-                                    Fail("decode window", decodeDescriptions, i);
-                            }
-                            if (q.windows < 2 && q.windowUnits[1] != 0) Fail("decode missing window has units", decodeDescriptions, i);
+                            CheckImagePlan("decode", q, p, DecodeYccIntInterior(p), DecodeHostColBytes(d), bitDepth > 8 ? 2 : 1, 0, 0, decodeDescriptions, i);
                         }
                         CheckLayoutAndSearch(rng, plans, decodeDescriptions);
                     }

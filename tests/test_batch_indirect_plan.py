@@ -1,11 +1,14 @@
-"""The plan behind avifgpu_encode_batch_indirect / avifgpu_decode_batch_indirect (csrc/batch_indirect.h), on the CPU.
+"""The per-image planning step both batch APIs share (PlanBatchEncodeImage / PlanBatchDecodeImage, csrc/batch_plan.h),
+and the workspace of the device-described batch, on the CPU.
 
-tests/native/indirect_plan_check.cpp compiles the plan kernel's per-image step -- the same __host__ __device__ functions --
-with the host compiler.  Over seeded random image sets (sizes 0 to 600, negative sizes, NULL rows and planes, misaligned
-pointers and strides) for every supported encode and decode description it checks that rejected images get BAD_PARAM
-and no record, that interiors, windows and their units equal the host-described planners' (PlanEncodeBatch /
-PlanDecodeBatch, chunking ignored), that an image those send to a direct call becomes one whole-image window, and that
-FindRecord finds the owner of every unit of the prefix-summed layout."""
+tests/native/indirect_plan_check.cpp compiles the per-image step -- the same __host__ __device__ functions the plan kernel
+runs -- with the host compiler.  Over seeded random image sets (sizes 0 to 600, negative sizes, NULL rows and planes,
+misaligned pointers and strides) for every supported encode and decode description it checks that rejected images get
+BAD_PARAM and no record; that an accepted image's records cover every pixel exactly once, judged from their rows
+pointers, with their planes at their first pixel and chroma site; that an image has an interior exactly when the
+single-image predicate of its own block (EncodeRgbIntInterior / DecodeYccIntInterior) takes it, with the strips around
+it as windows, and is otherwise one whole-image window; and that FindRecord finds the owner of every unit of the
+prefix-summed layout."""
 import ctypes as C
 import os
 import re
@@ -17,7 +20,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "avif-format_b200", "csrc")
 
 
-def test_indirect_plan_matches_the_host_planners(tmp_path):
+def test_batch_image_plan_covers_and_routes_every_image(tmp_path):
     exe = tmp_path / "indirect_plan_check"
     subprocess.run(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-I", "/usr/local/cuda/include", "-I", CSRC,
                     os.path.join(ROOT, "tests", "native", "indirect_plan_check.cpp"), os.path.join(CSRC, "host_params.cpp"),

@@ -1,5 +1,5 @@
 """The batch planners behind avifgpu_encode_batch_device / avifgpu_decode_batch_device (PlanEncodeBatch,
-PlanDecodeBatch in csrc/host_params.cpp), on the CPU.
+PlanDecodeBatch in csrc/host_params.cpp: chunks packed from the per-image step of csrc/batch_plan.h), on the CPU.
 
 tests/native/batch_plan_check.cpp plans seeded random batches of 1 to 300 images of mixed sizes (1 x 1, widths below 8,
 odd widths and heights, misaligned rows) for every valid encode description, on fake padded planes, and checks that
@@ -18,7 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "avif-format_b200", "csrc")
 
 
-def test_plan_covers_every_pixel_once(tmp_path):
+def test_chunked_plan_covers_every_pixel_once(tmp_path):
     exe = tmp_path / "batch_plan_check"
     subprocess.run(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-I", "/usr/local/cuda/include", "-I", CSRC,
                     os.path.join(ROOT, "tests", "native", "batch_plan_check.cpp"), os.path.join(CSRC, "host_params.cpp"),

@@ -203,7 +203,7 @@ def test_persistent_walk_runs_several_passes(ctx):
     import torch
     desc = PARITY[0][1]
     sm = torch.cuda.get_device_properties(0).multi_processor_count
-    # interior grid: at most 16 CTAs of 8 warps per SM (kernels_batch.cu), one 256-pixel unit per warp
+    # interior grid: at most 16 CTAs of 8 warps per SM (LaunchEncodeBatchChunk, kernels_batch.cu), one 256-pixel unit per warp
     warps = sm * 16 * 8
     images = eligible_images(desc, 64, 512, 512, "passes")
     units = len(images) * 2 * 512

@@ -1,5 +1,6 @@
 """avifgpu_encode_batch_indirect / avifgpu_decode_batch_indirect: batches whose image records and count are read from
-device memory when the work runs (include/avifgpu.h, "batches described in device memory").
+device memory when the work runs (include/avifgpu.h, "batches described in device memory"), run by the batched kernels
+of kernels_batch.cu under their workspace record source.
 
 Every accepted image is compared bit for bit with a direct *_rows_device call of the same image and with the CPU checker
 (the restatement for encode, the compiled reference for decode, by pick()), and the sentinel in the row padding must

@@ -1195,9 +1195,9 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_indirect(avifgpu_context* ctx, const avi
     {
         return status;
     }
-    if ((d.host_depth != 8 && d.host_depth != 16) || d.colorspace != AVIFGPU_COLORSPACE_YCBCR || d.alpha_state == AVIFGPU_ALPHA_PREMULTIPLIED)
+    if (d.colorspace != AVIFGPU_COLORSPACE_YCBCR || d.alpha_state == AVIFGPU_ALPHA_PREMULTIPLIED)
     {
-        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "device-described batches decode YCbCr with no or straight alpha into 8- or 16-bit hosts");
+        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "device-described batches decode YCbCr with no or straight alpha");
     }
     DecodeParams shared;
     if (!FillDecodeParams(d, transfer, &shared, &error))
@@ -1217,7 +1217,7 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_indirect(avifgpu_context* ctx, const avi
     }
     shared.smCount = ctx->smCount;
     ctx->FirstUseDecode(d, transfer, capturing, &shared);
-    const int launched = LaunchDecodeIndirect(shared, DecodeYccIntTuned(shared), planeMask, device_images, device_count, max_count, device_workspace,
+    const int launched = LaunchDecodeIndirect(shared, DecodeBatchTuned(shared), planeMask, device_images, device_count, max_count, device_workspace,
                                               device_status, cuda_stream);
     if (launched < 0)
     {

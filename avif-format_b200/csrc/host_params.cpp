@@ -469,6 +469,76 @@ Interior DecodeYccIntInterior(const DecodeParams& p)
     return DecodeYccIntTuned(p) ? DecodeYccIntBlockInterior(p) : Interior{ 0, 0 };
 }
 
+F32DecodeFactors F32DecodeFactorsOf(const avifpix::InverseMatrix& matrix)
+{
+    F32DecodeFactors f;
+    f.rGain = (2 * (1 - matrix.kr));
+    f.bGain = (2 * (1 - matrix.kb));
+    f.gCr = matrix.kr * (1 - matrix.kr);
+    f.gCb = matrix.kb * (1 - matrix.kb);
+    f.kgReciprocal = 1.0f / matrix.kg;
+    return f;
+}
+
+namespace
+{
+// True when every clamped channel sum Y + offset of the configuration is +0 or a normal float.  Table entries are 0 or at
+// least 2^-14 in magnitude (depth <= 12: k / max, k / max - 0.5); with the matrix factors at least 2^-16 every product is 0 or
+// at least 2^-30, a sum of two such floats is a multiple of 2^-53 (0 or at least that), the green term after its division a
+// float of at least 2^-54, and Y minus it a multiple of 2^-77: nowhere near 2^-126.  Every H.273 matrix passes.
+bool ChannelSumsStayNormal(int bitDepth, const F32DecodeFactors& f, float kg)
+{
+    const float least = 1.0f / 65536.0f;
+    const auto moderate = [least](float v) { return v >= least && v <= 4.0f; };
+    return bitDepth <= 12 && moderate(f.rGain) && moderate(f.bGain) && moderate(f.gCr) && moderate(f.gCb) && moderate(kg) &&
+           moderate(f.kgReciprocal / 65536.0f * 4.0f);
+}
+} // namespace
+
+// The description's conditions of the tuned float decode kernel (kernels_fast_decode.cu), in the order its launcher used
+// to check them; DecodeYccF32BlockInterior has the block's.
+bool DecodeYccF32Tuned(const DecodeParams& p)
+{
+    if (p.colorspace != AVIFGPU_COLORSPACE_YCBCR || p.hostDepth != 32 || (p.hasAlpha && p.premultiplied) || p.bitDepth > 12 || p.bitDepth <= 8)
+    {
+        return false;
+    }
+    if (p.transfer != AVIFGPU_TRANSFER_PQ && p.transfer != AVIFGPU_TRANSFER_HLG && p.transfer != AVIFGPU_TRANSFER_SMPTE428)
+    {
+        return false;
+    }
+    if (p.transfer == AVIFGPU_TRANSFER_HLG && !p.verifiedHlgDivisions)
+    {
+        return false; // the tuned kernel is built on the verified constant divisions; the generic kernel divides
+    }
+    if (p.transfer == AVIFGPU_TRANSFER_HLG && p.applyOotf && !avifmath::PowfStraightLineCovers(p.gammaMinusOne, false))
+    {
+        return false; // the tuned kernel's OOTF is the branch-free powf (device_math.cuh PowfStraightLine): moderate exponents only
+    }
+    if (p.transfer == AVIFGPU_TRANSFER_HLG && p.applyOotf &&
+        !(p.lumaR >= 0.0f && p.lumaG >= 0.0f && p.lumaB >= 0.0f && p.lumaR + p.lumaG + p.lumaB <= 2.5f))
+    {
+        return false; // the OOTF's luma must stay inside the kernel's log2 table (below 2.75) and non-negative
+    }
+    if (!avifmath::PowfStraightLineCovers(avifpix::PqConstants::inv_m2, true) || !avifmath::PowfStraightLineCovers(avifpix::PqConstants::inv_m1, true) ||
+        !avifmath::PowfStraightLineCovers(2.6f, true))
+    {
+        return false; // constants of the curves: cannot happen, but the kernel's powf rests on it
+    }
+    if (p.transfer != AVIFGPU_TRANSFER_HLG && !ChannelSumsStayNormal(p.bitDepth, F32DecodeFactorsOf(p.matrix), p.matrix.kg))
+    {
+        return false; // PQ's and SMPTE 428's branch-free powf takes +0 or NORMAL bases (the generic kernel has the full powf)
+    }
+    return true;
+}
+
+Interior DecodeYccF32Interior(const DecodeParams& p)
+{
+    return DecodeYccF32Tuned(p) ? DecodeYccF32BlockInterior(p) : Interior{ 0, 0 };
+}
+
+bool DecodeBatchTuned(const DecodeParams& p) { return p.hostDepth == 32 ? DecodeYccF32Tuned(p) : DecodeYccIntTuned(p); }
+
 namespace
 {
 // Adds image i's plan to `plan`: its interior and windows to the last chunk (a new one when that is full), or the image to
@@ -517,7 +587,7 @@ void PlanDecodeBatch(const DecodeParams& shared, int planeMask, const avifgpu_ba
 {
     plan->chunks.clear();
     plan->fallback.clear();
-    const bool tuned = DecodeYccIntTuned(shared);
+    const bool tuned = DecodeBatchTuned(shared);
     for (int32_t i = 0; i < count; ++i)
     {
         AddToBatch(PlanBatchDecodeImage(shared, tuned, planeMask, images[i]), i, plan);

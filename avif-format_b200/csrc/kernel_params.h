@@ -256,6 +256,47 @@ AVIFGPU_HD inline Interior DecodeYccIntBlockInterior(const DecodeParams& p)
 }
 Interior DecodeYccIntInterior(const DecodeParams& p); // DecodeYccIntTuned ? DecodeYccIntBlockInterior : none
 
+// The same for the tuned float YCbCr decode kernel (DecodeYccToRgbF32Kernel), split the same way.  The description's half:
+// 10/12-bit YCbCr (+ straight alpha) into 32-bit hosts with the PQ, HLG or SMPTE 428 curve; for HLG the context's verified
+// divisions, and with the OOTF an exponent and luma coefficients the branch-free powf covers; for PQ and SMPTE 428 a matrix
+// whose channel sums are never subnormal.  The block's half: a block starting on a 4:2:0 row pair, aligned buffers, equal
+// Cb and Cr strides, at least 4 x (1 << ys) pixels.  width is a multiple of 4, rows of 1 << ys.
+bool DecodeYccF32Tuned(const DecodeParams& p);
+AVIFGPU_HD inline Interior DecodeYccF32BlockInterior(const DecodeParams& p)
+{
+    const Interior none = { 0, 0 };
+    const int chromaAlign = p.xs ? 4 : 8;
+    if (p.yPhase != 0 || !Aligned(p.plane[0], p.planeStride[0], 8) || !Aligned(p.plane[1], p.planeStride[1], chromaAlign) ||
+        !Aligned(p.plane[2], p.planeStride[2], chromaAlign) || !Aligned(p.rows, p.rowStride, 16) || (p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], 8)))
+    {
+        return none;
+    }
+    if (p.planeStride[1] != p.planeStride[2])
+    {
+        return none; // the single-image kernel walks Cb and Cr with one offset
+    }
+    const int width4 = p.width & ~3;
+    const int evenRows = p.ys ? (p.rowCount & ~1) : p.rowCount;
+    if (width4 < 4 || evenRows < 1)
+    {
+        return none;
+    }
+    return Interior{ width4, evenRows };
+}
+Interior DecodeYccF32Interior(const DecodeParams& p); // DecodeYccF32Tuned ? DecodeYccF32BlockInterior : none
+
+// The description half of whichever tuned YCbCr decode kernel serves the description's host depth: the float one for
+// 32-bit hosts, the integer one otherwise.  Both batch APIs route by it.
+bool DecodeBatchTuned(const DecodeParams& p);
+
+// The pixel-independent factors of the float decode's channel sums, YuvDecode.cpp:555-557 and :308 -- the reference's
+// float expressions, evaluated once on the host without contraction (host_params.cpp).
+struct F32DecodeFactors
+{
+    float rGain, bGain, gCr, gCb, kgReciprocal;
+};
+F32DecodeFactors F32DecodeFactorsOf(const avifpix::InverseMatrix& matrix);
+
 // The strips CompleteEncode / CompleteDecode hand to the generic kernel around a block's interior, in their order: the
 // right strip [inner.width, width) x [0, rows), then the bottom strip [0, inner.width) x [inner.rows, rows).  Returns how
 // many of the two are non-empty; those come first in `strip`.
@@ -295,13 +336,16 @@ struct BatchRecord
 
 constexpr int kBatchChunkImages = 64;
 constexpr int kBatchUnitPixels = 256; // interior unit: 256 pixels of one row (row pair for 4:2:0), one warp
+constexpr int kF32BatchUnitPixels = 128; // the float decode's interior unit: its single-image kernel's 128-pixel tile
 constexpr int kBatchEdgeThreads = 256; // edge unit: one CTA-sized run of chroma sites (encode) or pixels (decode) of one row (pair)
 
 // Units of an interior of `width` x `rows` pixels, and of an edge window.
-AVIFGPU_HD inline int64_t BatchInteriorUnits(int width, int rows, int ys)
+AVIFGPU_HD inline int64_t BatchInteriorUnits(int width, int rows, int ys, int unitPixels = kBatchUnitPixels)
 {
-    return static_cast<int64_t>((width + kBatchUnitPixels - 1) / kBatchUnitPixels) * ((rows + ys) >> ys);
+    return static_cast<int64_t>((width + unitPixels - 1) / unitPixels) * ((rows + ys) >> ys);
 }
+// The interior unit width of a decode into `hostDepth`-bit hosts.
+AVIFGPU_HD inline int DecodeBatchUnitPixels(int hostDepth) { return hostDepth == 32 ? kF32BatchUnitPixels : kBatchUnitPixels; }
 AVIFGPU_HD inline int64_t BatchEdgeUnits(int width, int rows, int xs, int ys)
 {
     return static_cast<int64_t>((((width + xs) >> xs) + kBatchEdgeThreads - 1) / kBatchEdgeThreads) * ((rows + ys) >> ys);

@@ -10,6 +10,9 @@
 //                                 code; a CTA takes one run of 256 chroma sites at a time;
 //   DecodeYccToRgbIntBatchKernel  the decode interiors, with LoadYccUnit / ExpandYccUnit / StoreYccUnit (int_units.cuh);
 //                                 the unorm -> float tables are staged once per CTA for the whole batch (one description);
+//   DecodeYccToRgbF32BatchKernel  the float-host decode interiors, with LookUpLuma / ChromaSiteTerms / ConvertRows
+//                                 (float_units.cuh); a warp takes one 128-pixel tile of a row (4:2:0 row pair) at a time,
+//                                 and the libm, log2 and unorm tables are staged once per CTA for the whole batch;
 //   DecodeBatchKernel             the decode windows, with DecodeChunkPixel (generic_units.cuh).
 //
 // Each is a template on where its records come from:
@@ -22,6 +25,7 @@
 //                    its unit's record with a binary search (FindRecord), starting after the record of its previous unit.
 // Either way the search is once per unit and warp- (CTA-) uniform, never per pixel.
 #include "batch_plan.h"
+#include "float_units.cuh"
 #include "generic_units.cuh"
 #include "int_units.cuh"
 #include "kernel_params.h"
@@ -123,10 +127,13 @@ using RgbIntChunk = ChunkSource<Rgb16Params, kBatchChunkImages>;
 using PlanarChunk = ChunkSource<EncodeParams, 2 * kBatchChunkImages>;
 using YccIntChunk = ChunkSource<IntDecodeParams, kBatchChunkImages>;
 using DecodeEdgeChunk = ChunkSource<DecodeParams, 2 * kBatchChunkImages>;
+using YccF32Chunk = ChunkSource<FastDecodeParams, kBatchChunkImages>;
 
 // CUDA 12.1+ on Volta and later: at most 32764 bytes of kernel parameters.
 static_assert(sizeof(RgbIntChunk) <= 32764 && sizeof(PlanarChunk) <= 32764 && sizeof(YccIntChunk) <= 32764 && sizeof(DecodeEdgeChunk) <= 32764,
               "a chunk must fit one kernel parameter block");
+static_assert(sizeof(YccF32Chunk) <= 32764, "a float decode chunk must fit one kernel parameter block");
+static_assert(kF32DecodeThreads == kRgbThreads, "the batched kernels share kWarps");
 
 // Block-wide exclusive scan of a pair of counts over kPlanThreads threads; every thread gets the block's totals too.
 __device__ __forceinline__ void ScanPair(long long a, long long b, long long& beforeA, long long& beforeB, long long& totalA, long long& totalB)
@@ -382,6 +389,81 @@ __global__ void __launch_bounds__(kRgbThreads, kYccBlocksPerSm) DecodeYccToRgbIn
     }
 }
 
+// The single-image kernel's unit -- 128 pixels of a row, or of a row pair for 4:2:0, a lane on 4 pixels of each row -- with
+// 64-bit addresses from the unit's record instead of the 32-bit walk, and no software pipelining: the next unit may belong
+// to another image.  An interior is 4-pixel aligned, so a lane is wholly inside its row or wholly past its end.
+template <typename Source, int XS, int YS, int TRANSFER, int ALPHA, int FASTDIV>
+__global__ void __launch_bounds__(kF32DecodeThreads, kDecodeBlocksPerSm) DecodeYccToRgbF32BatchKernel(const __grid_constant__ Source s)
+{
+    const typename Source::Walk walk(s);
+    if (walk.Idle(static_cast<long long>(blockIdx.x) * kWarps))
+    {
+        return;
+    }
+    const int count = walk.Count();
+    constexpr int kRows = YS ? 2 : 1;
+    constexpr int kChromaPerRow = XS ? 2 : 4;
+    constexpr int kOutChannels = ALPHA ? 4 : 3;
+    extern __shared__ __align__(16) uint8_t sharedBytes[];
+    const F32Tables tables = StageF32Tables<TRANSFER, ALPHA>(sharedBytes, s.shared);
+    const uint32_t maxCodePair = s.shared.maxCode * 0x10001u;
+    const int lane = threadIdx.x & 31;
+    const long long warpCount = static_cast<long long>(gridDim.x) * kWarps;
+    int record = 0;
+#pragma unroll 1
+    for (long long unit = static_cast<long long>(blockIdx.x) * kWarps + (threadIdx.x >> 5); unit < walk.Units(); unit += warpCount)
+    {
+        record = walk.Find(count, record, unit);
+        const BatchRecord& r = walk.Record(record);
+        const int tilesX = (r.width + kF32TilePixels - 1) / kF32TilePixels;
+        const int local = static_cast<int>(unit - r.firstUnit);
+        const int unitRow = local / tilesX;
+        const int x = (local - unitRow * tilesX) * kF32TilePixels + lane * 4;
+        if (x >= r.width)
+        {
+            continue;
+        }
+        const int64_t y = static_cast<int64_t>(unitRow) * kRows;
+        uint2 yWords[kRows], aWords[kRows];
+        const uint8_t* yAddress = static_cast<const uint8_t*>(r.plane[0]) + y * r.planeStride[0] + x * 2;
+#pragma unroll
+        for (int k = 0; k < kRows; ++k)
+        {
+            yWords[k] = __ldg(reinterpret_cast<const uint2*>(yAddress + k * r.planeStride[0]));
+            aWords[k] = make_uint2(0u, 0u);
+        }
+        if (ALPHA)
+        {
+            const uint8_t* aAddress = static_cast<const uint8_t*>(r.plane[3]) + y * r.planeStride[3] + x * 2;
+#pragma unroll
+            for (int k = 0; k < kRows; ++k)
+            {
+                aWords[k] = __ldg(reinterpret_cast<const uint2*>(aAddress + k * r.planeStride[3]));
+            }
+        }
+        // chroma row unitRow (one per row, or per 4:2:0 row pair), sites from x >> XS: 2 (XS) or 4 codes
+        const int64_t chromaAt = static_cast<int64_t>(unitRow) * r.planeStride[1] + (x >> XS) * 2;
+        uint2 cbWords = make_uint2(0u, 0u), crWords = make_uint2(0u, 0u);
+        if (XS)
+        {
+            cbWords.x = __ldg(reinterpret_cast<const uint32_t*>(static_cast<const uint8_t*>(r.plane[1]) + chromaAt));
+            crWords.x = __ldg(reinterpret_cast<const uint32_t*>(static_cast<const uint8_t*>(r.plane[2]) + chromaAt));
+        }
+        else
+        {
+            cbWords = __ldg(reinterpret_cast<const uint2*>(static_cast<const uint8_t*>(r.plane[1]) + chromaAt));
+            crWords = __ldg(reinterpret_cast<const uint2*>(static_cast<const uint8_t*>(r.plane[2]) + chromaAt));
+        }
+        float Yf[kRows][4];
+        uint2 aPairs[kRows];
+        LookUpLuma<kRows>(yWords, aWords, maxCodePair, tables.sharedY, Yf, aPairs);
+        float rOffset[kChromaPerRow], bOffset[kChromaPerRow], gOffset[kChromaPerRow];
+        ChromaSiteTerms<XS>(s.shared, cbWords, crWords, maxCodePair, tables.sharedUV, rOffset, bOffset, gOffset);
+        uint8_t* target = static_cast<uint8_t*>(const_cast<void*>(r.rows)) + y * r.rowStride + static_cast<int64_t>(x) * kOutChannels * 4;
+        ConvertRows<XS, YS, TRANSFER, ALPHA, FASTDIV>(s.shared, Yf, aPairs, rOffset, bOffset, gOffset, target, r.rowStride, tables.sharedA, tables.t);
+    }
+}
+
 template <typename Source, typename PlaneT, typename HostT>
 __global__ void __launch_bounds__(kBatchEdgeThreads) DecodeBatchKernel(const __grid_constant__ Source s)
 {
@@ -480,10 +562,51 @@ void LaunchYccInt(const Source& s, const DecodeParams& d, unsigned grid, size_t 
     }
 }
 
+template <typename Source, int XS, int YS, int TRANSFER, int ALPHA, int FASTDIV>
+void LaunchYccF32One(const Source& s, unsigned grid, size_t bytes, cudaStream_t stream)
+{
+    static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
+    if (AllowDynamicShared(DecodeYccToRgbF32BatchKernel<Source, XS, YS, TRANSFER, ALPHA, FASTDIV>, kF32MaxTableBytes, configuredDevices) == cudaSuccess)
+    {
+        DecodeYccToRgbF32BatchKernel<Source, XS, YS, TRANSFER, ALPHA, FASTDIV><<<grid, kF32DecodeThreads, bytes, stream>>>(s);
+    } // else the failed attribute call is the error Launched() finds
+}
+
+template <typename Source, int TRANSFER, int ALPHA, int FASTDIV>
+void LaunchYccF32Chroma(const Source& s, int xs, int ys, unsigned grid, size_t bytes, cudaStream_t stream)
+{
+    if (xs == 1 && ys == 1) LaunchYccF32One<Source, 1, 1, TRANSFER, ALPHA, FASTDIV>(s, grid, bytes, stream);
+    else if (xs == 1) LaunchYccF32One<Source, 1, 0, TRANSFER, ALPHA, FASTDIV>(s, grid, bytes, stream);
+    else LaunchYccF32One<Source, 0, 0, TRANSFER, ALPHA, FASTDIV>(s, grid, bytes, stream);
+}
+
+template <typename Source, int TRANSFER, int FASTDIV = 0>
+void LaunchYccF32Alpha(const Source& s, const DecodeParams& d, unsigned grid, size_t bytes, cudaStream_t stream)
+{
+    if (d.hasAlpha) LaunchYccF32Chroma<Source, TRANSFER, 1, FASTDIV>(s, d.xs, d.ys, grid, bytes, stream);
+    else LaunchYccF32Chroma<Source, TRANSFER, 0, FASTDIV>(s, d.xs, d.ys, grid, bytes, stream);
+}
+
+// The float interior kernel of description `d` (transfer / verified PQ division x alpha x chroma), with `bytes` of staged
+// tables.  The single-image launcher's ladder: DecodeYccF32Tuned leaves PQ, HLG and SMPTE 428.
+template <typename Source>
+void LaunchYccF32(const Source& s, const DecodeParams& d, unsigned grid, size_t bytes, cudaStream_t stream)
+{
+    if (d.transfer == AVIFGPU_TRANSFER_PQ && d.verifiedPqRatio) LaunchYccF32Alpha<Source, AVIFGPU_TRANSFER_PQ, 1>(s, d, grid, bytes, stream);
+    else if (d.transfer == AVIFGPU_TRANSFER_PQ) LaunchYccF32Alpha<Source, AVIFGPU_TRANSFER_PQ, 0>(s, d, grid, bytes, stream);
+    else if (d.transfer == AVIFGPU_TRANSFER_HLG) LaunchYccF32Alpha<Source, AVIFGPU_TRANSFER_HLG>(s, d, grid, bytes, stream);
+    else LaunchYccF32Alpha<Source, AVIFGPU_TRANSFER_SMPTE428>(s, d, grid, bytes, stream);
+}
+
+// The float decode's tables for description `d`.
+size_t F32TableBytesOf(const DecodeParams& d) { return F32TableBytes(d.transfer, d.bitDepth, d.hasAlpha != 0); }
+
+// The windows run the generic kernel's instantiation for the host depth (LaunchDecodeGeneric's).
 template <typename Source>
 void LaunchDecodeEdge(const Source& s, int hostDepth, unsigned grid, cudaStream_t stream)
 {
-    if (hostDepth == 16) DecodeBatchKernel<Source, uint16_t, uint16_t><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
+    if (hostDepth == 32) DecodeBatchKernel<Source, uint16_t, float><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
+    else if (hostDepth == 16) DecodeBatchKernel<Source, uint16_t, uint16_t><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
     else DecodeBatchKernel<Source, uint8_t, uint8_t><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
 }
 
@@ -546,8 +669,17 @@ int LaunchDecodeBatchChunk(const DecodeParams& shared, const BatchChunk& chunk, 
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
     const int smCount = SmCountOrDefault(shared.smCount);
-    LaunchYccInt(ChunkOf<YccIntChunk>(IntDecodeShared(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared,
-                 GridFor((chunk.interiorUnits + kWarps - 1) / kWarps, static_cast<long long>(smCount) * kYccBlocksPerSm), YccTableBytesOf(shared), stream);
+    const long long warps = (chunk.interiorUnits + kWarps - 1) / kWarps; // one warp per unit
+    if (shared.hostDepth == 32)
+    {
+        LaunchYccF32(ChunkOf<YccF32Chunk>(FillF32Description(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared,
+                     GridFor(warps, static_cast<long long>(smCount) * kDecodeBlocksPerSm), F32TableBytesOf(shared), stream);
+    }
+    else
+    {
+        LaunchYccInt(ChunkOf<YccIntChunk>(IntDecodeShared(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared,
+                     GridFor(warps, static_cast<long long>(smCount) * kYccBlocksPerSm), YccTableBytesOf(shared), stream);
+    }
     const int interior = Launched(1);
     if (interior < 0 || chunk.windows == 0)
     {
@@ -597,8 +729,16 @@ int LaunchDecodeIndirect(const DecodeParams& shared, bool tuned, int planeMask, 
         return AVIFGPU_ERR_CUDA;
     }
     // A description the tuned kernel does not take plans no interior unit: its grid returns before staging, so it gets no tables.
-    LaunchYccInt(WorkspaceSource<IntDecodeParams, 0>{ IntDecodeShared(shared), workspace, maxCount }, shared,
-                 static_cast<unsigned>(smCount * kYccBlocksPerSm), tuned ? YccTableBytesOf(shared) : 0, stream);
+    if (shared.hostDepth == 32)
+    {
+        LaunchYccF32(WorkspaceSource<FastDecodeParams, 0>{ FillF32Description(shared), workspace, maxCount }, shared,
+                     static_cast<unsigned>(smCount * kDecodeBlocksPerSm), tuned ? F32TableBytesOf(shared) : 0, stream);
+    }
+    else
+    {
+        LaunchYccInt(WorkspaceSource<IntDecodeParams, 0>{ IntDecodeShared(shared), workspace, maxCount }, shared,
+                     static_cast<unsigned>(smCount * kYccBlocksPerSm), tuned ? YccTableBytesOf(shared) : 0, stream);
+    }
     if (Launched(1) < 0)
     {
         return AVIFGPU_ERR_CUDA;

@@ -50,7 +50,7 @@ extern "C" {
 #define AVIFGPU_EXPORT __attribute__((visibility("default")))
 #endif
 
-#define AVIFGPU_API_VERSION 7
+#define AVIFGPU_API_VERSION 8
 
 typedef enum avifgpu_status
 {
@@ -376,10 +376,12 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
                                                const avifgpu_batch_image* images, int32_t count, void* cuda_stream);
 
 /* The same for decodes: like `count` calls of avifgpu_decode_rows_device with y0 = 0 and nrows = height, one per image, in
- * order.  Images the tuned integer YCbCr decode takes in a direct call (8/16-bit hosts reading YCbCr 8/10/12-bit,
- * straight or no alpha, aligned buffers, width >= 8) go through chunks of up to 64 images, at most two launches per
- * chunk; every other image takes one direct call, after the chunks.  The first-use work (the verified divisions) is
- * done once per call, outside a capture. */
+ * order.  Images a tuned YCbCr decode takes in a direct call go through chunks of up to 64 images, at most two launches
+ * per chunk: the integer one (8/16-bit hosts reading YCbCr 8/10/12-bit, straight or no alpha, aligned buffers,
+ * width >= 8) and, since API version 8, the float one (32-bit hosts reading YCbCr 10/12-bit with PQ, HLG or SMPTE 428,
+ * straight or no alpha, aligned buffers, equal Cb / Cr strides, width >= 4; HLG once its divisions are verified).  Every
+ * other image -- monochrome, planar RGB, premultiplied alpha, 16-bit planes, a misaligned buffer -- takes one direct
+ * call, after the chunks.  The first-use work (the verified divisions) is done once per call, outside a capture. */
 AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
                                                const avifgpu_batch_image* images, int32_t count, void* cuda_stream);
 
@@ -399,8 +401,9 @@ AVIFGPU_EXPORT int avifgpu_batch_workspace_bytes(int32_t max_count, size_t* out_
  *   - Host checks, before any launch (each returns its status and launches nothing): ctx, desc, device_images,
  *     device_count or device_workspace NULL; desc invalid (validated as for the other calls, its size ignored);
  *     max_count outside [1, 4096]; workspace_bytes below avifgpu_batch_workspace_bytes(max_count).
- *   - Supported descriptions: encode, 8- or 16-bit RGB(A) hosts into planar YCbCr, any alpha state; decode, 8- or 16-bit
- *     hosts reading YCbCr with no or straight alpha.  Anything else is AVIFGPU_ERR_UNSUPPORTED, with no launch.
+ *   - Supported descriptions: encode, 8- or 16-bit RGB(A) hosts into planar YCbCr, any alpha state; decode, 8-, 16- or
+ *     (since API version 8) 32-bit hosts reading YCbCr with no or straight alpha.  Anything else is
+ *     AVIFGPU_ERR_UNSUPPORTED, with no launch.
  *   - Device-side checks.  With n = *device_count: n < 0 or n > max_count converts nothing and sets all max_count
  *     entries of device_status to AVIFGPU_ERR_BAD_PARAM.  Otherwise image i < n gets device_status[i] = 0, or
  *     AVIFGPU_ERR_BAD_PARAM when its width or height is negative, or when it is non-empty and its rows or a plane the
@@ -414,11 +417,11 @@ AVIFGPU_EXPORT int avifgpu_batch_workspace_bytes(int32_t max_count, size_t* out_
  *     addresses of the records, count, workspace and status array, not their contents: a replay converts whatever those
  *     buffers hold at that moment.
  *   - First-use work: an encode makes the premultiply check outside a capture; call avifgpu_prepare_decode before
- *     capturing a decode.  An encode captured before the check sends every image through the edge kernel: the same
- *     output bit for bit, a slower kernel.
+ *     capturing a decode.  An encode captured before the check, or an HLG decode into 32-bit hosts captured before its
+ *     divisions are verified, sends every image through the edge kernel: the same output bit for bit, a slower kernel.
  *   - Workspace: one workspace must not serve two calls that can be in flight at the same time.  The library allocates
  *     nothing for this call.
- * Images the tuned integer kernels take in a direct call have their aligned interior converted by the interior kernel,
+ * Images the tuned integer or float kernels take in a direct call have their aligned interior converted by the interior kernel,
  * their right strip and odd last 4:2:0 row by the edge kernel; every other image is one whole-image window of the edge
  * kernel, which runs the generic kernels' own per-site / per-pixel code.
  */

@@ -54,39 +54,16 @@ __device__ __forceinline__ uint32_t LookupCurveCode(uint32_t bits, const uint2* 
     return (word >> kBucketOffsetBits) + (offsetQ >= stepOffset ? 1u : 0u);
 }
 
-// Flat-table look-up (see CurveTableView::flat): `flat` is indexed by (bucket number - low), `span` = high - low.
-// Branch-free: ten integer/float instructions + one 64-bit shared-memory load, result as a float.  The bucket number
-// is taken with an ARITHMETIC shift, so every float with the sign bit set (negative values, -0, negative NaNs)
-// yields a negative index that the single add-clamp-to-[0, span] instruction (DPX) sends to the lowest bucket; that
-// bucket holds no step (.x = 0, so `bits < .x` is false) and decodes to code 0 exactly as the reference's
-// `value < 0 -> 0` / NaN -> 0 does.  +inf and the positive NaNs (bits > 0x7f7fffff) do NOT follow the steps; they
-// land in the top bucket (max code, never in band) and the caller must route them to ExactCurveCode itself.
-__device__ __forceinline__ float LookupCurveFlat(uint32_t bits, const uint2* __restrict__ flat, uint32_t shift, int32_t negativeLow, int32_t span,
-                                                 bool& inBand, uint2& entryOut)
-{
-    const int32_t index = __viaddmin_s32_relu(static_cast<int32_t>(bits) >> shift, negativeLow, span);
-    const uint2 entry = flat[index];
-    entryOut = entry;
-    const uint32_t distance = bits - entry.x;
-    inBand = distance < (entry.y & kFlatWidthMask);
-    float code;
-    asm("{ .reg .pred below; .reg .b32 upper; setp.lt.u32 below, %1, %2; and.b32 upper, %3, 0xfffff000; mov.b32 %0, upper; @below add.rn.f32 %0, %0, 0fBF800000; }"
-        : "=f"(code) : "r"(bits), "r"(entry.x), "r"(entry.y));
-    return code;
-}
-
-__device__ __forceinline__ float LookupCurveFlat(uint32_t bits, const uint2* __restrict__ flat, uint32_t shift, int32_t negativeLow, int32_t span,
-                                                 bool& inBand)
-{
-    uint2 entry;
-    return LookupCurveFlat(bits, flat, shift, negativeLow, span, inBand, entry);
-}
-
-// Compact look-up (curve_tables.h "Compact entries").  topShift = 32 - flatShift.
+// Compact look-up (curve_tables.h "Compact entries").  `compact` is indexed by (bucket number - low), `span` = high - low,
+// topShift = 32 - flatShift.  The bucket number is taken with an ARITHMETIC shift, so every float with the sign bit set
+// (negative values, -0, negative NaNs) yields a negative index that the single add-clamp-to-[0, span] instruction (DPX)
+// sends to the lowest bucket; that bucket holds no step and decodes to code 0 exactly as the reference's
+// `value < 0 -> 0` / NaN -> 0 does.  +inf and the positive NaNs (bits > 0x7f7fffff) do NOT follow the steps; they land in
+// the top bucket and the caller must route them to ExactCurveCode itself.
 // SHIFT != 0 fixes flatShift at compile time (the shifts become immediates and entry + (bits << topShift) a single
 // multiply-add on the FMA pipe); `magic` is 0x4b000000 handed in as a run-time value so that (entry & codeMask) | magic
 // stays ONE three-input logic instruction.  Eleven instructions and one 32-bit shared-memory load per sample; the code
-// comes out as a float like LookupCurveFlat's.
+// comes out as a float (the forward matrix wants floats).
 template <int SHIFT>
 __device__ __forceinline__ float LookupCurveCompact(uint32_t bits, const uint32_t* __restrict__ compact, uint32_t shift, int32_t negativeLow, int32_t span,
                                                     uint32_t topShift, uint32_t codeMask, uint32_t magic, bool& inBand, uint32_t& entryOut)
@@ -124,7 +101,8 @@ __device__ __forceinline__ uint32_t ResolveCompactInBand(uint32_t bits, uint32_t
     return ((word >> (index & 31u)) & 1u) ? k : k - 1u;
 }
 
-// Complete compact look-up for one finite sample (verifier).
+// Complete compact look-up for one finite sample, bitmap included (the verifier, and the generic kernel from global
+// memory; the tuned kernels inline the same steps around their own batching).
 __device__ __forceinline__ uint32_t LookupCurveCodeCompactResolved(uint32_t bits, const CurveTableView& table, bool& inBand)
 {
     const uint32_t topShift = 32u - table.flatShift;
@@ -136,30 +114,6 @@ __device__ __forceinline__ uint32_t LookupCurveCodeCompactResolved(uint32_t bits
     if (inBand)
     {
         result = ResolveCompactInBand(bits, entry, result, topShift, table.compactCodeMask, table.firstBits, table.bandBits, table.bandStrideLog2);
-    }
-    return result;
-}
-
-// Position of an in-band sample's bit in CurveTableView::bandBits (entry = the sample's flat entry).
-__device__ __forceinline__ uint32_t BandBitIndex(uint32_t bits, const uint2 entry, uint32_t strideLog2)
-{
-    const uint32_t k = static_cast<uint32_t>(__float2int_rz(__uint_as_float(entry.y & ~kFlatWidthMask)));
-    return (k << strideLog2) + (bits - entry.x);
-}
-
-// Complete flat look-up for one finite sample, bitmap included (used by the verifier; the conversion kernel inlines
-// the same steps around its own batching).
-__device__ __forceinline__ uint32_t LookupCurveCodeFlatResolved(uint32_t bits, const CurveTableView& table, bool& inBand)
-{
-    uint2 entry;
-    const float code = LookupCurveFlat(bits, table.flat, table.flatShift, -static_cast<int32_t>(table.flatLow),
-                                       static_cast<int32_t>(table.flatHigh - table.flatLow), inBand, entry);
-    uint32_t result = static_cast<uint32_t>(code);
-    if (inBand)
-    {
-        const uint32_t bitIndex = BandBitIndex(bits, entry, table.bandStrideLog2);
-        const uint32_t word = table.bandBits[bitIndex >> 5];
-        result -= ((word >> (bitIndex & 31u)) & 1u) ^ 1u;
     }
     return result;
 }

@@ -6,7 +6,6 @@
 
 #include <algorithm>
 #include <chrono>
-#include <cstring>
 #include <vector>
 
 namespace avifgpu
@@ -53,7 +52,8 @@ __global__ void __launch_bounds__(kSweepThreads) SweepKernel(float pqMultiplier,
     }
 }
 
-// Pass 2: every input again, table against exact.  counters[0] = mismatches outside bands, [1] = inputs in bands.
+// Pass 2: every input again, both tables against exact.  counters[0] = mismatches (two-level outside its bands, compact
+// everywhere finite), [1] = inputs in the two-level table's bands, [2] = inputs the compact table flags.
 template <int CURVE>
 __global__ void __launch_bounds__(kSweepThreads) VerifyKernel(float pqMultiplier, float maxCodeFloat, CurveTableView table,
                                                              unsigned long long* __restrict__ counters)
@@ -64,7 +64,6 @@ __global__ void __launch_bounds__(kSweepThreads) VerifyKernel(float pqMultiplier
 
     unsigned long long mismatches = 0;
     unsigned long long inBandCount = 0;
-    unsigned long long flatInBand = 0;
     unsigned long long compactInBand = 0;
     // +inf and the positive NaNs are part of the check (bits up to 0x7fffffff): they must come out as code 0.
     const uint64_t total = 0x80000000ull;
@@ -74,34 +73,18 @@ __global__ void __launch_bounds__(kSweepThreads) VerifyKernel(float pqMultiplier
         const uint32_t bits = static_cast<uint32_t>(u);
         bool inBand;
         uint32_t fast = LookupCurveCode(bits, table.octaves, table.buckets, inBand);
-        if (table.flat != nullptr)
+        // The compact variant, band bitmap included, must reproduce the exact curve for every finite input;
+        // +inf / NaN are the caller's to route to the exact evaluation (curve_lookup.cuh).
+        if (table.compact != nullptr && bits <= 0x7f7fffffu)
         {
-            // The flat variant, band bitmap included, must reproduce the exact curve for every finite input;
-            // +inf / NaN are the caller's to route to the exact evaluation (curve_lookup.cuh).
-            if (bits <= 0x7f7fffffu)
+            bool inBandCompact;
+            if (LookupCurveCodeCompactResolved(bits, table, inBandCompact) != ExactCurveCode<CURVE>(__uint_as_float(bits), pqMultiplier, maxCodeFloat, t))
             {
-                bool inBandFlat;
-                const uint32_t fastFlat = LookupCurveCodeFlatResolved(bits, table, inBandFlat);
-                if (fastFlat != ExactCurveCode<CURVE>(__uint_as_float(bits), pqMultiplier, maxCodeFloat, t))
-                {
-                    ++mismatches;
-                }
-                if (inBandFlat)
-                {
-                    ++flatInBand;
-                }
-                if (table.compact != nullptr)
-                {
-                    bool inBandCompact;
-                    if (LookupCurveCodeCompactResolved(bits, table, inBandCompact) != ExactCurveCode<CURVE>(__uint_as_float(bits), pqMultiplier, maxCodeFloat, t))
-                    {
-                        ++mismatches;
-                    }
-                    if (inBandCompact)
-                    {
-                        ++compactInBand;
-                    }
-                }
+                ++mismatches;
+            }
+            if (inBandCompact)
+            {
+                ++compactInBand;
             }
         }
         if (inBand)
@@ -117,15 +100,13 @@ __global__ void __launch_bounds__(kSweepThreads) VerifyKernel(float pqMultiplier
     {
         mismatches += __shfl_down_sync(0xffffffffu, mismatches, offset);
         inBandCount += __shfl_down_sync(0xffffffffu, inBandCount, offset);
-        flatInBand += __shfl_down_sync(0xffffffffu, flatInBand, offset);
         compactInBand += __shfl_down_sync(0xffffffffu, compactInBand, offset);
     }
     if ((threadIdx.x & 31) == 0)
     {
         if (mismatches) atomicAdd(&counters[0], mismatches);
         if (inBandCount) atomicAdd(&counters[1], inBandCount);
-        if (flatInBand) atomicAdd(&counters[2], flatInBand);
-        if (compactInBand) atomicAdd(&counters[3], compactInBand);
+        if (compactInBand) atomicAdd(&counters[2], compactInBand);
     }
 }
 
@@ -170,13 +151,6 @@ struct Step
     uint32_t k;
 };
 
-uint32_t FloatBits(float v)
-{
-    uint32_t bits;
-    std::memcpy(&bits, &v, sizeof bits);
-    return bits;
-}
-
 bool Check(cudaError_t e, const char* what, std::string* error)
 {
     if (e == cudaSuccess)
@@ -193,7 +167,6 @@ void FreeCurveTable(CurveTable* table)
 {
     if (table->deviceOctaves) cudaFree(table->deviceOctaves);
     if (table->deviceBuckets) cudaFree(table->deviceBuckets);
-    if (table->deviceFlat) cudaFree(table->deviceFlat);
     if (table->deviceBandBits) cudaFree(table->deviceBandBits);
     if (table->deviceCompact) cudaFree(table->deviceCompact);
     if (table->deviceFirstBits) cudaFree(table->deviceFirstBits);
@@ -201,7 +174,6 @@ void FreeCurveTable(CurveTable* table)
     table->deviceFirstBits = nullptr;
     table->deviceOctaves = nullptr;
     table->deviceBuckets = nullptr;
-    table->deviceFlat = nullptr;
     table->deviceBandBits = nullptr;
     table->valid = false;
 }
@@ -411,14 +383,13 @@ bool BuildCurveTable(int curve, int param, int depth, void* streamHandle, CurveT
         return false;
     }
 
-    // ---- flat variant ----------------------------------------------------------------------------------------
-    std::vector<uint2> flat;
+    // ---- compact variant (curve_tables.h "Compact entries") -----------------------------------------------------
     std::vector<uint32_t> compact;
-    std::vector<uint3> flatBands; // {first, width, k} of every step with a fuzzy band
+    std::vector<uint3> bands; // {first, width, k} of every step with a fuzzy band
     uint32_t flatShift = 0, flatLow = 0, flatHigh = 0, bandStrideLog2 = 5;
     if (!steps.empty())
     {
-        int shift = static_cast<int>(kFlatMaxShift);
+        int shift = static_cast<int>(std::min(kFlatMaxShift, 32u - static_cast<uint32_t>(depth) - kCompactLenBits));
         for (; shift >= kMinShift; --shift)
         {
             bool separated = true;
@@ -438,110 +409,68 @@ bool BuildCurveTable(int curve, int param, int depth, void* streamHandle, CurveT
             flatLow = (steps.front().first >> shift) - 1u;
             flatHigh = (steps.back().end >> shift) + 1u;
             const uint64_t count = static_cast<uint64_t>(flatHigh) - flatLow + 1u;
-            usable = count * sizeof(uint2) <= kFlatMaxBytes && (static_cast<uint64_t>(flatHigh + 1u) << shift) <= kSweepEnd;
-            if (usable)
+            usable = count * sizeof(uint32_t) <= kFlatMaxBytes && (static_cast<uint64_t>(flatHigh + 1u) << shift) <= kSweepEnd;
+            const uint32_t topShift = 32u - static_cast<uint32_t>(shift);
+            const uint32_t lenMax = (1u << kCompactLenBits) - 1u;
+            const uint32_t unitLog2 = static_cast<uint32_t>(shift) - kCompactLenBits; // flatShift >= kMinShift = 6
+            compact.resize(usable ? count : 0);
+            size_t at = 0;
+            for (uint64_t b = 0; b < compact.size() && usable; ++b)
             {
-                flat.resize(count);
-                size_t next = 0;
-                for (uint64_t b = 0; b < count; ++b)
+                const uint64_t bLo = (static_cast<uint64_t>(flatLow) + b) << shift;
+                const uint64_t bHi = bLo + (1ull << shift);
+                while (at < steps.size() && steps[at].end < bLo)
                 {
-                    const uint64_t bLo = (static_cast<uint64_t>(flatLow) + b) << shift;
-                    const uint64_t bHi = bLo + (1ull << shift);
-                    while (next < steps.size() && steps[next].end < bLo)
+                    ++at;
+                }
+                uint32_t top = 0, field, inBandFloats = 0;
+                if (at < steps.size() && steps[at].first < bHi)
+                {
+                    const Step& step = steps[at];
+                    const bool banded = step.end > step.first;
+                    if (step.first > bLo)
                     {
-                        ++next;
-                    }
-                    if (next < steps.size() && steps[next].first < bHi)
-                    {
-                        // the bucket meets step `next`: its start, its band, or the tail of its band.  Samples in
-                        // [first, end] are in band when the step has a fuzzy band (end > first).
-                        const uint32_t bandWidth = steps[next].end > steps[next].first ? (steps[next].end - steps[next].first + 1u) : 0u;
-                        usable = usable && bandWidth <= kFlatWidthMask;
-                        flat[b] = make_uint2(steps[next].first, FloatBits(static_cast<float>(steps[next].k)) | bandWidth);
+                        // the step starts inside this bucket: code = (k - 1) + carry
+                        top = static_cast<uint32_t>((1ull << shift) - (step.first - bLo));
+                        field = step.k - 1u;
+                        inBandFloats = banded ? static_cast<uint32_t>(std::min<uint64_t>(step.end, bHi - 1) - step.first + 1u) : 0u;
                     }
                     else
                     {
-                        flat[b] = make_uint2(0u, FloatBits(static_cast<float>(next))); // no step: code = steps below
+                        // the step sits exactly on the bucket start, or this is the tail of a band that began in the
+                        // previous bucket: every float here is at or above first_k
+                        field = step.k;
+                        inBandFloats = banded ? static_cast<uint32_t>(std::min<uint64_t>(step.end, bHi - 1) - bLo + 1u) : 0u;
                     }
                 }
-                for (const Step& s : steps)
+                else
                 {
-                    if (s.end > s.first)
-                    {
-                        const uint32_t width = s.end - s.first + 1u;
-                        flatBands.push_back(make_uint3(s.first, width, s.k));
-                        while ((1u << bandStrideLog2) < width)
-                        {
-                            ++bandStrideLog2;
-                        }
-                    }
+                    field = static_cast<uint32_t>(at); // no step: code = steps below
                 }
-                usable = usable && ((static_cast<uint64_t>(codeCount) << bandStrideLog2) / 8u) <= kBandBitmapMaxBytes;
-                // ---- compact variant (curve_tables.h "Compact entries") over the same buckets
-                if (usable && static_cast<uint32_t>(shift) + static_cast<uint32_t>(depth) + kCompactLenBits <= 32u)
+                const uint32_t lenq = (inBandFloats + (1u << unitLog2) - 1u) >> unitLog2;
+                usable = lenq <= lenMax && field <= maxCode;
+                compact[b] = (top << topShift) | (field << kCompactLenBits) | lenq;
+            }
+            // the band bitmap answers bits - first_k < 2^stride for every banded step: a band rounded up to the unit (plus
+            // the part of it that lies in the previous bucket) must stay inside it
+            while (usable && (1u << bandStrideLog2) < table->stats.widestBand + (2u << unitLog2))
+            {
+                ++bandStrideLog2;
+            }
+            usable = usable && ((static_cast<uint64_t>(codeCount) << bandStrideLog2) / 8u) <= kBandBitmapMaxBytes;
+        }
+        if (usable)
+        {
+            for (const Step& s : steps)
+            {
+                if (s.end > s.first)
                 {
-                    const uint32_t topShift = 32u - static_cast<uint32_t>(shift);
-                    const uint32_t lenMax = (1u << kCompactLenBits) - 1u;
-                    const uint32_t unitLog2 = static_cast<uint32_t>(shift) - kCompactLenBits; // flatShift >= kMinShift = 6
-                    uint32_t longest = 0;
-                    bool fits = true;
-                    compact.resize(count);
-                    size_t at = 0;
-                    for (uint64_t b = 0; b < count && fits; ++b)
-                    {
-                        const uint64_t bLo = (static_cast<uint64_t>(flatLow) + b) << shift;
-                        const uint64_t bHi = bLo + (1ull << shift);
-                        while (at < steps.size() && steps[at].end < bLo)
-                        {
-                            ++at;
-                        }
-                        uint32_t top = 0, field, inBandFloats = 0;
-                        if (at < steps.size() && steps[at].first < bHi)
-                        {
-                            const Step& step = steps[at];
-                            const bool banded = step.end > step.first;
-                            if (step.first > bLo)
-                            {
-                                // the step starts inside this bucket: code = (k - 1) + carry
-                                top = static_cast<uint32_t>((1ull << shift) - (step.first - bLo));
-                                field = step.k - 1u;
-                                inBandFloats = banded ? static_cast<uint32_t>(std::min<uint64_t>(step.end, bHi - 1) - step.first + 1u) : 0u;
-                            }
-                            else
-                            {
-                                // the step sits exactly on the bucket start, or this is the tail of a band that began in the
-                                // previous bucket: every float here is at or above first_k
-                                field = step.k;
-                                inBandFloats = banded ? static_cast<uint32_t>(std::min<uint64_t>(step.end, bHi - 1) - bLo + 1u) : 0u;
-                            }
-                        }
-                        else
-                        {
-                            field = static_cast<uint32_t>(at); // no step: code = steps below
-                        }
-                        const uint32_t lenq = (inBandFloats + (1u << unitLog2) - 1u) >> unitLog2;
-                        fits = lenq <= lenMax && field <= maxCode;
-                        longest = std::max(longest, lenq << unitLog2);
-                        compact[b] = (top << topShift) | (field << kCompactLenBits) | lenq;
-                    }
-                    // the band bitmap answers bits - first_k < 2^stride for every banded step: a band rounded up to the unit (plus
-                    // the part of it that lies in the previous bucket) must stay inside it
-                    (void)longest;
-                    while (fits && (1u << bandStrideLog2) < table->stats.widestBand + (2u << unitLog2))
-                    {
-                        ++bandStrideLog2;
-                    }
-                    fits = fits && ((static_cast<uint64_t>(codeCount) << bandStrideLog2) / 8u) <= kBandBitmapMaxBytes;
-                    if (!fits)
-                    {
-                        compact.clear();
-                    }
+                    bands.push_back(make_uint3(s.first, s.end - s.first + 1u, s.k));
                 }
             }
         }
-        if (!usable)
+        else
         {
-            flat.clear();
             compact.clear();
         }
     }
@@ -556,7 +485,6 @@ bool BuildCurveTable(int curve, int param, int depth, void* streamHandle, CurveT
     table->view.octaves = static_cast<const uint2*>(table->deviceOctaves);
     table->view.buckets = static_cast<const uint32_t*>(table->deviceBuckets);
     table->view.bucketCount = static_cast<int32_t>(buckets.size());
-    table->view.flat = nullptr;
     table->view.flatCount = 0;
     table->view.bandBits = nullptr;
     table->view.bandStrideLog2 = 0;
@@ -565,33 +493,21 @@ bool BuildCurveTable(int curve, int param, int depth, void* streamHandle, CurveT
     table->view.compactImageBytes = 0;
     table->view.compactCodeMask = 0;
     table->view.compactMagic = 0;
-    if (!flat.empty())
+    if (!compact.empty())
     {
-        if (!Check(cudaMalloc(&table->deviceFlat, (flat.size() + 1) * sizeof(uint2)), "cudaMalloc", &table->error) ||
-            !Check(cudaMemcpyAsync(table->deviceFlat, flat.data(), flat.size() * sizeof(uint2), cudaMemcpyHostToDevice, stream), "H2D", &table->error))
-        {
-            FreeCurveTable(table);
-            return false;
-        }
-        table->view.flat = static_cast<const uint2*>(table->deviceFlat);
-        table->view.flatCount = static_cast<int32_t>(flat.size());
-        table->view.flatShift = flatShift;
-        table->view.flatLow = flatLow;
-        table->view.flatHigh = flatHigh;
-
         // Band bitmap: the exact answer for every in-band float, one bit each, at (k << stride) + (bits - first_k).
         const size_t bitmapBytes = (codeCount << bandStrideLog2) / 8u;
         uint3* dBands = nullptr;
         bool filled = Check(cudaMalloc(&table->deviceBandBits, bitmapBytes), "cudaMalloc", &table->error) &&
                       Check(cudaMemsetAsync(table->deviceBandBits, 0, bitmapBytes, stream), "memset", &table->error);
-        if (filled && !flatBands.empty())
+        if (filled && !bands.empty())
         {
-            filled = Check(cudaMalloc(&dBands, flatBands.size() * sizeof(uint3)), "cudaMalloc", &table->error) &&
-                     Check(cudaMemcpyAsync(dBands, flatBands.data(), flatBands.size() * sizeof(uint3), cudaMemcpyHostToDevice, stream), "H2D", &table->error);
+            filled = Check(cudaMalloc(&dBands, bands.size() * sizeof(uint3)), "cudaMalloc", &table->error) &&
+                     Check(cudaMemcpyAsync(dBands, bands.data(), bands.size() * sizeof(uint3), cudaMemcpyHostToDevice, stream), "H2D", &table->error);
             if (filled)
             {
                 uint32_t* bitsOut = static_cast<uint32_t*>(table->deviceBandBits);
-                const int bandCount = static_cast<int>(flatBands.size());
+                const int bandCount = static_cast<int>(bands.size());
                 if (curve == kCurveLinearToPQ)
                 {
                     FillBandBitsKernel<kCurveLinearToPQ><<<grid, kSweepThreads, 0, stream>>>(pqMultiplier, maxCodeFloat, dBands, bandCount, bandStrideLog2, bitsOut);
@@ -608,46 +524,43 @@ bool BuildCurveTable(int curve, int param, int depth, void* streamHandle, CurveT
             }
             cudaFree(dBands);
         }
-        if (!filled)
+        std::vector<uint32_t> firstBits(codeCount + 1, 0u);
+        for (const Step& step : steps)
+        {
+            firstBits[step.k] = step.first;
+        }
+        // one allocation = the kernels' shared-memory image (CurveTableView::compactImageBytes)
+        const size_t paddedCompact = (compact.size() + 3u) & ~static_cast<size_t>(3u);
+        const size_t paddedFirst = (firstBits.size() + 3u) & ~static_cast<size_t>(3u);
+        std::vector<uint32_t> image(paddedCompact + paddedFirst, 0u);
+        std::copy(compact.begin(), compact.end(), image.begin());
+        std::copy(firstBits.begin(), firstBits.end(), image.begin() + static_cast<std::ptrdiff_t>(paddedCompact));
+        if (!filled ||
+            !Check(cudaMalloc(&table->deviceCompact, image.size() * sizeof(uint32_t)), "cudaMalloc", &table->error) ||
+            !Check(cudaMemcpyAsync(table->deviceCompact, image.data(), image.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), "H2D", &table->error) ||
+            !Check(cudaStreamSynchronize(stream), "compact table upload", &table->error))
         {
             FreeCurveTable(table);
             return false;
         }
+        table->view.flatCount = static_cast<int32_t>(compact.size());
+        table->view.flatShift = flatShift;
+        table->view.flatLow = flatLow;
+        table->view.flatHigh = flatHigh;
         table->view.bandBits = static_cast<const uint32_t*>(table->deviceBandBits);
         table->view.bandStrideLog2 = bandStrideLog2;
+        table->view.compact = static_cast<const uint32_t*>(table->deviceCompact);
+        table->view.firstBits = table->view.compact + paddedCompact;
+        table->view.compactImageBytes = static_cast<uint32_t>(image.size() * sizeof(uint32_t));
+        table->view.compactCodeMask = maxCode << kCompactLenBits;
+        table->view.compactMagic = 0x4b000000u;
         table->stats.bandBitmapBytes = bitmapBytes;
-        if (!compact.empty())
-        {
-            std::vector<uint32_t> firstBits(codeCount + 1, 0u);
-            for (const Step& step : steps)
-            {
-                firstBits[step.k] = step.first;
-            }
-            // one allocation = the kernels' shared-memory image (CurveTableView::compactImageBytes)
-            const size_t paddedCompact = (compact.size() + 3u) & ~static_cast<size_t>(3u);
-            const size_t paddedFirst = (firstBits.size() + 3u) & ~static_cast<size_t>(3u);
-            std::vector<uint32_t> image(paddedCompact + paddedFirst, 0u);
-            std::copy(compact.begin(), compact.end(), image.begin());
-            std::copy(firstBits.begin(), firstBits.end(), image.begin() + static_cast<std::ptrdiff_t>(paddedCompact));
-            if (!Check(cudaMalloc(&table->deviceCompact, image.size() * sizeof(uint32_t)), "cudaMalloc", &table->error) ||
-                !Check(cudaMemcpyAsync(table->deviceCompact, image.data(), image.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), "H2D", &table->error) ||
-                !Check(cudaStreamSynchronize(stream), "compact table upload", &table->error))
-            {
-                FreeCurveTable(table);
-                return false;
-            }
-            table->view.compact = static_cast<const uint32_t*>(table->deviceCompact);
-            table->view.firstBits = table->view.compact + paddedCompact;
-            table->view.compactImageBytes = static_cast<uint32_t>(image.size() * sizeof(uint32_t));
-            table->view.compactCodeMask = maxCode << kCompactLenBits;
-            table->view.compactMagic = 0x4b000000u;
-            table->stats.compactBuckets = static_cast<int32_t>(compact.size());
-        }
+        table->stats.compactBuckets = static_cast<int32_t>(compact.size());
     }
     unsigned long long* dCounters = nullptr;
     ok = Check(cudaMemcpyAsync(table->deviceOctaves, octaves.data(), octaves.size() * sizeof(uint2), cudaMemcpyHostToDevice, stream), "H2D", &table->error) &&
          Check(cudaMemcpyAsync(table->deviceBuckets, buckets.data(), buckets.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), "H2D", &table->error) &&
-         Check(cudaMalloc(&dCounters, 4 * sizeof(unsigned long long)), "cudaMalloc", &table->error);
+         Check(cudaMalloc(&dCounters, 3 * sizeof(unsigned long long)), "cudaMalloc", &table->error);
     if (!ok)
     {
         FreeCurveTable(table);
@@ -655,7 +568,7 @@ bool BuildCurveTable(int curve, int param, int depth, void* streamHandle, CurveT
     }
 
     // ---- pass 2: verify every input ---------------------------------------------------------------------------
-    cudaMemsetAsync(dCounters, 0, 4 * sizeof(unsigned long long), stream);
+    cudaMemsetAsync(dCounters, 0, 3 * sizeof(unsigned long long), stream);
     if (curve == kCurveLinearToPQ)
     {
         VerifyKernel<kCurveLinearToPQ><<<grid, kSweepThreads, 0, stream>>>(pqMultiplier, maxCodeFloat, table->view, dCounters);
@@ -668,7 +581,7 @@ bool BuildCurveTable(int curve, int param, int depth, void* streamHandle, CurveT
     {
         VerifyKernel<kCurveLinearToHLG><<<grid, kSweepThreads, 0, stream>>>(pqMultiplier, maxCodeFloat, table->view, dCounters);
     }
-    unsigned long long counters[4] = { 0, 0, 0, 0 };
+    unsigned long long counters[3] = { 0, 0, 0 };
     ok = Check(cudaMemcpyAsync(counters, dCounters, sizeof(counters), cudaMemcpyDeviceToHost, stream), "D2H", &table->error) &&
          Check(cudaStreamSynchronize(stream), "curve verify", &table->error);
     cudaFree(dCounters);
@@ -679,9 +592,7 @@ bool BuildCurveTable(int curve, int param, int depth, void* streamHandle, CurveT
     }
     table->stats.verifyMismatches = counters[0];
     table->stats.inBandInputs = counters[1];
-    table->stats.flatInBandInputs = counters[2];
-    table->stats.compactInBandInputs = counters[3];
-    table->stats.flatBuckets = table->view.flatCount;
+    table->stats.compactInBandInputs = counters[2];
     table->stats.buildMilliseconds = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     if (counters[0] != 0)
     {

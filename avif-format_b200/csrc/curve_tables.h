@@ -16,13 +16,13 @@
 //   * the conversion kernel does two shared-memory look-ups and a handful of integer instructions per sample;
 //     samples that fall inside a (conservatively widened) band are handed to the exact evaluation (rare for the
 //     curves that need this form: a single powf is monotone, so only the quantisation of the table itself widens);
-//   * the flat variant (one bucket size for all binades, PQ) goes one step further: inside the band of step k the exact code is k-1 or k (neighbouring
-//     bands never overlap, the builder checks), so ONE BIT per in-band float records the exact answer.  A fill
-//     kernel evaluates the exact curve for every in-band float (a few million) into a bitmap that lives in L2
-//     (1 MB for 12 bits); the conversion kernel resolves an in-band sample with one 32-bit load instead of ~150
-//     instructions of glibc-exact powf;
-//   * a verification kernel then re-sweeps every float and checks table (+ bitmap) == exact; a table that
-//     fails (it never has) is discarded and the generic kernel keeps serving that configuration.
+//   * the compact variant (one bucket size for all binades, one 32-bit word per bucket, PQ) goes one step further:
+//     inside the band of step k the exact code is k-1 or k (neighbouring bands never overlap, the builder checks), so
+//     ONE BIT per in-band float records the exact answer.  A fill kernel evaluates the exact curve for every in-band
+//     float (a few million) into a bitmap that lives in L2 (up to 2 MB for 12 bits); the conversion kernel resolves an
+//     in-band sample with one 32-bit load instead of ~150 instructions of glibc-exact powf;
+//   * a verification kernel then re-sweeps every float through both forms and checks table (+ bitmap) == exact; a
+//     table that fails (it never has) is discarded and the generic kernel keeps serving that configuration.
 //
 // Nothing here approximates: every output is either decided by a threshold derived from the exact curve, read from
 // a bit the exact curve wrote, or is the exact curve itself.
@@ -49,20 +49,13 @@ constexpr uint32_t kBucketOffsetBits = 20;          // low bits of a bucket word
 constexpr uint32_t kBucketOffsetNone = 1u << 19;    // "no step in this bucket": every offset compares below it
 constexpr uint32_t kOffsetResolutionBits = 19;      // offsets inside a bucket are kept to 19 bits
 
-// Flat (single-level) variant, used when one bucket size separates the steps of every binade and the table
-// still fits in shared memory (true for PQ): buckets of 2^flatShift floats covering bit patterns
-// [flatLow << flatShift, (flatHigh + 1) << flatShift); inputs outside are clamped to the end buckets, which
-// hold no step.  One 64-bit entry per bucket:
-//     .x = bit pattern of the step's band start (first_k), 0 when the bucket meets no step
-//     .y = bit pattern of (float)kUpper | bandWidth   (kUpper < 2^12 leaves the low 12 mantissa bits free;
-//          bandWidth = number of in-band floats from first_k on, < 2^12)
-// code = kUpper - (bits < .x), delivered as a float (the forward matrix wants floats); the sample is in band iff
-// 0 <= bits - .x < bandWidth, and then bit ((kUpper << bandStrideLog2) + bits - .x) of bandBits says whether the
-// exact code is kUpper (1) or kUpper - 1 (0).
+// Compact (single-level) variant, used when one bucket size separates the steps of every binade (true for PQ):
+// buckets of 2^flatShift floats covering bit patterns [flatLow << flatShift, (flatHigh + 1) << flatShift); inputs
+// outside are clamped to the end buckets, which hold no step.  flatShift is the largest shift up to kFlatMaxShift that
+// separates the steps, capped at 32 - depth - kCompactLenBits so that an entry fits one word (a shift that separates
+// the steps separates them at every smaller shift too).  The entries are at most kFlatMaxBytes.
 constexpr uint32_t kFlatMaxShift = 16;
 constexpr uint32_t kFlatMaxBytes = 132 * 1024;
-constexpr uint32_t kFlatWidthBits = 12;
-constexpr uint32_t kFlatWidthMask = (1u << kFlatWidthBits) - 1u;
 constexpr uint64_t kBandBitmapMaxBytes = 8ull << 20;
 
 // Device-resident table (global memory; kernels stage it into shared memory).
@@ -70,16 +63,15 @@ struct CurveTableView
 {
     const uint2* octaves;     // 256 entries: .x = first bucket index, .y = S | r << 8 | wq << 16
     const uint32_t* buckets;  // bucketCount words: (k-1) << 20 | offset
-    int32_t bucketCount;
-    const uint2* flat;        // flatCount entries, or nullptr when the flat variant does not apply
-    int32_t flatCount;
+    // flatCount / flatShift and flatLow / flatHigh are 8-byte aligned pairs: a kernel reads each pair with one load.
+    int32_t flatCount;        // compact entries
     uint32_t flatShift;
-    uint32_t flatLow;         // bucket number (bits >> flatShift) of flat[0]
-    uint32_t flatHigh;        // bucket number of flat[flatCount - 1]
+    uint32_t flatLow;         // bucket number (bits >> flatShift) of compact[0]
+    uint32_t flatHigh;        // bucket number of compact[flatCount - 1]
+    int32_t bucketCount;
     const uint32_t* bandBits; // (maxCode + 1) << bandStrideLog2 bits: the exact answer for every in-band float
-    uint32_t bandStrideLog2;  // bits reserved per step (power of two >= the widest band)
-    // Compact variant of the flat table (same buckets: flatShift / flatLow / flatHigh), one 32-bit word per bucket, or
-    // nullptr.  See "Compact entries" below.
+    uint32_t bandStrideLog2;  // bits reserved per step (power of two >= the widest band plus two in-band units)
+    // The compact variant, one 32-bit word per bucket, or nullptr when it does not apply.  See "Compact entries" below.
     const uint32_t* compact;
     const uint32_t* firstBits; // first_k for k = 0 .. maxCode + 1 (0 for codes that no input reaches)
     // compact and firstBits are one device allocation, the shared-memory image of the kernels that use them:
@@ -91,8 +83,8 @@ struct CurveTableView
 };
 
 // Compact entries.  A random 64-bit gather from shared memory costs ~5.2 data-pipe wavefronts (two half-warp phases of
-// 16 random bank pairs), a 32-bit one ~3.5, and the config-2 kernel is bound by exactly that pipe -- so the flat table
-// is also kept in a one-word form, S = flatShift, D = depth (needs S + D + 6 <= 32):
+// 16 random bank pairs), a 32-bit one ~3.5, and the config-2 kernel is bound by exactly that pipe -- so a bucket is one
+// word, S = flatShift, D = depth (S + D + 6 <= 32):
 //     bits 31 .. 32-S   step bucket: 2^S - off, off = first_k - bucketStart in (0, 2^S);  otherwise 0
 //     bits D+5 .. 6     step bucket: k - 1;  otherwise the code of every float of the bucket (before band corrections)
 //     bits 5 .. 0       lenq: the in-band floats of the bucket are those less than lenq * 2^(S-6) above the band start
@@ -111,10 +103,8 @@ struct CurveTableStats
     double buildMilliseconds = 0.0;
     uint64_t sweptInputs = 0;
     uint64_t inBandInputs = 0;     // inputs the kernel sends to the exact path (two-level table)
-    uint64_t flatInBandInputs = 0; // flat variant: inputs resolved through the band bitmap (exact per-step widths)
-    uint64_t bandBitmapBytes = 0;  // size of the flat variant's band bitmap
-    int32_t flatBuckets = 0;       // 0 when the flat variant does not apply
-    uint64_t compactInBandInputs = 0; // compact variant: inputs flagged in band (a superset of flatInBandInputs)
+    uint64_t bandBitmapBytes = 0;  // size of the compact variant's band bitmap
+    uint64_t compactInBandInputs = 0; // compact variant: inputs flagged in band, resolved through the band bitmap
     int32_t compactBuckets = 0;    // 0 when the compact variant does not apply
     uint64_t verifyMismatches = 0; // must be 0
     int32_t steps = 0;             // thresholds found
@@ -133,7 +123,6 @@ struct CurveTable
     std::string error;
     void* deviceOctaves = nullptr;
     void* deviceBuckets = nullptr;
-    void* deviceFlat = nullptr;
     void* deviceBandBits = nullptr;
     void* deviceCompact = nullptr;
     void* deviceFirstBits = nullptr;

@@ -102,11 +102,12 @@ __device__ __forceinline__ void HostPixelToCodes(const EncodeParams& p, const Ho
             if (i < colors)
             {
                 // A built and verified step table (curve_tables.h) answers every finite sample from global memory: one
-                // 64-bit gather, plus one bit of the band bitmap for the ~1.5 % of samples inside a fuzzy band.
+                // 32-bit gather, plus first_k and one bit of the band bitmap for the samples flagged as possibly inside
+                // a fuzzy band.  +inf and NaN take the exact evaluation below.
                 if (p.useCurveView && static_cast<int32_t>(__float_as_uint(color[i])) <= 0x7f7fffff)
                 {
                     bool inBand;
-                    codes[i] = LookupCurveCodeFlatResolved(__float_as_uint(color[i]), p.curveView, inBand);
+                    codes[i] = LookupCurveCodeCompactResolved(__float_as_uint(color[i]), p.curveView, inBand);
                     continue;
                 }
                 float curved;

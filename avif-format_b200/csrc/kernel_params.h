@@ -86,7 +86,7 @@ struct EncodeParams
     float hlgPeak;
     int32_t rowMatrixEnabled; // avifgpu_encode_desc.row_matrix: the colour-profile 3x3 ahead of everything else (float colour hosts)
     float rowMatrix[9];
-    // Float hosts with a transfer curve: the flat step table + band bitmap in global memory (a by-value copy of
+    // Float hosts with a transfer curve: the compact step table + band bitmap in global memory (a by-value copy of
     // *curveTable made by the generic launcher), or useCurveView = 0 -> every sample takes the exact powf.
     CurveTableView curveView;
     int32_t useCurveView;

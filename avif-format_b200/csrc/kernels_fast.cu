@@ -12,8 +12,6 @@
 
 #include <cuda_runtime.h>
 
-#include <cstdlib>
-
 namespace avifgpu
 {
 
@@ -192,9 +190,9 @@ int LaunchEncodeFast(const EncodeParams& p, int hostDepth, void* streamHandle)
     {
         return 0;
     }
-    if (rgba && (curve == kCurveClip || p.curveTable->flat == nullptr || p.curveTable->bandBits == nullptr))
+    if (rgba && (curve == kCurveClip || p.curveTable->compact == nullptr || p.curveTable->bandBits == nullptr))
     {
-        return 0; // the RGBA kernel is built on the flat table + band bitmap; everything else with alpha: generic
+        return 0; // the RGBA kernel is built on the compact table + band bitmap; everything else with alpha: generic
     }
     const int width4 = p.width & ~3;
     const int evenRows = p.ys ? (p.rowCount & ~1) : p.rowCount;
@@ -223,8 +221,6 @@ int LaunchEncodeFast(const EncodeParams& p, int hostDepth, void* streamHandle)
     if (curve != kCurveClip)
     {
         fp.table = *p.curveTable;
-        static const bool wide = []() { const char* v = std::getenv("AVIFGPU_WIDE_TABLE_ENTRIES"); return v != nullptr && v[0] == '1'; }();
-        fp.preferWideEntries = wide ? 1 : 0;
     }
     if (rgba)
     {

@@ -42,7 +42,6 @@ struct FastEncodeParams
     ForwardMatrix matrix;
     float chromaOffset;
     int32_t topLeft;
-    int32_t preferWideEntries; // AVIFGPU_WIDE_TABLE_ENTRIES=1 in the environment: the 64-bit flat table even where the compact one applies (A/B measurements)
     CurveTableView table;
 };
 

@@ -1,9 +1,9 @@
-// kernels_fast_flat.cu -- the float RGB -> planar YCbCr encode kernel for curves whose step table has the flat
-// form (curve_tables.h): BASELINE config 2, 7680x4320 RGB32f -> 12-bit PQ 4:2:0.
+// kernels_fast_flat.cu -- the float RGB -> planar YCbCr encode kernel for curves with a step table in shared memory
+// (curve_tables.h): BASELINE config 2, 7680x4320 RGB32f -> 12-bit PQ 4:2:0.
 //
 //   * one CTA per SM, kFlatWarps warps; the step table (compact one-word entries + first_k, 67 KB at 12 bits; or the
-//     128 KB 64-bit flat table / the two-level table where the compact form does not apply) sits in shared memory next to
-//     one 3 KB staging buffer per warp.  The compact table's image is brought in by the copy engine (table_staging.cuh).
+//     two-level table where the compact form does not apply) sits in shared memory next to one 3 KB staging buffer per
+//     warp.  The compact table's image is brought in by the copy engine (table_staging.cuh).
 //     Measured on the 8K PQ frame (Gpx/s, round 1): 16 warps 238 | 20: 251 | 24: 273 | 28: 278 | 30: 267 (30 leaves 64
 //     registers); the kernel is bound by instruction issue and shared-memory wavefronts, so resident warps matter, and
 //     the copy engine keeps the per-warp register cost of a fetch at zero;
@@ -56,11 +56,6 @@ struct FlatSchedule
     int32_t segmentRows, longSegments; // segment s holds segmentRows (+ 1 if s < longSegments) tile rows
     int32_t lastColumnBytes;          // row-segment bytes of the last tile column (width need not be a multiple of 128)
     int32_t unpairedTileRow;          // tile row whose second image row does not exist (odd row count), or -1
-    // Run lengths differ by one tile row.  With the warps of a CTA on adjacent items a CTA is all long runs or all short
-    // ones, and the launch ends when the long CTAs do.  scatter = 1 deals the items round-robin over the CTAs instead
-    // (item = warp * CTAs + CTA): every CTA gets the same mix, so the extra round is spread over every SM rather than
-    // run by a fraction of them.
-    int32_t scatter;
 };
 
 // One lane of the (converged) warp.
@@ -71,26 +66,28 @@ __device__ __forceinline__ bool ElectOne()
     return elected != 0;
 }
 
-// TWO_LEVEL = 0: the flat table (64-bit entries) + band bitmap.  TWO_LEVEL = 1: the per-binade two-level table (curves whose
-// steps are too dense for one bucket size, e.g. 12-bit SMPTE 428); its rare in-band samples take the exact evaluation in
-// place.  TWO_LEVEL = 2: the flat table in its compact one-word form (curve_tables.h "Compact entries") + the first_k
-// array + band bitmap: a 32-bit gather costs ~3.5 shared-memory wavefronts where the 64-bit one costs ~5.2, and that pipe
-// is what bounds the 64-bit variant.  TWO_LEVEL = 3: the same with flatShift = 14 known at compile time (12-bit PQ).
+// Which step table a kernel stages.  kTableTwoLevel: the per-binade two-level table (curves whose steps are too dense
+// for one bucket size, e.g. 12-bit SMPTE 428); its rare in-band samples take the exact evaluation in place.
+// kTableCompact: the compact one-word entries (curve_tables.h "Compact entries") + the first_k array + band bitmap.
+// kTableCompact14: the same with flatShift = 14 known at compile time (12-bit PQ).
+constexpr int kTableTwoLevel = 1;
+constexpr int kTableCompact = 2;
+constexpr int kTableCompact14 = 3;
+
 // INTERLEAVED = 1: the reference's own output layout (heif_channel_interleaved RGB, WriteHeifImage.cpp:1098-1130) -- the
 // codes are stored as they are, 3 x uint16 per pixel into plane Y's buffer, no matrix (XS = YS = 0 then).
-template <int CURVE, int XS, int YS, int TWO_LEVEL, int INTERLEAVED>
+template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED>
 __global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const FastEncodeParams p, const FlatSchedule schedule)
 {
-    constexpr bool kCompact = TWO_LEVEL >= 2;
-    constexpr int kCompactShift = TWO_LEVEL == 3 ? 14 : 0;
+    constexpr bool kCompact = TABLE != kTableTwoLevel;
+    constexpr int kCompactShift = TABLE == kTableCompact14 ? 14 : 0;
     extern __shared__ __align__(128) uint8_t sharedBytes[];
     uint64_t* libmStorage = reinterpret_cast<uint64_t*>(sharedBytes);
     uint64_t* barriers = reinterpret_cast<uint64_t*>(sharedBytes + kSharedLibm);
     uint8_t* stageAll = sharedBytes + kSharedLibm + kSharedBarriers;
-    uint2* flatEntries = reinterpret_cast<uint2*>(sharedBytes + FlatFixedBytes());
-    uint32_t* compactEntries = reinterpret_cast<uint32_t*>(sharedBytes + FlatFixedBytes());                                  // TWO_LEVEL == 2 ...
-    const uint32_t* firstBits = compactEntries + ((p.table.flatCount + 3) & ~3);                                             // ... then first_k per code
-    uint2* octaves = reinterpret_cast<uint2*>(sharedBytes + FlatFixedBytes());            // TWO_LEVEL: 256 entries ...
+    uint32_t* compactEntries = reinterpret_cast<uint32_t*>(sharedBytes + FlatFixedBytes());  // compact: the entries ...
+    const uint32_t* firstBits = compactEntries + ((p.table.flatCount + 3) & ~3);             // ... then first_k per code
+    uint2* octaves = reinterpret_cast<uint2*>(sharedBytes + FlatFixedBytes());               // two-level: 256 entries ...
     uint32_t* bucketWords = reinterpret_cast<uint32_t*>(sharedBytes + FlatFixedBytes() + 2048); // ... then the bucket words
 
     const int lane = threadIdx.x & 31;
@@ -104,7 +101,10 @@ __global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const 
 
     const int tilesX = schedule.tilesX;
     const int warpCount = schedule.warpCount;
-    const int firstItem = schedule.scatter ? warpInBlock * static_cast<int>(gridDim.x) + static_cast<int>(blockIdx.x) : static_cast<int>(blockIdx.x) * kFlatWarps + warpInBlock;
+    // Run lengths differ by one tile row.  The items are dealt round-robin over the CTAs (item = warp * CTAs + CTA), so every
+    // CTA gets the same mix of long and short runs and the extra round is spread over every SM rather than run by a
+    // fraction of them.
+    const int firstItem = warpInBlock * static_cast<int>(gridDim.x) + static_cast<int>(blockIdx.x);
     constexpr int kChromaRowsPerTile = YS ? 1 : 2;
     constexpr int kChromaTileBytes = XS ? kTilePixels : 2 * kTilePixels;
 
@@ -151,11 +151,7 @@ __global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const 
     }
 
     const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
-    if (kCompact)
-    {
-        // in flight (above)
-    }
-    else if (TWO_LEVEL)
+    if (!kCompact) // the compact image is in flight (above)
     {
         for (int i = threadIdx.x; i < 256; i += blockDim.x)
         {
@@ -164,18 +160,6 @@ __global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const 
         for (int i = threadIdx.x; i < p.table.bucketCount; i += blockDim.x)
         {
             bucketWords[i] = p.table.buckets[i];
-        }
-    }
-    else
-    {
-        // 128 KB from L2: 128-bit copies, eight in flight per thread (the table is 16-byte aligned, count is even-padded)
-        const uint4* source = reinterpret_cast<const uint4*>(p.table.flat);
-        uint4* target = reinterpret_cast<uint4*>(flatEntries);
-        const int pairs = (p.table.flatCount + 1) / 2;
-#pragma unroll 8
-        for (int i = threadIdx.x; i < pairs; i += blockDim.x)
-        {
-            target[i] = __ldg(source + i);
         }
     }
     __syncthreads(); // the libm tables, the barriers' initialisation
@@ -240,17 +224,13 @@ __global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const 
                     codeF[j] = LookupCurveCompact<kCompactShift>(bits[e], compactEntries, flatShift, negativeLow, span, compactTopShift, compactCodeMask,
                                                                  compactMagic, inBand, entry);
                 }
-                else if (TWO_LEVEL)
+                else
                 {
                     codeF[j] = CodeToFloat(LookupCurveCode(bits[e], octaves, bucketWords, inBand)); // reports +inf / NaN in band itself
                 }
-                else
-                {
-                    codeF[j] = LookupCurveFlat(bits[e], flatEntries, flatShift, negativeLow, span, inBand);
-                }
                 asm("{ .reg .pred p; setp.ne.u32 p, %1, 0; @p or.b32 %0, %0, %2; }" : "+r"(bandMask) : "r"(static_cast<uint32_t>(inBand)), "r"(1u << j));
             }
-            if (TWO_LEVEL != 1)
+            if (kCompact)
             {
                 largest = max(largest, __vimax3_s32(static_cast<int32_t>(w.x), static_cast<int32_t>(w.y), static_cast<int32_t>(w.z)));
                 largest = max(largest, static_cast<int32_t>(w.w));
@@ -297,46 +277,14 @@ __global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const 
                 }
             }
         }
-        else if (!TWO_LEVEL)
-        {
-            uint32_t pending = bandMask;
-            while (pending != 0)
-            {
-                const int j0 = __ffs(static_cast<int>(pending)) - 1;
-                pending &= pending - 1;
-                const uint32_t bits0 = stagedBits(j0);
-                bool inBand;
-                uint2 entry0;
-                LookupCurveFlat(bits0, flatEntries, flatShift, negativeLow, span, inBand, entry0);
-                const uint32_t index0 = BandBitIndex(bits0, entry0, bandStrideLog2);
-                const uint32_t word0 = __ldg(bandBits + (index0 >> 5));
-                uint32_t word1 = 0xffffffffu, index1 = 0, sample1 = 0;
-                if (pending != 0)
-                {
-                    const int j1 = __ffs(static_cast<int>(pending)) - 1;
-                    pending &= pending - 1;
-                    const uint32_t bits1 = stagedBits(j1);
-                    uint2 entry1;
-                    LookupCurveFlat(bits1, flatEntries, flatShift, negativeLow, span, inBand, entry1);
-                    index1 = BandBitIndex(bits1, entry1, bandStrideLog2);
-                    word1 = __ldg(bandBits + (index1 >> 5));
-                    sample1 = 1u << j1;
-                }
-                lowerMask |= (((word0 >> (index0 & 31u)) & 1u) ^ 1u) << j0;
-                if (((word1 >> (index1 & 31u)) & 1u) == 0)
-                {
-                    lowerMask |= sample1;
-                }
-            }
-        }
 
         // ---- +inf / NaN (never in real frames): the exact evaluation, lane by lane ------------------------------------
-        if (__any_sync(0xffffffffu, TWO_LEVEL == 1 ? bandMask != 0 : largest > 0x7f7fffff))
+        if (__any_sync(0xffffffffu, kCompact ? largest > 0x7f7fffff : bandMask != 0))
         {
             for (int j = 0; j < kValuesPerLane; ++j)
             {
                 const uint32_t bits = stagedBits(j);
-                if (TWO_LEVEL == 1 ? ((bandMask >> j) & 1u) != 0 : static_cast<int32_t>(bits) > 0x7f7fffff)
+                if (kCompact ? static_cast<int32_t>(bits) > 0x7f7fffff : ((bandMask >> j) & 1u) != 0)
                 {
                     const float exact = CodeToFloat(ExactCurveCode<CURVE>(__uint_as_float(bits), p.pqMultiplier, p.maxCodeFloat, t));
 #pragma unroll
@@ -400,21 +348,18 @@ __global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const 
     }
 }
 
-// tableKind: 0 flat (64-bit entries), 1 two-level, 2 compact (32-bit entries + first_k per code)
-inline size_t TableSharedBytes(const FastEncodeParams& fp, int tableKind)
+inline size_t TableSharedBytes(const FastEncodeParams& fp, int table)
 {
-    if (tableKind == 1) return 2048 + static_cast<size_t>(fp.table.bucketCount) * sizeof(uint32_t);
-    if (tableKind >= 2) return fp.table.compactImageBytes;
-    return static_cast<size_t>((fp.table.flatCount + 1) / 2) * sizeof(uint4);
+    return table == kTableTwoLevel ? 2048 + static_cast<size_t>(fp.table.bucketCount) * sizeof(uint32_t) : fp.table.compactImageBytes;
 }
 
-template <int CURVE, int XS, int YS, int TWO_LEVEL, int INTERLEAVED = 0>
+template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED = 0>
 cudaError_t LaunchFlatKernel(const FastEncodeParams& fp, int smCount, cudaStream_t stream)
 {
-    const size_t shared = static_cast<size_t>(FlatFixedBytes()) + TableSharedBytes(fp, TWO_LEVEL);
+    const size_t shared = static_cast<size_t>(FlatFixedBytes()) + TableSharedBytes(fp, TABLE);
     static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
     {
-        const cudaError_t e = AllowDynamicShared(EncodeRgbF32FlatKernel<CURVE, XS, YS, TWO_LEVEL, INTERLEAVED>, kSharedLimit, configuredDevices);
+        const cudaError_t e = AllowDynamicShared(EncodeRgbF32FlatKernel<CURVE, XS, YS, TABLE, INTERLEAVED>, kSharedLimit, configuredDevices);
         if (e != cudaSuccess)
         {
             return e;
@@ -442,45 +387,37 @@ cudaError_t LaunchFlatKernel(const FastEncodeParams& fp, int smCount, cudaStream
     schedule.longSegments = schedule.tileRows % schedule.segments;
     schedule.lastColumnBytes = (fp.width - (schedule.tilesX - 1) * kTilePixels) * 12;
     schedule.unpairedTileRow = (fp.rowCount & 1) ? fp.rowCount / 2 : -1;
-    static const bool scatterOff = []() { const char* v = getenv("AVIFGPU_FLAT_SCATTER"); return v != nullptr && v[0] == '0'; }(); // A/B measurements
-    schedule.scatter = scatterOff ? 0 : 1;
-    EncodeRgbF32FlatKernel<CURVE, XS, YS, TWO_LEVEL, INTERLEAVED><<<static_cast<unsigned>(blocks), kFlatThreads, shared, stream>>>(fp, schedule);
+    EncodeRgbF32FlatKernel<CURVE, XS, YS, TABLE, INTERLEAVED><<<static_cast<unsigned>(blocks), kFlatThreads, shared, stream>>>(fp, schedule);
     return cudaGetLastError();
 }
 
-template <int CURVE, int TWO_LEVEL>
+template <int CURVE, int TABLE>
 cudaError_t DispatchFlatChroma(const FastEncodeParams& fp, int xs, int ys, int smCount, cudaStream_t stream)
 {
-    if (xs == 1 && ys == 1) return LaunchFlatKernel<CURVE, 1, 1, TWO_LEVEL>(fp, smCount, stream);
-    if (xs == 1) return LaunchFlatKernel<CURVE, 1, 0, TWO_LEVEL>(fp, smCount, stream);
-    return LaunchFlatKernel<CURVE, 0, 0, TWO_LEVEL>(fp, smCount, stream);
+    if (xs == 1 && ys == 1) return LaunchFlatKernel<CURVE, 1, 1, TABLE>(fp, smCount, stream);
+    if (xs == 1) return LaunchFlatKernel<CURVE, 1, 0, TABLE>(fp, smCount, stream);
+    return LaunchFlatKernel<CURVE, 0, 0, TABLE>(fp, smCount, stream);
 }
 
 } // namespace
 
-static bool FlatTableFits(const FastEncodeParams& fp)
-{
-    return fp.table.flat != nullptr && fp.table.bandBits != nullptr &&
-           static_cast<size_t>(FlatFixedBytes()) + TableSharedBytes(fp, 0) <= static_cast<size_t>(kSharedLimit);
-}
-
 static bool CompactTableFits(const FastEncodeParams& fp)
 {
     return fp.table.compact != nullptr && fp.table.firstBits != nullptr && fp.table.bandBits != nullptr &&
-           static_cast<size_t>(FlatFixedBytes()) + TableSharedBytes(fp, 2) <= static_cast<size_t>(kSharedLimit);
+           static_cast<size_t>(FlatFixedBytes()) + TableSharedBytes(fp, kTableCompact) <= static_cast<size_t>(kSharedLimit);
 }
 
 static bool TwoLevelTableFits(const FastEncodeParams& fp)
 {
     return fp.table.buckets != nullptr && fp.table.octaves != nullptr &&
-           static_cast<size_t>(FlatFixedBytes()) + TableSharedBytes(fp, 1) <= static_cast<size_t>(kSharedLimit);
+           static_cast<size_t>(FlatFixedBytes()) + TableSharedBytes(fp, kTableTwoLevel) <= static_cast<size_t>(kSharedLimit);
 }
 
-// True when the copy-engine kernel can serve this table: the flat form with its bitmap, else the two-level form, in
+// True when the copy-engine kernel can serve this table: the compact form with its bitmap, else the two-level form, in
 // shared memory next to the staging buffers.
 bool FlatEncodeApplies(const FastEncodeParams& fp)
 {
-    return CompactTableFits(fp) || FlatTableFits(fp) || TwoLevelTableFits(fp);
+    return CompactTableFits(fp) || TwoLevelTableFits(fp);
 }
 
 // The reference's interleaved RGB layout through the same kernel (fp.planeY / strideY = the interleaved buffer).
@@ -490,36 +427,28 @@ cudaError_t LaunchFastEncodeFlatInterleaved(const FastEncodeParams& fp, int curv
     {
         if (curve == kCurveLinearToPQ)
         {
-            return fp.table.flatShift == 14 ? LaunchFlatKernel<kCurveLinearToPQ, 0, 0, 3, 1>(fp, smCount, stream) : LaunchFlatKernel<kCurveLinearToPQ, 0, 0, 2, 1>(fp, smCount, stream);
+            return fp.table.flatShift == 14 ? LaunchFlatKernel<kCurveLinearToPQ, 0, 0, kTableCompact14, 1>(fp, smCount, stream)
+                                            : LaunchFlatKernel<kCurveLinearToPQ, 0, 0, kTableCompact, 1>(fp, smCount, stream);
         }
-        return LaunchFlatKernel<kCurveLinearToSMPTE428, 0, 0, 2, 1>(fp, smCount, stream);
+        return LaunchFlatKernel<kCurveLinearToSMPTE428, 0, 0, kTableCompact, 1>(fp, smCount, stream);
     }
-    if (FlatTableFits(fp))
-    {
-        if (curve == kCurveLinearToPQ) return LaunchFlatKernel<kCurveLinearToPQ, 0, 0, 0, 1>(fp, smCount, stream);
-        return LaunchFlatKernel<kCurveLinearToSMPTE428, 0, 0, 0, 1>(fp, smCount, stream);
-    }
-    if (curve == kCurveLinearToPQ) return LaunchFlatKernel<kCurveLinearToPQ, 0, 0, 1, 1>(fp, smCount, stream);
-    return LaunchFlatKernel<kCurveLinearToSMPTE428, 0, 0, 1, 1>(fp, smCount, stream);
+    if (curve == kCurveLinearToPQ) return LaunchFlatKernel<kCurveLinearToPQ, 0, 0, kTableTwoLevel, 1>(fp, smCount, stream);
+    return LaunchFlatKernel<kCurveLinearToSMPTE428, 0, 0, kTableTwoLevel, 1>(fp, smCount, stream);
 }
 
 cudaError_t LaunchFastEncodeFlat(const FastEncodeParams& fp, int curve, int xs, int ys, int smCount, cudaStream_t stream)
 {
-    if (CompactTableFits(fp) && !fp.preferWideEntries)
+    if (CompactTableFits(fp))
     {
         if (curve == kCurveLinearToPQ)
         {
-            return fp.table.flatShift == 14 ? DispatchFlatChroma<kCurveLinearToPQ, 3>(fp, xs, ys, smCount, stream) : DispatchFlatChroma<kCurveLinearToPQ, 2>(fp, xs, ys, smCount, stream);
+            return fp.table.flatShift == 14 ? DispatchFlatChroma<kCurveLinearToPQ, kTableCompact14>(fp, xs, ys, smCount, stream)
+                                            : DispatchFlatChroma<kCurveLinearToPQ, kTableCompact>(fp, xs, ys, smCount, stream);
         }
-        return DispatchFlatChroma<kCurveLinearToSMPTE428, 2>(fp, xs, ys, smCount, stream);
+        return DispatchFlatChroma<kCurveLinearToSMPTE428, kTableCompact>(fp, xs, ys, smCount, stream);
     }
-    if (FlatTableFits(fp))
-    {
-        if (curve == kCurveLinearToPQ) return DispatchFlatChroma<kCurveLinearToPQ, 0>(fp, xs, ys, smCount, stream);
-        return DispatchFlatChroma<kCurveLinearToSMPTE428, 0>(fp, xs, ys, smCount, stream);
-    }
-    if (curve == kCurveLinearToPQ) return DispatchFlatChroma<kCurveLinearToPQ, 1>(fp, xs, ys, smCount, stream);
-    return DispatchFlatChroma<kCurveLinearToSMPTE428, 1>(fp, xs, ys, smCount, stream);
+    if (curve == kCurveLinearToPQ) return DispatchFlatChroma<kCurveLinearToPQ, kTableTwoLevel>(fp, xs, ys, smCount, stream);
+    return DispatchFlatChroma<kCurveLinearToSMPTE428, kTableTwoLevel>(fp, xs, ys, smCount, stream);
 }
 
 } // namespace avifgpu

@@ -1,5 +1,5 @@
-// kernels_fast_rgba.cu -- float RGBA hosts -> planar YCbCr + alpha plane through the step table (compact one-word entries
-// where the table has them, else the 64-bit flat entries; curve_tables.h) and the band bitmap
+// kernels_fast_rgba.cu -- float RGBA hosts -> planar YCbCr + alpha plane through the compact step table (one-word entries
+// + first_k in shared memory, brought in by the copy engine; curve_tables.h) and the band bitmap
 // (CreateHeifImageRGBThirtyTwoBit's alpha branch, WriteHeifImage.cpp:1039-1077, fused with the libheif stage).
 //
 // Same warp tile as kernels_fast_flat.cu (2 rows x 128 pixels, a lane owns 4 adjacent pixels in both rows), but 16 bytes
@@ -31,34 +31,22 @@ constexpr int kSharedLimit = 227 * 1024;
 constexpr int kTableBarrierBytes = 16; // the table image's mbarrier, padded
 __host__ __device__ constexpr int RgbaFixedBytes() { return kSharedLibm + kTableBarrierBytes + kRgbaWarps * kStagePerWarp; }
 
-// COMPACT = 1: compact table + first_k array in shared memory (kernels_fast_flat.cu has the commentary).
-template <int CURVE, int XS, int YS, int COMPACT>
+// The compact table + first_k array in shared memory (kernels_fast_flat.cu has the commentary).
+template <int CURVE, int XS, int YS>
 __global__ void __launch_bounds__(kRgbaThreads, 1) EncodeRgbaF32FlatKernel(const FastEncodeParams p)
 {
     extern __shared__ __align__(16) uint8_t sharedBytes[];
     uint64_t* libmStorage = reinterpret_cast<uint64_t*>(sharedBytes);
     uint64_t* tableBarrier = reinterpret_cast<uint64_t*>(sharedBytes + kSharedLibm);
     uint32_t* stageAll = reinterpret_cast<uint32_t*>(sharedBytes + kSharedLibm + kTableBarrierBytes);
-    uint2* flatEntries = reinterpret_cast<uint2*>(sharedBytes + RgbaFixedBytes());
     uint32_t* compactEntries = reinterpret_cast<uint32_t*>(sharedBytes + RgbaFixedBytes());
     const uint32_t* firstBits = compactEntries + ((p.table.flatCount + 3) & ~3);
 
-    if (COMPACT && threadIdx.x == 0)
+    if (threadIdx.x == 0)
     {
         staging::BeginTableImageCopy(p.table, compactEntries, tableBarrier); // table_staging.cuh
     }
     const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
-    if (!COMPACT)
-    {
-        const uint4* source = reinterpret_cast<const uint4*>(p.table.flat);
-        uint4* target = reinterpret_cast<uint4*>(flatEntries);
-        const int pairs = (p.table.flatCount + 1) / 2;
-#pragma unroll 8
-        for (int i = threadIdx.x; i < pairs; i += blockDim.x)
-        {
-            target[i] = __ldg(source + i);
-        }
-    }
     __syncthreads(); // the libm tables, the table barrier's initialisation
 
     const int lane = threadIdx.x & 31;
@@ -101,10 +89,7 @@ __global__ void __launch_bounds__(kRgbaThreads, 1) EncodeRgbaF32FlatKernel(const
         }
     };
     loadTile(tileRow, tileX, firstTile < tileCount); // in flight while the table image lands
-    if (COMPACT)
-    {
-        staging::WaitTableImage(tableBarrier);
-    }
+    staging::WaitTableImage(tableBarrier);
 
 #pragma unroll 1
     for (int tile = firstTile; tile < tileCount; tile += warpCount)
@@ -158,15 +143,8 @@ __global__ void __launch_bounds__(kRgbaThreads, 1) EncodeRgbaF32FlatKernel(const
         for (int j = 0; j < kValuesPerLane; ++j)
         {
             bool inBand;
-            if (COMPACT)
-            {
-                uint32_t entry;
-                codeF[j] = LookupCurveCompact<0>(colourBits[j], compactEntries, flatShift, negativeLow, span, compactTopShift, compactCodeMask, compactMagic, inBand, entry);
-            }
-            else
-            {
-                codeF[j] = LookupCurveFlat(colourBits[j], flatEntries, flatShift, negativeLow, span, inBand);
-            }
+            uint32_t entry;
+            codeF[j] = LookupCurveCompact<0>(colourBits[j], compactEntries, flatShift, negativeLow, span, compactTopShift, compactCodeMask, compactMagic, inBand, entry);
             asm("{ .reg .pred q; setp.ne.u32 q, %1, 0; @q or.b32 %0, %0, %2; }" : "+r"(bandMask) : "r"(static_cast<uint32_t>(inBand)), "r"(1u << j));
             largest = max(largest, static_cast<int32_t>(colourBits[j]));
         }
@@ -181,26 +159,16 @@ __global__ void __launch_bounds__(kRgbaThreads, 1) EncodeRgbaF32FlatKernel(const
                 const int j = __ffs(static_cast<int>(pending)) - 1;
                 pending &= pending - 1;
                 const uint32_t bits = myStage[j];
-                if (COMPACT)
+                const int32_t bucket = __viaddmin_s32_relu(static_cast<int32_t>(bits) >> flatShift, negativeLow, span);
+                const uint32_t entry = compactEntries[bucket];
+                const uint32_t k = ((entry & compactCodeMask) >> kCompactLenBits) + ((entry >> compactTopShift) != 0 ? 1u : 0u);
+                const uint32_t distance = bits - firstBits[k];
+                if (k != 0 && distance < (1u << bandStrideLog2)) // else flagged by the superset test only
                 {
-                    const int32_t bucket = __viaddmin_s32_relu(static_cast<int32_t>(bits) >> flatShift, negativeLow, span);
-                    const uint32_t entry = compactEntries[bucket];
-                    const uint32_t k = ((entry & compactCodeMask) >> kCompactLenBits) + ((entry >> compactTopShift) != 0 ? 1u : 0u);
-                    const uint32_t distance = bits - firstBits[k];
-                    if (k != 0 && distance < (1u << bandStrideLog2)) // else flagged by the superset test only
-                    {
-                        const uint32_t bitIndex = (k << bandStrideLog2) + distance;
-                        const uint32_t word = __ldg(bandBits + (bitIndex >> 5));
-                        lowerMask |= (((word >> (bitIndex & 31u)) & 1u) ^ 1u) << j;
-                    }
-                    continue;
+                    const uint32_t bitIndex = (k << bandStrideLog2) + distance;
+                    const uint32_t word = __ldg(bandBits + (bitIndex >> 5));
+                    lowerMask |= (((word >> (bitIndex & 31u)) & 1u) ^ 1u) << j;
                 }
-                bool inBand;
-                uint2 entry;
-                LookupCurveFlat(bits, flatEntries, flatShift, negativeLow, span, inBand, entry);
-                const uint32_t bitIndex = BandBitIndex(bits, entry, bandStrideLog2);
-                const uint32_t word = __ldg(bandBits + (bitIndex >> 5));
-                lowerMask |= (((word >> (bitIndex & 31u)) & 1u) ^ 1u) << j;
             }
         }
         // ---- +inf / NaN: the exact evaluation, lane by lane -------------------------------------------------------------
@@ -250,18 +218,13 @@ __global__ void __launch_bounds__(kRgbaThreads, 1) EncodeRgbaF32FlatKernel(const
     }
 }
 
-size_t RgbaTableBytes(const FastEncodeParams& fp, bool compact)
-{
-    return compact ? static_cast<size_t>(fp.table.compactImageBytes) : static_cast<size_t>((fp.table.flatCount + 1) / 2) * sizeof(uint4);
-}
-
-template <int CURVE, int XS, int YS, int COMPACT>
+template <int CURVE, int XS, int YS>
 cudaError_t LaunchRgbaKernel(const FastEncodeParams& fp, int smCount, cudaStream_t stream)
 {
-    const size_t shared = static_cast<size_t>(RgbaFixedBytes()) + RgbaTableBytes(fp, COMPACT != 0);
+    const size_t shared = static_cast<size_t>(RgbaFixedBytes()) + fp.table.compactImageBytes;
     static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
     {
-        const cudaError_t e = AllowDynamicShared(EncodeRgbaF32FlatKernel<CURVE, XS, YS, COMPACT>, kSharedLimit, configuredDevices);
+        const cudaError_t e = AllowDynamicShared(EncodeRgbaF32FlatKernel<CURVE, XS, YS>, kSharedLimit, configuredDevices);
         if (e != cudaSuccess)
         {
             return e;
@@ -277,35 +240,31 @@ cudaError_t LaunchRgbaKernel(const FastEncodeParams& fp, int smCount, cudaStream
     {
         blocks = smCount;
     }
-    EncodeRgbaF32FlatKernel<CURVE, XS, YS, COMPACT><<<static_cast<unsigned>(blocks), kRgbaThreads, shared, stream>>>(fp);
+    EncodeRgbaF32FlatKernel<CURVE, XS, YS><<<static_cast<unsigned>(blocks), kRgbaThreads, shared, stream>>>(fp);
     return cudaGetLastError();
 }
 
-template <int CURVE, int COMPACT>
+template <int CURVE>
 cudaError_t DispatchRgbaChroma(const FastEncodeParams& fp, int xs, int ys, int smCount, cudaStream_t stream)
 {
-    if (xs == 1 && ys == 1) return LaunchRgbaKernel<CURVE, 1, 1, COMPACT>(fp, smCount, stream);
-    if (xs == 1) return LaunchRgbaKernel<CURVE, 1, 0, COMPACT>(fp, smCount, stream);
-    return LaunchRgbaKernel<CURVE, 0, 0, COMPACT>(fp, smCount, stream);
+    if (xs == 1 && ys == 1) return LaunchRgbaKernel<CURVE, 1, 1>(fp, smCount, stream);
+    if (xs == 1) return LaunchRgbaKernel<CURVE, 1, 0>(fp, smCount, stream);
+    return LaunchRgbaKernel<CURVE, 0, 0>(fp, smCount, stream);
 }
 
 } // namespace
 
+// True when the kernel can stage this table's compact image next to its buffers.
 bool RgbaEncodeApplies(const FastEncodeParams& fp)
 {
-    return fp.planeA != nullptr && fp.table.flat != nullptr && fp.table.bandBits != nullptr &&
-           static_cast<size_t>(RgbaFixedBytes()) + static_cast<size_t>((fp.table.flatCount + 1) / 2) * sizeof(uint4) <= static_cast<size_t>(kSharedLimit);
+    return fp.planeA != nullptr && fp.table.compact != nullptr && fp.table.firstBits != nullptr && fp.table.bandBits != nullptr &&
+           static_cast<size_t>(RgbaFixedBytes()) + fp.table.compactImageBytes <= static_cast<size_t>(kSharedLimit);
 }
 
 cudaError_t LaunchFastEncodeRgba(const FastEncodeParams& fp, int curve, int xs, int ys, int smCount, cudaStream_t stream)
 {
-    if (fp.table.compact != nullptr && fp.table.firstBits != nullptr && !fp.preferWideEntries)
-    {
-        if (curve == kCurveLinearToPQ) return DispatchRgbaChroma<kCurveLinearToPQ, 1>(fp, xs, ys, smCount, stream);
-        return DispatchRgbaChroma<kCurveLinearToSMPTE428, 1>(fp, xs, ys, smCount, stream);
-    }
-    if (curve == kCurveLinearToPQ) return DispatchRgbaChroma<kCurveLinearToPQ, 0>(fp, xs, ys, smCount, stream);
-    return DispatchRgbaChroma<kCurveLinearToSMPTE428, 0>(fp, xs, ys, smCount, stream);
+    if (curve == kCurveLinearToPQ) return DispatchRgbaChroma<kCurveLinearToPQ>(fp, xs, ys, smCount, stream);
+    return DispatchRgbaChroma<kCurveLinearToSMPTE428>(fp, xs, ys, smCount, stream);
 }
 
 } // namespace avifgpu

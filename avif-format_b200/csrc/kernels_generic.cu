@@ -124,7 +124,7 @@ int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* streamH
     }
     EncodeParams p = params;
     p.useCurveView = 0;
-    if (hostDepth == 32 && p.curveTable != nullptr && p.curveTable->flat != nullptr && p.curveTable->bandBits != nullptr &&
+    if (hostDepth == 32 && p.curveTable != nullptr && p.curveTable->compact != nullptr && p.curveTable->bandBits != nullptr &&
         (p.transfer == AVIFGPU_TRANSFER_PQ || p.transfer == AVIFGPU_TRANSFER_SMPTE428 || p.transfer == AVIFGPU_TRANSFER_HLG))
     {
         p.curveView = *p.curveTable;

@@ -222,6 +222,8 @@ for tables in (False, True):
     tag = "step tables" if tables else "exact powf"
     float_encode_case(f"encode RGBA32f -> 12-bit PQ 4:2:0 + A, {tag} (a1)", 4, abi.LAYOUT_PLANAR_YCBCR, 16 + 5, tables)
     float_encode_case(f"encode RGB32f -> interleaved RGB 12-bit PQ (the reference's own layout), {tag} (a1)", 3, abi.LAYOUT_REFERENCE, 12 + 6, tables)
+# RGBA in the reference's layout has no tuned kernel: the generic kernel reads the compact step table from global memory
+float_encode_case("encode RGBA32f -> interleaved RGBA 12-bit PQ (the reference's own layout), step tables, generic kernel (a1)", 4, abi.LAYOUT_REFERENCE, 16 + 8, True)
 float_encode_case("encode RGB32f -> 10-bit PQ 4:2:0, tuned kernel (config 2 at 10 bits)", 3, abi.LAYOUT_PLANAR_YCBCR, 15, True, depth=10)
 float_encode_case("encode RGB32f -> 12-bit PQ @ 1000 nit 4:2:0, tuned kernel (config 2 at another peak)", 3, abi.LAYOUT_PLANAR_YCBCR, 15, True, peak=1000)
 float_encode_case("encode RGB32f -> 12-bit SMPTE 428 4:2:0 (two-level table in the copy-engine kernel)", 3, abi.LAYOUT_PLANAR_YCBCR, 15, True, transfer=abi.TRANSFER_SMPTE428)

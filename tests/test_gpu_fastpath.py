@@ -17,9 +17,12 @@ def planar_desc(w, h, depth=12, transfer=abi.TRANSFER_PQ, peak=80, chroma=abi.CH
 
 @pytest.mark.parametrize("transfer,peak,depth", [(abi.TRANSFER_PQ, 80, 12), (abi.TRANSFER_PQ, 80, 10), (abi.TRANSFER_PQ, 1000, 12),
                                                  (abi.TRANSFER_PQ, 10000, 12), (abi.TRANSFER_PQ, 1, 10), (abi.TRANSFER_SMPTE428, 80, 12),
-                                                 (abi.TRANSFER_SMPTE428, 80, 10)])
+                                                 (abi.TRANSFER_SMPTE428, 80, 10), (abi.TRANSFER_HLG, 80, 10), (abi.TRANSFER_HLG, 80, 12)])
 def test_step_tables_verify_against_every_float(gpu, transfer, peak, depth):
-    stats = gpu.prepare_encode(planar_desc(8, 8, depth, transfer, peak)).as_dict()
+    desc = planar_desc(8, 8, depth, transfer, peak)
+    if transfer == abi.TRANSFER_HLG:
+        desc.hlg_extension = abi.HLG_OETF  # the HLG save path: its table serves the generic kernel
+    stats = gpu.prepare_encode(desc).as_dict()
     print(stats)
     assert stats["applicable"] == 1 and stats["valid"] == 1, stats
     assert stats["verify_mismatches"] == 0

@@ -1195,9 +1195,9 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_indirect(avifgpu_context* ctx, const avi
     {
         return status;
     }
-    if (d.colorspace != AVIFGPU_COLORSPACE_YCBCR || d.alpha_state == AVIFGPU_ALPHA_PREMULTIPLIED)
+    if (d.colorspace == AVIFGPU_COLORSPACE_MONOCHROME || d.alpha_state == AVIFGPU_ALPHA_PREMULTIPLIED)
     {
-        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "device-described batches decode YCbCr with no or straight alpha");
+        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "device-described batches decode YCbCr or planar RGB with no or straight alpha");
     }
     DecodeParams shared;
     if (!FillDecodeParams(d, transfer, &shared, &error))

@@ -7,8 +7,8 @@
 // it) converts whatever the buffers hold at that moment.  A call is three launches:
 //   1. the plan kernel (one CTA) routes every image with the same per-image step and writes, per image, one interior
 //      record and up to two window records, the exclusive prefix sums of their units and the two totals into the workspace;
-//   2. the interior kernel walks the interior units with the tuned integer (float, for 32-bit decode hosts) kernel's
-//      per-unit code;
+//   2. the interior kernel walks the interior units with the tuned integer (float, for 32-bit decode hosts; planar-RGB,
+//      for planar-RGB decodes) kernel's per-unit code;
 //   3. the edge kernel walks the window units with the generic kernel's per-site / per-pixel code.
 // Both run the batched kernels of kernels_batch.cu.  Plain C++ (AVIFGPU_HD): host_params.cpp and the checks under
 // tests/native compile the per-image step with the host compiler.
@@ -165,8 +165,9 @@ AVIFGPU_HD inline BatchImagePlan PlanBatchEncodeImage(const EncodeParams& shared
     return plan;
 }
 
-// The same for decodes (`tuned` = DecodeBatchTuned: the float kernel's block half and 128-pixel units for 32-bit hosts,
-// the integer kernel's and 256-pixel units otherwise); edge units are runs of pixels of one row.
+// The same for decodes (`tuned` = DecodeBatchTuned: for planar RGB the planar-RGB kernels' block half; for YCbCr the float
+// kernel's for 32-bit hosts and the integer kernel's otherwise; units of DecodeBatchUnitPixels); edge units are runs of
+// pixels of one row.
 AVIFGPU_HD inline BatchImagePlan PlanBatchDecodeImage(const DecodeParams& shared, bool tuned, int planeMask, const avifgpu_batch_image& image)
 {
     BatchImagePlan plan{};
@@ -177,8 +178,10 @@ AVIFGPU_HD inline BatchImagePlan PlanBatchDecodeImage(const DecodeParams& shared
         return plan;
     }
     p.yPhase = 0;
-    const bool f32 = p.hostDepth == 32;
-    const Interior inner = !tuned ? Interior{ 0, 0 } : f32 ? DecodeYccF32BlockInterior(p) : DecodeYccIntBlockInterior(p);
+    const Interior inner = !tuned                                    ? Interior{ 0, 0 }
+                           : p.colorspace == AVIFGPU_COLORSPACE_RGB ? DecodePlanarRgbBlockInterior(p)
+                           : p.hostDepth == 32                      ? DecodeYccF32BlockInterior(p)
+                                                                    : DecodeYccIntBlockInterior(p);
     if (inner.width == 0)
     {
         plan.window[0] = RecordOf(DecodeWindow(p, 0, 0, p.width, p.rowCount));
@@ -187,7 +190,7 @@ AVIFGPU_HD inline BatchImagePlan PlanBatchDecodeImage(const DecodeParams& shared
         return plan;
     }
     plan.interior = RecordOf(DecodeWindow(p, 0, 0, inner.width, inner.rows));
-    plan.interiorUnits = BatchInteriorUnits(inner.width, inner.rows, p.ys, DecodeBatchUnitPixels(p.hostDepth));
+    plan.interiorUnits = BatchInteriorUnits(inner.width, inner.rows, p.ys, DecodeBatchUnitPixels(p.hostDepth, p.colorspace));
     Strip strip[2];
     plan.windows = InteriorStrips(p.width, p.rowCount, inner, strip);
     for (int k = 0; k < plan.windows; ++k)

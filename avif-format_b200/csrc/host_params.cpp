@@ -537,7 +537,37 @@ Interior DecodeYccF32Interior(const DecodeParams& p)
     return DecodeYccF32Tuned(p) ? DecodeYccF32BlockInterior(p) : Interior{ 0, 0 };
 }
 
-bool DecodeBatchTuned(const DecodeParams& p) { return p.hostDepth == 32 ? DecodeYccF32Tuned(p) : DecodeYccIntTuned(p); }
+// The description's conditions of the planar-RGB kernels: LaunchDecodeFastInteger's and LaunchDecodeStream's for 8/16-bit
+// hosts, LaunchDecodeFastTable's non-monochrome ones for 32-bit hosts -- less premultiplied alpha, which only the direct
+// table kernel un-premultiplies; DecodePlanarRgbBlockInterior has the block's.
+bool DecodePlanarRgbTuned(const DecodeParams& p)
+{
+    if (p.colorspace != AVIFGPU_COLORSPACE_RGB || (p.hasAlpha && p.premultiplied))
+    {
+        return false;
+    }
+    if (p.hostDepth == 32)
+    {
+        return p.bitDepth > 8 && p.bitDepth <= 12 &&
+               (p.transfer == AVIFGPU_TRANSFER_PQ || p.transfer == AVIFGPU_TRANSFER_HLG || p.transfer == AVIFGPU_TRANSFER_SMPTE428);
+    }
+    // 8-bit hosts read 8-bit planes, 16-bit hosts 10/12-bit planes (ReadHeifImage.cpp:561-861)
+    return (p.hostDepth == 8 || p.hostDepth == 16) && p.bitDepth <= 12 && (p.hostDepth == 8) == (p.bitDepth <= 8);
+}
+
+Interior DecodePlanarRgbInterior(const DecodeParams& p)
+{
+    return DecodePlanarRgbTuned(p) ? DecodePlanarRgbBlockInterior(p) : Interior{ 0, 0 };
+}
+
+bool DecodeBatchTuned(const DecodeParams& p)
+{
+    if (p.colorspace == AVIFGPU_COLORSPACE_RGB)
+    {
+        return DecodePlanarRgbTuned(p);
+    }
+    return p.hostDepth == 32 ? DecodeYccF32Tuned(p) : DecodeYccIntTuned(p);
+}
 
 namespace
 {

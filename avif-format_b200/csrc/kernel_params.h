@@ -285,8 +285,40 @@ AVIFGPU_HD inline Interior DecodeYccF32BlockInterior(const DecodeParams& p)
 }
 Interior DecodeYccF32Interior(const DecodeParams& p); // DecodeYccF32Tuned ? DecodeYccF32BlockInterior : none
 
-// The description half of whichever tuned YCbCr decode kernel serves the description's host depth: the float one for
-// 32-bit hosts, the integer one otherwise.  Both batch APIs route by it.
+// The same for the tuned planar-RGB decode kernels (StreamDecodeKernel for 8/16-bit hosts, TableDecodeF32Kernel for 32-bit
+// hosts), split the same way.  The description's half: colour space RGB with no or straight alpha; for 8/16-bit hosts at
+// most 12 bits, 8-bit planes into 8-bit hosts and 10/12-bit planes into 16-bit hosts; for 32-bit hosts 10/12-bit planes
+// with the PQ, HLG or SMPTE 428 curve.  The block's half: planes aligned to a thread's 8 samples, rows to its stores, at
+// least 8 pixels and one row.  width is a multiple of 8 and rows is the block's: the interior only ever leaves a right strip.
+bool DecodePlanarRgbTuned(const DecodeParams& p);
+AVIFGPU_HD inline Interior DecodePlanarRgbBlockInterior(const DecodeParams& p)
+{
+    const Interior none = { 0, 0 };
+    const int planeAlign = 8 * (p.hostDepth == 8 ? 1 : 2); // 8-bit hosts read 8-bit planes, the others 10/12-bit ones
+    const int groupBytes = 8 * (p.hasAlpha ? 4 : 3) * (p.hostDepth / 8);
+    const int rowAlign = groupBytes % 16 == 0 ? 16 : 8; // RGB8: 64-bit stores, everything else 128-bit
+    for (int c = 0; c < 3; ++c)
+    {
+        if (!Aligned(p.plane[c], p.planeStride[c], planeAlign))
+        {
+            return none;
+        }
+    }
+    if ((p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], planeAlign)) || !Aligned(p.rows, p.rowStride, rowAlign))
+    {
+        return none;
+    }
+    const int width8 = p.width & ~7;
+    if (width8 < 8 || p.rowCount < 1)
+    {
+        return none;
+    }
+    return Interior{ width8, p.rowCount };
+}
+Interior DecodePlanarRgbInterior(const DecodeParams& p); // DecodePlanarRgbTuned ? DecodePlanarRgbBlockInterior : none
+
+// The description half of whichever tuned decode kernel serves the description: the planar-RGB one for colour space RGB,
+// otherwise the float YCbCr one for 32-bit hosts and the integer one for the others.  Both batch APIs route by it.
 bool DecodeBatchTuned(const DecodeParams& p);
 
 // The pixel-independent factors of the float decode's channel sums, YuvDecode.cpp:555-557 and :308 -- the reference's
@@ -336,7 +368,7 @@ struct BatchRecord
 
 constexpr int kBatchChunkImages = 64;
 constexpr int kBatchUnitPixels = 256; // interior unit: 256 pixels of one row (row pair for 4:2:0), one warp
-constexpr int kF32BatchUnitPixels = 128; // the float decode's interior unit: its single-image kernel's 128-pixel tile
+constexpr int kF32BatchUnitPixels = 128; // the float YCbCr decode's interior unit: its single-image kernel's 128-pixel tile
 constexpr int kBatchEdgeThreads = 256; // edge unit: one CTA-sized run of chroma sites (encode) or pixels (decode) of one row (pair)
 
 // Units of an interior of `width` x `rows` pixels, and of an edge window.
@@ -344,8 +376,12 @@ AVIFGPU_HD inline int64_t BatchInteriorUnits(int width, int rows, int ys, int un
 {
     return static_cast<int64_t>((width + unitPixels - 1) / unitPixels) * ((rows + ys) >> ys);
 }
-// The interior unit width of a decode into `hostDepth`-bit hosts.
-AVIFGPU_HD inline int DecodeBatchUnitPixels(int hostDepth) { return hostDepth == 32 ? kF32BatchUnitPixels : kBatchUnitPixels; }
+// The interior unit width of a decode of `colorspace` into `hostDepth`-bit hosts: 128 pixels for YCbCr into 32-bit hosts,
+// 256 for everything else (planar RGB into every host depth).
+AVIFGPU_HD inline int DecodeBatchUnitPixels(int hostDepth, int colorspace)
+{
+    return hostDepth == 32 && colorspace != AVIFGPU_COLORSPACE_RGB ? kF32BatchUnitPixels : kBatchUnitPixels;
+}
 AVIFGPU_HD inline int64_t BatchEdgeUnits(int width, int rows, int xs, int ys)
 {
     return static_cast<int64_t>((((width + xs) >> xs) + kBatchEdgeThreads - 1) / kBatchEdgeThreads) * ((rows + ys) >> ys);

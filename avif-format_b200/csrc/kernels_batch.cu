@@ -13,6 +13,12 @@
 //   DecodeYccToRgbF32BatchKernel  the float-host decode interiors, with LookUpLuma / ChromaSiteTerms / ConvertRows
 //                                 (float_units.cuh); a warp takes one 128-pixel tile of a row (4:2:0 row pair) at a time,
 //                                 and the libm, log2 and unorm tables are staged once per CTA for the whole batch;
+//   DecodePlanarRgbIntBatchKernel the planar-RGB decode interiors into 8/16-bit hosts, with LoadStreamGroup /
+//                                 ConvertRgbGroup (stream_units.cuh); a warp takes one unit (256 pixels of one row, 8 per
+//                                 lane) at a time;
+//   TableDecodeF32BatchKernel     the planar-RGB decode interiors into 32-bit hosts, with TableDecodeGroup
+//                                 (float_units.cuh), in the same units; the libm tables and every code's curve (and alpha)
+//                                 entry are staged once per CTA for the whole batch, not once per CTA per image;
 //   DecodeBatchKernel             the decode windows, with DecodeChunkPixel (generic_units.cuh).
 //
 // Each is a template on where its records come from:
@@ -29,7 +35,10 @@
 #include "generic_units.cuh"
 #include "int_units.cuh"
 #include "kernel_params.h"
+#include "stream_units.cuh"
 #include "../../include/avifgpu.h"
+
+#include <climits>
 
 #include <cuda_runtime.h>
 
@@ -128,12 +137,15 @@ using PlanarChunk = ChunkSource<EncodeParams, 2 * kBatchChunkImages>;
 using YccIntChunk = ChunkSource<IntDecodeParams, kBatchChunkImages>;
 using DecodeEdgeChunk = ChunkSource<DecodeParams, 2 * kBatchChunkImages>;
 using YccF32Chunk = ChunkSource<FastDecodeParams, kBatchChunkImages>;
+using PlanarRgbIntChunk = ChunkSource<StreamDecodeParams, kBatchChunkImages>;
+using PlanarRgbF32Chunk = ChunkSource<TableDecodeParams, kBatchChunkImages>;
 
 // CUDA 12.1+ on Volta and later: at most 32764 bytes of kernel parameters.
 static_assert(sizeof(RgbIntChunk) <= 32764 && sizeof(PlanarChunk) <= 32764 && sizeof(YccIntChunk) <= 32764 && sizeof(DecodeEdgeChunk) <= 32764,
               "a chunk must fit one kernel parameter block");
 static_assert(sizeof(YccF32Chunk) <= 32764, "a float decode chunk must fit one kernel parameter block");
-static_assert(kF32DecodeThreads == kRgbThreads, "the batched kernels share kWarps");
+static_assert(sizeof(PlanarRgbIntChunk) <= 32764 && sizeof(PlanarRgbF32Chunk) <= 32764, "a planar-RGB decode chunk must fit one kernel parameter block");
+static_assert(kF32DecodeThreads == kRgbThreads && kStreamThreads == kRgbThreads && kTableThreads == kRgbThreads, "the batched kernels share kWarps");
 
 // Block-wide exclusive scan of a pair of counts over kPlanThreads threads; every thread gets the block's totals too.
 __device__ __forceinline__ void ScanPair(long long a, long long b, long long& beforeA, long long& beforeB, long long& totalA, long long& totalB)
@@ -464,6 +476,91 @@ __global__ void __launch_bounds__(kF32DecodeThreads, kDecodeBlocksPerSm) DecodeY
     }
 }
 
+// The pixel `column` (a multiple of 8) and row of a warp's lane in planar-RGB unit `unit` of record `r`: 256 pixels of one row.
+__device__ __forceinline__ void PlanarRgbUnitPixel(const BatchRecord& r, long long unit, int lane, int& row, int& column)
+{
+    const int unitsX = (r.width + kBatchUnitPixels - 1) / kBatchUnitPixels;
+    const int local = static_cast<int>(unit - r.firstUnit);
+    row = local / unitsX;
+    column = (local - row * unitsX) * kBatchUnitPixels + lane * 8;
+}
+
+// StreamDecodeKernel's planar-RGB group, one per lane, with the unit's record's pointers.  An interior is 8-pixel aligned, so
+// a lane is wholly inside its row or wholly past its end.
+template <typename Source, typename SampleT, int CHANNELS>
+__global__ void __launch_bounds__(kStreamThreads) DecodePlanarRgbIntBatchKernel(const __grid_constant__ Source s)
+{
+    const typename Source::Walk walk(s);
+    if (walk.Idle(static_cast<long long>(blockIdx.x) * kWarps))
+    {
+        return;
+    }
+    const int count = walk.Count();
+    const int lane = threadIdx.x & 31;
+    const long long warpCount = static_cast<long long>(gridDim.x) * kWarps;
+    int record = 0;
+    for (long long unit = static_cast<long long>(blockIdx.x) * kWarps + (threadIdx.x >> 5); unit < walk.Units(); unit += warpCount)
+    {
+        record = walk.Find(count, record, unit);
+        const BatchRecord& r = walk.Record(record);
+        int row, column;
+        PlanarRgbUnitPixel(r, unit, lane, row, column);
+        if (column >= r.width)
+        {
+            continue;
+        }
+        StreamDecodeParams p = s.shared;
+        for (int k = 0; k < 4; ++k)
+        {
+            p.plane[k] = static_cast<const uint8_t*>(r.plane[k]);
+            p.planeStride[k] = r.planeStride[k];
+        }
+        Raw8<SampleT> raw[CHANNELS];
+        LoadStreamGroup<SampleT, CHANNELS, false>(p, raw, row, column);
+        uint8_t* target = static_cast<uint8_t*>(const_cast<void*>(r.rows)) + row * r.rowStride + static_cast<int64_t>(column) * CHANNELS * sizeof(SampleT);
+        ConvertRgbGroup<SampleT, CHANNELS>(raw, p.maxCode, target);
+    }
+}
+
+// TableDecodeF32Kernel's planar-RGB group, one per lane, with the unit's record's pointers; the tables are staged once per
+// CTA for every image of the launch (one description).
+template <typename Source, int ALPHA>
+__global__ void __launch_bounds__(kTableThreads) TableDecodeF32BatchKernel(const __grid_constant__ Source s)
+{
+    const typename Source::Walk walk(s);
+    if (walk.Idle(static_cast<long long>(blockIdx.x) * kWarps))
+    {
+        return;
+    }
+    const int count = walk.Count();
+    extern __shared__ __align__(16) uint8_t sharedBytes[];
+    const CodeTables tables = StageCodeTables<3, ALPHA>(sharedBytes, s.shared);
+    const float maxCodeFloat = static_cast<float>(s.shared.maxCode);
+    const int lane = threadIdx.x & 31;
+    const long long warpCount = static_cast<long long>(gridDim.x) * kWarps;
+    int record = 0;
+    for (long long unit = static_cast<long long>(blockIdx.x) * kWarps + (threadIdx.x >> 5); unit < walk.Units(); unit += warpCount)
+    {
+        record = walk.Find(count, record, unit);
+        const BatchRecord& r = walk.Record(record);
+        int row, column;
+        PlanarRgbUnitPixel(r, unit, lane, row, column);
+        if (column >= r.width)
+        {
+            continue;
+        }
+        TableDecodeParams p = s.shared;
+        for (int k = 0; k < 4; ++k)
+        {
+            p.plane[k] = static_cast<const uint8_t*>(r.plane[k]);
+            p.planeStride[k] = r.planeStride[k];
+        }
+        p.rows = static_cast<uint8_t*>(const_cast<void*>(r.rows));
+        p.rowStride = r.rowStride;
+        TableDecodeGroup<3, ALPHA>(p, tables, maxCodeFloat, row, column);
+    }
+}
+
 template <typename Source, typename PlaneT, typename HostT>
 __global__ void __launch_bounds__(kBatchEdgeThreads) DecodeBatchKernel(const __grid_constant__ Source s)
 {
@@ -494,6 +591,11 @@ __global__ void __launch_bounds__(kBatchEdgeThreads) DecodeBatchKernel(const __g
         p.yPhase = 0; // every window starts on a 4:2:0 row pair
         DecodeChunkPixel<PlaneT, HostT, kBatchEdgeThreads>(p, t, static_cast<unsigned>(unit - r.firstUnit));
     }
+}
+
+unsigned GridFor(long long blocks, long long cap)
+{
+    return static_cast<unsigned>(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
 // ---- the dispatch ladders, one per kernel, for either source ------------------------------------------------------------
@@ -601,6 +703,40 @@ void LaunchYccF32(const Source& s, const DecodeParams& d, unsigned grid, size_t 
 // The float decode's tables for description `d`.
 size_t F32TableBytesOf(const DecodeParams& d) { return F32TableBytes(d.transfer, d.bitDepth, d.hasAlpha != 0); }
 
+// The planar-RGB interior kernel of description `d` into 8/16-bit hosts (host depth x alpha), capped like
+// StreamDecodeKernel at 16 CTAs per SM.
+template <typename Source>
+void LaunchPlanarRgbInt(const Source& s, const DecodeParams& d, long long blocks, int smCount, cudaStream_t stream)
+{
+    const unsigned grid = GridFor(blocks, static_cast<long long>(smCount) * 16);
+    if (d.hostDepth == 8)
+    {
+        if (d.hasAlpha) DecodePlanarRgbIntBatchKernel<Source, uint8_t, 4><<<grid, kStreamThreads, 0, stream>>>(s);
+        else DecodePlanarRgbIntBatchKernel<Source, uint8_t, 3><<<grid, kStreamThreads, 0, stream>>>(s);
+    }
+    else
+    {
+        if (d.hasAlpha) DecodePlanarRgbIntBatchKernel<Source, uint16_t, 4><<<grid, kStreamThreads, 0, stream>>>(s);
+        else DecodePlanarRgbIntBatchKernel<Source, uint16_t, 3><<<grid, kStreamThreads, 0, stream>>>(s);
+    }
+}
+
+template <typename Source, int ALPHA>
+void LaunchPlanarRgbF32One(const Source& s, long long blocks, int smCount, size_t bytes, cudaStream_t stream)
+{
+    const long long cap = CodeTableGridCap(TableDecodeF32BatchKernel<Source, ALPHA>, bytes, smCount);
+    TableDecodeF32BatchKernel<Source, ALPHA><<<GridFor(blocks, cap), kTableThreads, bytes, stream>>>(s);
+}
+
+// The planar-RGB interior kernel of description `d` into 32-bit hosts (alpha; transfer and OOTF are runtime values, as in
+// TableDecodeF32Kernel), with `bytes` of staged tables, capped like it at the CTAs resident at once.
+template <typename Source>
+void LaunchPlanarRgbF32(const Source& s, const DecodeParams& d, long long blocks, int smCount, size_t bytes, cudaStream_t stream)
+{
+    if (d.hasAlpha) LaunchPlanarRgbF32One<Source, 1>(s, blocks, smCount, bytes, stream);
+    else LaunchPlanarRgbF32One<Source, 0>(s, blocks, smCount, bytes, stream);
+}
+
 // The windows run the generic kernel's instantiation for the host depth (LaunchDecodeGeneric's).
 template <typename Source>
 void LaunchDecodeEdge(const Source& s, int hostDepth, unsigned grid, cudaStream_t stream)
@@ -635,11 +771,6 @@ Chunk ChunkOf(const decltype(Chunk::shared)& shared, const BatchRecord* records,
     return b;
 }
 
-unsigned GridFor(long long blocks, long long cap)
-{
-    return static_cast<unsigned>(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
-}
-
 // `launches` if the launches before it succeeded, else the failure's status.
 int Launched(int launches)
 {
@@ -670,7 +801,17 @@ int LaunchDecodeBatchChunk(const DecodeParams& shared, const BatchChunk& chunk, 
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
     const int smCount = SmCountOrDefault(shared.smCount);
     const long long warps = (chunk.interiorUnits + kWarps - 1) / kWarps; // one warp per unit
-    if (shared.hostDepth == 32)
+    if (shared.colorspace == AVIFGPU_COLORSPACE_RGB && shared.hostDepth == 32)
+    {
+        LaunchPlanarRgbF32(ChunkOf<PlanarRgbF32Chunk>(TableDecodeDescription(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared, warps,
+                           smCount, CodeTableBytes(shared.bitDepth, shared.hasAlpha != 0), stream);
+    }
+    else if (shared.colorspace == AVIFGPU_COLORSPACE_RGB)
+    {
+        LaunchPlanarRgbInt(ChunkOf<PlanarRgbIntChunk>(StreamDecodeDescription(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared, warps,
+                           smCount, stream);
+    }
+    else if (shared.hostDepth == 32)
     {
         LaunchYccF32(ChunkOf<YccF32Chunk>(FillF32Description(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared,
                      GridFor(warps, static_cast<long long>(smCount) * kDecodeBlocksPerSm), F32TableBytesOf(shared), stream);
@@ -729,7 +870,17 @@ int LaunchDecodeIndirect(const DecodeParams& shared, bool tuned, int planeMask, 
         return AVIFGPU_ERR_CUDA;
     }
     // A description the tuned kernel does not take plans no interior unit: its grid returns before staging, so it gets no tables.
-    if (shared.hostDepth == 32)
+    // The grids are the chunk launchers' caps.
+    if (shared.colorspace == AVIFGPU_COLORSPACE_RGB && shared.hostDepth == 32)
+    {
+        LaunchPlanarRgbF32(WorkspaceSource<TableDecodeParams, 0>{ TableDecodeDescription(shared), workspace, maxCount }, shared, LLONG_MAX, smCount,
+                           tuned ? CodeTableBytes(shared.bitDepth, shared.hasAlpha != 0) : 0, stream);
+    }
+    else if (shared.colorspace == AVIFGPU_COLORSPACE_RGB)
+    {
+        LaunchPlanarRgbInt(WorkspaceSource<StreamDecodeParams, 0>{ StreamDecodeDescription(shared), workspace, maxCount }, shared, LLONG_MAX, smCount, stream);
+    }
+    else if (shared.hostDepth == 32)
     {
         LaunchYccF32(WorkspaceSource<FastDecodeParams, 0>{ FillF32Description(shared), workspace, maxCount }, shared,
                      static_cast<unsigned>(smCount * kDecodeBlocksPerSm), tuned ? F32TableBytesOf(shared) : 0, stream);

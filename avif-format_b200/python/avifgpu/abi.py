@@ -8,7 +8,7 @@ import ctypes as C
 
 import numpy as np
 
-API_VERSION = 8
+API_VERSION = 9
 
 # avifgpu_status
 OK = 0

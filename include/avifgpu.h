@@ -50,7 +50,7 @@ extern "C" {
 #define AVIFGPU_EXPORT __attribute__((visibility("default")))
 #endif
 
-#define AVIFGPU_API_VERSION 8
+#define AVIFGPU_API_VERSION 9
 
 typedef enum avifgpu_status
 {
@@ -376,12 +376,14 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
                                                const avifgpu_batch_image* images, int32_t count, void* cuda_stream);
 
 /* The same for decodes: like `count` calls of avifgpu_decode_rows_device with y0 = 0 and nrows = height, one per image, in
- * order.  Images a tuned YCbCr decode takes in a direct call go through chunks of up to 64 images, at most two launches
- * per chunk: the integer one (8/16-bit hosts reading YCbCr 8/10/12-bit, straight or no alpha, aligned buffers,
- * width >= 8) and, since API version 8, the float one (32-bit hosts reading YCbCr 10/12-bit with PQ, HLG or SMPTE 428,
- * straight or no alpha, aligned buffers, equal Cb / Cr strides, width >= 4; HLG once its divisions are verified).  Every
- * other image -- monochrome, planar RGB, premultiplied alpha, 16-bit planes, a misaligned buffer -- takes one direct
- * call, after the chunks.  The first-use work (the verified divisions) is done once per call, outside a capture. */
+ * order.  Images a tuned decode takes in a direct call go through chunks of up to 64 images, at most two launches
+ * per chunk: the integer YCbCr one (8/16-bit hosts reading YCbCr 8/10/12-bit, straight or no alpha, aligned buffers,
+ * width >= 8); since API version 8, the float YCbCr one (32-bit hosts reading YCbCr 10/12-bit with PQ, HLG or SMPTE 428,
+ * straight or no alpha, aligned buffers, equal Cb / Cr strides, width >= 4; HLG once its divisions are verified); and,
+ * since API version 9, the planar-RGB ones (lossless images: 8-bit planes into 8-bit hosts and 10/12-bit planes into
+ * 16-bit hosts, or 10/12-bit planes with PQ, HLG or SMPTE 428 into 32-bit hosts; straight or no alpha, aligned buffers,
+ * width >= 8).  Every other image -- monochrome, premultiplied alpha, 16-bit planes, a misaligned buffer -- takes one
+ * direct call, after the chunks.  The first-use work (the verified divisions) is done once per call, outside a capture. */
 AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
                                                const avifgpu_batch_image* images, int32_t count, void* cuda_stream);
 
@@ -402,8 +404,8 @@ AVIFGPU_EXPORT int avifgpu_batch_workspace_bytes(int32_t max_count, size_t* out_
  *     device_count or device_workspace NULL; desc invalid (validated as for the other calls, its size ignored);
  *     max_count outside [1, 4096]; workspace_bytes below avifgpu_batch_workspace_bytes(max_count).
  *   - Supported descriptions: encode, 8- or 16-bit RGB(A) hosts into planar YCbCr, any alpha state; decode, 8-, 16- or
- *     (since API version 8) 32-bit hosts reading YCbCr with no or straight alpha.  Anything else is
- *     AVIFGPU_ERR_UNSUPPORTED, with no launch.
+ *     (since API version 8) 32-bit hosts reading YCbCr, or (since API version 9) planar RGB, with no or straight alpha.
+ *     Anything else -- monochrome, premultiplied alpha -- is AVIFGPU_ERR_UNSUPPORTED, with no launch.
  *   - Device-side checks.  With n = *device_count: n < 0 or n > max_count converts nothing and sets all max_count
  *     entries of device_status to AVIFGPU_ERR_BAD_PARAM.  Otherwise image i < n gets device_status[i] = 0, or
  *     AVIFGPU_ERR_BAD_PARAM when its width or height is negative, or when it is non-empty and its rows or a plane the
@@ -421,8 +423,8 @@ AVIFGPU_EXPORT int avifgpu_batch_workspace_bytes(int32_t max_count, size_t* out_
  *     divisions are verified, sends every image through the edge kernel: the same output bit for bit, a slower kernel.
  *   - Workspace: one workspace must not serve two calls that can be in flight at the same time.  The library allocates
  *     nothing for this call.
- * Images the tuned integer or float kernels take in a direct call have their aligned interior converted by the interior kernel,
- * their right strip and odd last 4:2:0 row by the edge kernel; every other image is one whole-image window of the edge
+ * Images the tuned integer, float or planar-RGB kernels take in a direct call have their aligned interior converted by the
+ * interior kernel, their right strip and odd last 4:2:0 row by the edge kernel; every other image is one whole-image window of the edge
  * kernel, which runs the generic kernels' own per-site / per-pixel code.
  */
 AVIFGPU_EXPORT int avifgpu_encode_batch_indirect(avifgpu_context* ctx, const avifgpu_encode_desc* desc,

@@ -416,6 +416,7 @@ __device__ __forceinline__ void EncodeRgbIntGroup(const Rgb16Params& p, const fl
 
 constexpr int kUnitPixels = 256; // per row: 32 lanes x 8 pixels
 constexpr int kYccBlocksPerSm = 3; // DecodeYccToRgbIntKernel's and its batched forms' occupancy, and their grid caps per SM
+constexpr int kStreamBlocksPerSm = 16; // the grid cap per SM of the streaming kernels (no table per CTA), single-image and batched, and of the batches' edge kernels
 
 struct IntDecodeParams
 {

@@ -56,6 +56,25 @@ inline cudaError_t AllowDynamicShared(Kernel kernel, int bytes, std::atomic<uint
     }
     return e;
 }
+
+// One exhaustive device check of an arithmetic shortcut: `launch(counter, stream)` enqueues the kernel that adds its
+// disagreements to the cleared device counter.  Returns their number (0 = verified) or -1 on a CUDA error.  Synchronous.
+template <typename Launch>
+inline long long CountDisagreements(cudaStream_t stream, Launch&& launch)
+{
+    unsigned long long* counter = nullptr;
+    if (cudaMalloc(&counter, sizeof(unsigned long long)) != cudaSuccess)
+    {
+        return -1;
+    }
+    cudaMemsetAsync(counter, 0, sizeof(unsigned long long), stream);
+    launch(counter, stream);
+    unsigned long long bad = 0;
+    const bool ok = cudaMemcpyAsync(&bad, counter, sizeof(bad), cudaMemcpyDeviceToHost, stream) == cudaSuccess &&
+                    cudaStreamSynchronize(stream) == cudaSuccess;
+    cudaFree(counter);
+    return ok ? static_cast<long long>(bad) : -1;
+}
 #endif
 
 struct EncodeParams
@@ -191,6 +210,12 @@ AVIFGPU_HD inline bool Aligned(const void* p, int64_t stride, int alignment)
 inline int SmCountOrDefault(int32_t smCount)
 {
     return smCount > 0 ? smCount : 132;
+}
+
+// The grid of a persistent kernel: one CTA per `blocks` of work, at most `cap` (CTAs per SM x SMs) and at least one.
+inline unsigned GridFor(long long blocks, long long cap)
+{
+    return static_cast<unsigned>(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
 // The aligned interior [0, width) x [0, rows) the tuned integer planar encode kernel (EncodeRgbIntPlanarKernel)

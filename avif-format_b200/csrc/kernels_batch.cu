@@ -30,11 +30,13 @@
 //                    is the chunk launchers' cap and a CTA with no unit returns before it stages anything; a worker finds
 //                    its unit's record with a binary search (FindRecord), starting after the record of its previous unit.
 // Either way the search is once per unit and warp- (CTA-) uniform, never per pixel.
+// Which instantiation a description takes is the family's picker's decision (launch_keys.h), as in the single-image launchers.
 #include "batch_plan.h"
 #include "float_units.cuh"
 #include "generic_units.cuh"
 #include "int_units.cuh"
 #include "kernel_params.h"
+#include "launch_keys.h"
 #include "stream_units.cuh"
 #include "../../include/avifgpu.h"
 
@@ -593,75 +595,31 @@ __global__ void __launch_bounds__(kBatchEdgeThreads) DecodeBatchKernel(const __g
     }
 }
 
-unsigned GridFor(long long blocks, long long cap)
-{
-    return static_cast<unsigned>(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
-}
+// ---- the launches, one per kernel family, for either source: the family's picker (launch_keys.h) chooses the instantiation ----
 
-// ---- the dispatch ladders, one per kernel, for either source ------------------------------------------------------------
-
-template <typename Source, typename HostT, typename PlaneT, int CHANNELS, int PREMULTIPLY>
-void LaunchRgbIntChroma(const Source& s, int xs, int ys, unsigned grid, cudaStream_t stream)
-{
-    if (xs == 1 && ys == 1) EncodeRgbIntBatchKernel<Source, HostT, PlaneT, CHANNELS, 1, 1, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(s);
-    else if (xs == 1) EncodeRgbIntBatchKernel<Source, HostT, PlaneT, CHANNELS, 1, 0, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(s);
-    else EncodeRgbIntBatchKernel<Source, HostT, PlaneT, CHANNELS, 0, 0, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(s);
-}
-
-template <typename Source, typename HostT, typename PlaneT>
-void LaunchRgbIntChannels(const Source& s, const EncodeParams& d, unsigned grid, cudaStream_t stream)
-{
-    if (d.channels == 4 && d.premultiply) LaunchRgbIntChroma<Source, HostT, PlaneT, 4, 1>(s, d.xs, d.ys, grid, stream);
-    else if (d.channels == 4) LaunchRgbIntChroma<Source, HostT, PlaneT, 4, 0>(s, d.xs, d.ys, grid, stream);
-    else LaunchRgbIntChroma<Source, HostT, PlaneT, 3, 0>(s, d.xs, d.ys, grid, stream);
-}
-
-// The interior kernel of description `d`: host depth x plane depth x channels / premultiply x chroma.
+// The encode interiors.
 template <typename Source>
 void LaunchRgbInt(const Source& s, const EncodeParams& d, int hostDepth, unsigned grid, cudaStream_t stream)
 {
-    const bool wide = d.imageDepth > 8;
-    if (hostDepth == 16)
-    {
-        if (wide) LaunchRgbIntChannels<Source, uint16_t, uint16_t>(s, d, grid, stream);
-        else LaunchRgbIntChannels<Source, uint16_t, uint8_t>(s, d, grid, stream);
-    }
-    else
-    {
-        if (wide) LaunchRgbIntChannels<Source, uint8_t, uint16_t>(s, d, grid, stream);
-        else LaunchRgbIntChannels<Source, uint8_t, uint8_t>(s, d, grid, stream);
-    }
+    WithRgbIntKey(d, hostDepth, [&](auto host, auto plane, auto channels, auto premultiply, auto xs, auto ys) {
+        EncodeRgbIntBatchKernel<Source, TypeOf<decltype(host)>, TypeOf<decltype(plane)>, channels(), xs(), ys(), premultiply()><<<grid, kRgbThreads, 0, stream>>>(s);
+    });
 }
 
+// The windows of an encode batch: its hosts are 8- or 16-bit.
 template <typename Source>
 void LaunchPlanar(const Source& s, int hostDepth, unsigned grid, cudaStream_t stream)
 {
-    if (hostDepth == 16) EncodePlanarBatchKernel<Source, uint16_t><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
-    else EncodePlanarBatchKernel<Source, uint8_t><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
+    WithIntHost(hostDepth, [&](auto host) { EncodePlanarBatchKernel<Source, TypeOf<decltype(host)>><<<grid, kBatchEdgeThreads, 0, stream>>>(s); });
 }
 
-template <typename Source, typename SampleT, int ALPHA>
-void LaunchYccIntChroma(const Source& s, int xs, int ys, unsigned grid, size_t bytes, cudaStream_t stream)
-{
-    if (xs == 1 && ys == 1) DecodeYccToRgbIntBatchKernel<Source, SampleT, 1, 1, ALPHA><<<grid, kRgbThreads, bytes, stream>>>(s);
-    else if (xs == 1) DecodeYccToRgbIntBatchKernel<Source, SampleT, 1, 0, ALPHA><<<grid, kRgbThreads, bytes, stream>>>(s);
-    else DecodeYccToRgbIntBatchKernel<Source, SampleT, 0, 0, ALPHA><<<grid, kRgbThreads, bytes, stream>>>(s);
-}
-
-// The interior kernel of description `d` (host depth x alpha x chroma), with `bytes` of staged tables.
+// The YCbCr decode interiors into 8/16-bit hosts, with `bytes` of staged tables.
 template <typename Source>
 void LaunchYccInt(const Source& s, const DecodeParams& d, unsigned grid, size_t bytes, cudaStream_t stream)
 {
-    if (d.hostDepth == 8)
-    {
-        if (d.hasAlpha) LaunchYccIntChroma<Source, uint8_t, 1>(s, d.xs, d.ys, grid, bytes, stream);
-        else LaunchYccIntChroma<Source, uint8_t, 0>(s, d.xs, d.ys, grid, bytes, stream);
-    }
-    else
-    {
-        if (d.hasAlpha) LaunchYccIntChroma<Source, uint16_t, 1>(s, d.xs, d.ys, grid, bytes, stream);
-        else LaunchYccIntChroma<Source, uint16_t, 0>(s, d.xs, d.ys, grid, bytes, stream);
-    }
+    WithYccIntKey(d, [&](auto sample, auto alpha, auto xs, auto ys) {
+        DecodeYccToRgbIntBatchKernel<Source, TypeOf<decltype(sample)>, xs(), ys(), alpha()><<<grid, kRgbThreads, bytes, stream>>>(s);
+    });
 }
 
 template <typename Source, int XS, int YS, int TRANSFER, int ALPHA, int FASTDIV>
@@ -674,76 +632,45 @@ void LaunchYccF32One(const Source& s, unsigned grid, size_t bytes, cudaStream_t 
     } // else the failed attribute call is the error Launched() finds
 }
 
-template <typename Source, int TRANSFER, int ALPHA, int FASTDIV>
-void LaunchYccF32Chroma(const Source& s, int xs, int ys, unsigned grid, size_t bytes, cudaStream_t stream)
-{
-    if (xs == 1 && ys == 1) LaunchYccF32One<Source, 1, 1, TRANSFER, ALPHA, FASTDIV>(s, grid, bytes, stream);
-    else if (xs == 1) LaunchYccF32One<Source, 1, 0, TRANSFER, ALPHA, FASTDIV>(s, grid, bytes, stream);
-    else LaunchYccF32One<Source, 0, 0, TRANSFER, ALPHA, FASTDIV>(s, grid, bytes, stream);
-}
-
-template <typename Source, int TRANSFER, int FASTDIV = 0>
-void LaunchYccF32Alpha(const Source& s, const DecodeParams& d, unsigned grid, size_t bytes, cudaStream_t stream)
-{
-    if (d.hasAlpha) LaunchYccF32Chroma<Source, TRANSFER, 1, FASTDIV>(s, d.xs, d.ys, grid, bytes, stream);
-    else LaunchYccF32Chroma<Source, TRANSFER, 0, FASTDIV>(s, d.xs, d.ys, grid, bytes, stream);
-}
-
-// The float interior kernel of description `d` (transfer / verified PQ division x alpha x chroma), with `bytes` of staged
-// tables.  The single-image launcher's ladder: DecodeYccF32Tuned leaves PQ, HLG and SMPTE 428.
+// The YCbCr decode interiors into 32-bit hosts, with `bytes` of staged tables.
 template <typename Source>
 void LaunchYccF32(const Source& s, const DecodeParams& d, unsigned grid, size_t bytes, cudaStream_t stream)
 {
-    if (d.transfer == AVIFGPU_TRANSFER_PQ && d.verifiedPqRatio) LaunchYccF32Alpha<Source, AVIFGPU_TRANSFER_PQ, 1>(s, d, grid, bytes, stream);
-    else if (d.transfer == AVIFGPU_TRANSFER_PQ) LaunchYccF32Alpha<Source, AVIFGPU_TRANSFER_PQ, 0>(s, d, grid, bytes, stream);
-    else if (d.transfer == AVIFGPU_TRANSFER_HLG) LaunchYccF32Alpha<Source, AVIFGPU_TRANSFER_HLG>(s, d, grid, bytes, stream);
-    else LaunchYccF32Alpha<Source, AVIFGPU_TRANSFER_SMPTE428>(s, d, grid, bytes, stream);
+    WithYccF32Key(d, [&](auto transfer, auto fastDiv, auto alpha, auto xs, auto ys) {
+        LaunchYccF32One<Source, xs(), ys(), transfer(), alpha(), fastDiv()>(s, grid, bytes, stream);
+    });
 }
 
 // The float decode's tables for description `d`.
 size_t F32TableBytesOf(const DecodeParams& d) { return F32TableBytes(d.transfer, d.bitDepth, d.hasAlpha != 0); }
 
-// The planar-RGB interior kernel of description `d` into 8/16-bit hosts (host depth x alpha), capped like
-// StreamDecodeKernel at 16 CTAs per SM.
+// The planar-RGB decode interiors into 8/16-bit hosts.
 template <typename Source>
 void LaunchPlanarRgbInt(const Source& s, const DecodeParams& d, long long blocks, int smCount, cudaStream_t stream)
 {
-    const unsigned grid = GridFor(blocks, static_cast<long long>(smCount) * 16);
-    if (d.hostDepth == 8)
-    {
-        if (d.hasAlpha) DecodePlanarRgbIntBatchKernel<Source, uint8_t, 4><<<grid, kStreamThreads, 0, stream>>>(s);
-        else DecodePlanarRgbIntBatchKernel<Source, uint8_t, 3><<<grid, kStreamThreads, 0, stream>>>(s);
-    }
-    else
-    {
-        if (d.hasAlpha) DecodePlanarRgbIntBatchKernel<Source, uint16_t, 4><<<grid, kStreamThreads, 0, stream>>>(s);
-        else DecodePlanarRgbIntBatchKernel<Source, uint16_t, 3><<<grid, kStreamThreads, 0, stream>>>(s);
-    }
+    const unsigned grid = GridFor(blocks, static_cast<long long>(smCount) * kStreamBlocksPerSm);
+    WithIntDecodeKey(d, [&](auto sample, auto alpha) {
+        DecodePlanarRgbIntBatchKernel<Source, TypeOf<decltype(sample)>, 3 + alpha()><<<grid, kStreamThreads, 0, stream>>>(s);
+    });
 }
 
-template <typename Source, int ALPHA>
-void LaunchPlanarRgbF32One(const Source& s, long long blocks, int smCount, size_t bytes, cudaStream_t stream)
-{
-    const long long cap = CodeTableGridCap(TableDecodeF32BatchKernel<Source, ALPHA>, bytes, smCount);
-    TableDecodeF32BatchKernel<Source, ALPHA><<<GridFor(blocks, cap), kTableThreads, bytes, stream>>>(s);
-}
-
-// The planar-RGB interior kernel of description `d` into 32-bit hosts (alpha; transfer and OOTF are runtime values, as in
-// TableDecodeF32Kernel), with `bytes` of staged tables, capped like it at the CTAs resident at once.
+// The planar-RGB decode interiors into 32-bit hosts, with `bytes` of staged tables, capped at the CTAs resident at once.
 template <typename Source>
 void LaunchPlanarRgbF32(const Source& s, const DecodeParams& d, long long blocks, int smCount, size_t bytes, cudaStream_t stream)
 {
-    if (d.hasAlpha) LaunchPlanarRgbF32One<Source, 1>(s, blocks, smCount, bytes, stream);
-    else LaunchPlanarRgbF32One<Source, 0>(s, blocks, smCount, bytes, stream);
+    WithTableF32Key(d, [&](auto alpha) {
+        const long long cap = CodeTableGridCap(TableDecodeF32BatchKernel<Source, alpha()>, bytes, smCount);
+        TableDecodeF32BatchKernel<Source, alpha()><<<GridFor(blocks, cap), kTableThreads, bytes, stream>>>(s);
+    });
 }
 
-// The windows run the generic kernel's instantiation for the host depth (LaunchDecodeGeneric's).
+// The windows of a decode batch.
 template <typename Source>
 void LaunchDecodeEdge(const Source& s, int hostDepth, unsigned grid, cudaStream_t stream)
 {
-    if (hostDepth == 32) DecodeBatchKernel<Source, uint16_t, float><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
-    else if (hostDepth == 16) DecodeBatchKernel<Source, uint16_t, uint16_t><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
-    else DecodeBatchKernel<Source, uint8_t, uint8_t><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
+    WithHostDepth(hostDepth, [&](auto plane, auto host) {
+        DecodeBatchKernel<Source, TypeOf<decltype(plane)>, TypeOf<decltype(host)>><<<grid, kBatchEdgeThreads, 0, stream>>>(s);
+    });
 }
 
 // DecodeYccToRgbIntKernel's tables for description `d`.
@@ -783,7 +710,7 @@ int Launched(int launches)
 int LaunchEncodeBatchChunk(const EncodeParams& shared, int hostDepth, const BatchChunk& chunk, void* streamHandle)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
-    const long long cap = static_cast<long long>(SmCountOrDefault(shared.smCount)) * 16; // the single-image kernel's cap of 16 CTAs per SM
+    const long long cap = static_cast<long long>(SmCountOrDefault(shared.smCount)) * kStreamBlocksPerSm;
     // one warp per unit
     LaunchRgbInt(ChunkOf<RgbIntChunk>(RgbIntShared(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared, hostDepth,
                  GridFor((chunk.interiorUnits + kWarps - 1) / kWarps, cap), stream);
@@ -827,7 +754,7 @@ int LaunchDecodeBatchChunk(const DecodeParams& shared, const BatchChunk& chunk, 
         return interior;
     }
     LaunchDecodeEdge(ChunkOf<DecodeEdgeChunk>(shared, chunk.window, chunk.windows, chunk.windowUnits), shared.hostDepth,
-                     GridFor(chunk.windowUnits, static_cast<long long>(smCount) * 16), stream);
+                     GridFor(chunk.windowUnits, static_cast<long long>(smCount) * kStreamBlocksPerSm), stream);
     return Launched(2);
 }
 
@@ -835,7 +762,7 @@ int LaunchEncodeIndirect(const EncodeParams& shared, int hostDepth, bool tuned, 
                          const int32_t* count, int maxCount, void* workspace, int32_t* status, void* streamHandle)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
-    const unsigned cap = static_cast<unsigned>(SmCountOrDefault(shared.smCount)) * 16; // the chunk launchers' caps
+    const unsigned cap = static_cast<unsigned>(SmCountOrDefault(shared.smCount)) * kStreamBlocksPerSm; // the chunk launchers' caps
     EncodePlanner planner{};
     planner.shared = shared;
     planner.hostDepth = hostDepth;
@@ -894,7 +821,7 @@ int LaunchDecodeIndirect(const DecodeParams& shared, bool tuned, int planeMask, 
     {
         return AVIFGPU_ERR_CUDA;
     }
-    LaunchDecodeEdge(WorkspaceSource<DecodeParams, 1>{ shared, workspace, maxCount }, shared.hostDepth, static_cast<unsigned>(smCount * 16), stream);
+    LaunchDecodeEdge(WorkspaceSource<DecodeParams, 1>{ shared, workspace, maxCount }, shared.hostDepth, static_cast<unsigned>(smCount * kStreamBlocksPerSm), stream);
     return Launched(3);
 }
 

@@ -8,6 +8,7 @@
 //                                                       filter needs no cross-lane traffic), 3 x LDG.128 per row per lane
 //                                                       one tile ahead, persistent grid of 3 CTAs x 8 warps per SM.
 #include "kernels_fast_common.cuh"
+#include "launch_keys.h"
 #include "../../include/avifgpu.h"
 
 #include <cuda_runtime.h>
@@ -111,21 +112,9 @@ cudaError_t LaunchClipKernel(const FastEncodeParams& fp, int smCount, cudaStream
     {
         return cudaErrorInvalidValue;
     }
-    long long blocks = (tiles + kClipWarps - 1) / kClipWarps;
-    const long long resident = static_cast<long long>(smCount) * kClipBlocksPerSm;
-    if (blocks > resident)
-    {
-        blocks = resident;
-    }
-    EncodeRgbF32ClipKernel<XS, YS><<<static_cast<unsigned>(blocks), kClipThreads, 0, stream>>>(fp);
+    const unsigned grid = GridFor((tiles + kClipWarps - 1) / kClipWarps, static_cast<long long>(smCount) * kClipBlocksPerSm);
+    EncodeRgbF32ClipKernel<XS, YS><<<grid, kClipThreads, 0, stream>>>(fp);
     return cudaGetLastError();
-}
-
-cudaError_t DispatchClip(const FastEncodeParams& fp, int xs, int ys, int smCount, cudaStream_t stream)
-{
-    if (xs == 1 && ys == 1) return LaunchClipKernel<1, 1>(fp, smCount, stream);
-    if (xs == 1) return LaunchClipKernel<1, 0>(fp, smCount, stream);
-    return LaunchClipKernel<0, 0>(fp, smCount, stream);
 }
 
 } // namespace
@@ -249,7 +238,7 @@ int LaunchEncodeFast(const EncodeParams& p, int hostDepth, void* streamHandle)
     }
     else
     {
-        e = DispatchClip(fp, p.xs, p.ys, smCount, stream);
+        e = WithChroma(p.xs, p.ys, [&](auto xs, auto ys) { return LaunchClipKernel<xs(), ys()>(fp, smCount, stream); });
     }
     return CompleteEncode(e, p, hostDepth, width4, evenRows, streamHandle);
 }

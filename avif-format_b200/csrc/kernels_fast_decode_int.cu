@@ -14,6 +14,7 @@
 #include "group_walk.cuh"
 #include "int_units.cuh"
 #include "kernel_params.h"
+#include "launch_keys.h"
 #include "packed_f32x2.cuh"
 #include "pixel_math.cuh"
 #include "stream_units.cuh"
@@ -110,22 +111,9 @@ cudaError_t LaunchOne(const IntDecodeParams& fp, int smCount, cudaStream_t strea
     }
     constexpr int rowsPerUnit = YS ? 2 : 1;
     const long long units = static_cast<long long>((fp.width + kUnitPixels - 1) / kUnitPixels) * ((fp.rowCount + rowsPerUnit - 1) / rowsPerUnit);
-    long long blocks = (units + kWarps - 1) / kWarps;
-    const long long resident = static_cast<long long>(smCount) * kYccBlocksPerSm;
-    if (blocks > resident)
-    {
-        blocks = resident;
-    }
-    DecodeYccToRgbIntKernel<SampleT, XS, YS, ALPHA><<<static_cast<unsigned>(blocks), kThreads, shared, stream>>>(fp);
+    const unsigned grid = GridFor((units + kWarps - 1) / kWarps, static_cast<long long>(smCount) * kYccBlocksPerSm);
+    DecodeYccToRgbIntKernel<SampleT, XS, YS, ALPHA><<<grid, kThreads, shared, stream>>>(fp);
     return cudaGetLastError();
-}
-
-template <typename SampleT, int ALPHA>
-cudaError_t DispatchChroma(const IntDecodeParams& fp, int xs, int ys, int smCount, cudaStream_t stream)
-{
-    if (xs == 1 && ys == 1) return LaunchOne<SampleT, 1, 1, ALPHA>(fp, smCount, stream);
-    if (xs == 1) return LaunchOne<SampleT, 1, 0, ALPHA>(fp, smCount, stream);
-    return LaunchOne<SampleT, 0, 0, ALPHA>(fp, smCount, stream);
 }
 
 // ---- monochrome and planar-RGB images: pure streaming ------------------------------------------------------------------
@@ -255,12 +243,9 @@ template <typename SampleT, int CHANNELS, bool MONO>
 cudaError_t LaunchStream(const StreamDecodeParams& sp, int smCount, cudaStream_t stream)
 {
     const long long groups = static_cast<long long>(sp.groupsPerRow) * sp.rowCount;
-    long long blocks = (groups + kStreamThreads - 1) / kStreamThreads;
-    const long long cap = static_cast<long long>(smCount) * 16;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
+    const unsigned grid = GridFor((groups + kStreamThreads - 1) / kStreamThreads, static_cast<long long>(smCount) * kStreamBlocksPerSm);
     const size_t shared = MONO ? 2 * sizeof(uint16_t) * (static_cast<size_t>(1) << sp.bitDepth) : 0;
-    StreamDecodeKernel<SampleT, CHANNELS, MONO><<<static_cast<unsigned>(blocks), kStreamThreads, shared, stream>>>(sp);
+    StreamDecodeKernel<SampleT, CHANNELS, MONO><<<grid, kStreamThreads, shared, stream>>>(sp);
     return cudaGetLastError();
 }
 
@@ -313,17 +298,10 @@ static int LaunchDecodeStream(const DecodeParams& p, void* streamHandle)
     sp.groupsPerRow = inner.width / 8;
     sp.rowCount = inner.rows;
     const int smCount = SmCountOrDefault(p.smCount);
-    cudaError_t e;
-    if (p.hostDepth == 8)
-    {
-        if (mono) e = p.hasAlpha ? LaunchStream<uint8_t, 2, true>(sp, smCount, stream) : LaunchStream<uint8_t, 1, true>(sp, smCount, stream);
-        else e = p.hasAlpha ? LaunchStream<uint8_t, 4, false>(sp, smCount, stream) : LaunchStream<uint8_t, 3, false>(sp, smCount, stream);
-    }
-    else
-    {
-        if (mono) e = p.hasAlpha ? LaunchStream<uint16_t, 2, true>(sp, smCount, stream) : LaunchStream<uint16_t, 1, true>(sp, smCount, stream);
-        else e = p.hasAlpha ? LaunchStream<uint16_t, 4, false>(sp, smCount, stream) : LaunchStream<uint16_t, 3, false>(sp, smCount, stream);
-    }
+    const cudaError_t e = WithIntDecodeKey(p, [&](auto sample, auto alpha) {
+        using SampleT = TypeOf<decltype(sample)>;
+        return mono ? LaunchStream<SampleT, 1 + alpha(), true>(sp, smCount, stream) : LaunchStream<SampleT, 3 + alpha(), false>(sp, smCount, stream);
+    });
     return CompleteDecode(e, p, inner.width, inner.rows, streamHandle);
 }
 
@@ -344,7 +322,6 @@ int LaunchDecodeFastInteger(const DecodeParams& p, void* streamHandle)
     {
         return 0;
     }
-    const int sampleBytes = p.hostDepth == 8 ? 1 : 2;
     const int width8 = inner.width;
     const int evenRows = inner.rows;
     IntDecodeParams fp = IntDecodeShared(p);
@@ -359,15 +336,9 @@ int LaunchDecodeFastInteger(const DecodeParams& p, void* streamHandle)
     fp.rowCount = evenRows;
 
     const int smCount = SmCountOrDefault(p.smCount);
-    cudaError_t e;
-    if (sampleBytes == 1)
-    {
-        e = p.hasAlpha ? DispatchChroma<uint8_t, 1>(fp, p.xs, p.ys, smCount, stream) : DispatchChroma<uint8_t, 0>(fp, p.xs, p.ys, smCount, stream);
-    }
-    else
-    {
-        e = p.hasAlpha ? DispatchChroma<uint16_t, 1>(fp, p.xs, p.ys, smCount, stream) : DispatchChroma<uint16_t, 0>(fp, p.xs, p.ys, smCount, stream);
-    }
+    const cudaError_t e = WithYccIntKey(p, [&](auto sample, auto alpha, auto xs, auto ys) {
+        return LaunchOne<TypeOf<decltype(sample)>, xs(), ys(), alpha()>(fp, smCount, stream);
+    });
     return CompleteDecode(e, p, width8, evenRows, streamHandle);
 }
 

@@ -14,6 +14,7 @@
 #include "float_units.cuh"
 #include "group_walk.cuh"
 #include "kernel_params.h"
+#include "launch_keys.h"
 #include "../../include/avifgpu.h"
 
 #include <cuda_runtime.h>
@@ -45,13 +46,10 @@ template <int COLOURS, int ALPHA>
 cudaError_t LaunchTable(const TableDecodeParams& tp, int smCount, cudaStream_t stream)
 {
     const long long groups = static_cast<long long>(tp.groupsPerRow) * tp.rowCount;
-    long long blocks = (groups + kTableThreads - 1) / kTableThreads;
     const size_t shared = CodeTableBytes(tp.bitDepth, ALPHA != 0);
     // each CTA pays for its own table: exactly as many as are resident at once (4 at 52 registers, 8 at 32), long-lived
     const long long cap = CodeTableGridCap(TableDecodeF32Kernel<COLOURS, ALPHA>, shared, smCount);
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    TableDecodeF32Kernel<COLOURS, ALPHA><<<static_cast<unsigned>(blocks), kTableThreads, shared, stream>>>(tp);
+    TableDecodeF32Kernel<COLOURS, ALPHA><<<GridFor((groups + kTableThreads - 1) / kTableThreads, cap), kTableThreads, shared, stream>>>(tp);
     return cudaGetLastError();
 }
 
@@ -118,9 +116,9 @@ int LaunchDecodeFastTable(const DecodeParams& p, void* streamHandle)
     tp.groupsPerRow = inner.width / 8;
     tp.rowCount = inner.rows;
     const int smCount = SmCountOrDefault(p.smCount);
-    cudaError_t e;
-    if (mono) e = p.hasAlpha ? LaunchTable<1, 1>(tp, smCount, stream) : LaunchTable<1, 0>(tp, smCount, stream);
-    else e = p.hasAlpha ? LaunchTable<3, 1>(tp, smCount, stream) : LaunchTable<3, 0>(tp, smCount, stream);
+    const cudaError_t e = WithTableF32Key(p, [&](auto alpha) {
+        return mono ? LaunchTable<1, alpha()>(tp, smCount, stream) : LaunchTable<3, alpha()>(tp, smCount, stream);
+    });
     return CompleteDecode(e, p, inner.width, inner.rows, streamHandle);
 }
 

@@ -17,6 +17,7 @@
 //     bitmap, up to two samples of a lane at a time; +inf / NaN take the exact glibc-identical evaluation;
 //   * forward matrix, quantisation, chroma down-filter and stores: StoreTile (kernels_fast_common.cuh, packed FP32).
 #include "kernels_fast_common.cuh"
+#include "launch_keys.h"
 #include "table_staging.cuh"
 #include "../../include/avifgpu.h"
 
@@ -391,14 +392,6 @@ cudaError_t LaunchFlatKernel(const FastEncodeParams& fp, int smCount, cudaStream
     return cudaGetLastError();
 }
 
-template <int CURVE, int TABLE>
-cudaError_t DispatchFlatChroma(const FastEncodeParams& fp, int xs, int ys, int smCount, cudaStream_t stream)
-{
-    if (xs == 1 && ys == 1) return LaunchFlatKernel<CURVE, 1, 1, TABLE>(fp, smCount, stream);
-    if (xs == 1) return LaunchFlatKernel<CURVE, 1, 0, TABLE>(fp, smCount, stream);
-    return LaunchFlatKernel<CURVE, 0, 0, TABLE>(fp, smCount, stream);
-}
-
 } // namespace
 
 static bool CompactTableFits(const FastEncodeParams& fp)
@@ -438,17 +431,19 @@ cudaError_t LaunchFastEncodeFlatInterleaved(const FastEncodeParams& fp, int curv
 
 cudaError_t LaunchFastEncodeFlat(const FastEncodeParams& fp, int curve, int xs, int ys, int smCount, cudaStream_t stream)
 {
-    if (CompactTableFits(fp))
-    {
-        if (curve == kCurveLinearToPQ)
+    return WithChroma(xs, ys, [&](auto XS, auto YS) {
+        if (CompactTableFits(fp))
         {
-            return fp.table.flatShift == 14 ? DispatchFlatChroma<kCurveLinearToPQ, kTableCompact14>(fp, xs, ys, smCount, stream)
-                                            : DispatchFlatChroma<kCurveLinearToPQ, kTableCompact>(fp, xs, ys, smCount, stream);
+            if (curve == kCurveLinearToPQ)
+            {
+                return fp.table.flatShift == 14 ? LaunchFlatKernel<kCurveLinearToPQ, XS(), YS(), kTableCompact14>(fp, smCount, stream)
+                                                : LaunchFlatKernel<kCurveLinearToPQ, XS(), YS(), kTableCompact>(fp, smCount, stream);
+            }
+            return LaunchFlatKernel<kCurveLinearToSMPTE428, XS(), YS(), kTableCompact>(fp, smCount, stream);
         }
-        return DispatchFlatChroma<kCurveLinearToSMPTE428, kTableCompact>(fp, xs, ys, smCount, stream);
-    }
-    if (curve == kCurveLinearToPQ) return DispatchFlatChroma<kCurveLinearToPQ, kTableTwoLevel>(fp, xs, ys, smCount, stream);
-    return DispatchFlatChroma<kCurveLinearToSMPTE428, kTableTwoLevel>(fp, xs, ys, smCount, stream);
+        if (curve == kCurveLinearToPQ) return LaunchFlatKernel<kCurveLinearToPQ, XS(), YS(), kTableTwoLevel>(fp, smCount, stream);
+        return LaunchFlatKernel<kCurveLinearToSMPTE428, XS(), YS(), kTableTwoLevel>(fp, smCount, stream);
+    });
 }
 
 } // namespace avifgpu

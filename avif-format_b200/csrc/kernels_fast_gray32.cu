@@ -234,11 +234,8 @@ cudaError_t LaunchGray32(const Gray32Params& gp, size_t shared, int smCount, cud
     }
     constexpr int kThreads = PQ ? kGrayTableThreads : kGrayClipThreads;
     const long long groups = static_cast<long long>(gp.groupsPerRow) * gp.rowCount;
-    long long blocks = (groups + kThreads - 1) / kThreads;
     const long long cap = PQ ? static_cast<long long>(smCount) : static_cast<long long>(smCount) * 8; // a table per CTA: one long-lived CTA per SM
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    EncodeGrayF32Kernel<CHANNELS, PQ><<<static_cast<unsigned>(blocks), kThreads, shared, stream>>>(gp);
+    EncodeGrayF32Kernel<CHANNELS, PQ><<<GridFor((groups + kThreads - 1) / kThreads, cap), kThreads, shared, stream>>>(gp);
     return cudaGetLastError();
 }
 

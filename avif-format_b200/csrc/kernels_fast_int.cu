@@ -12,6 +12,7 @@
 #include "group_walk.cuh"
 #include "int_units.cuh"
 #include "kernel_params.h"
+#include "launch_keys.h"
 #include "packed_f32x2.cuh"
 #include "../../include/avifgpu.h"
 
@@ -290,36 +291,19 @@ template <typename HostT, typename PlaneT>
 cudaError_t LaunchGrayInt(const Rgb16Params& rp, int channels, int smCount, cudaStream_t stream)
 {
     const long long groups = static_cast<long long>(rp.groupsPerRow) * rp.rowCount;
-    long long blocks = (groups + kRgbThreads - 1) / kRgbThreads;
-    const long long cap = static_cast<long long>(smCount) * 16;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    const unsigned grid = static_cast<unsigned>(blocks);
+    const unsigned grid = GridFor((groups + kRgbThreads - 1) / kRgbThreads, static_cast<long long>(smCount) * kStreamBlocksPerSm);
     if (channels == 2) EncodeGrayIntKernel<HostT, PlaneT, 2><<<grid, kRgbThreads, 0, stream>>>(rp);
     else EncodeGrayIntKernel<HostT, PlaneT, 1><<<grid, kRgbThreads, 0, stream>>>(rp);
     return cudaGetLastError();
 }
 
-template <typename HostT, typename PlaneT, int CHANNELS, int PREMULTIPLY>
-cudaError_t LaunchRgbInt(const Rgb16Params& rp, int xs, int ys, int smCount, cudaStream_t stream)
+template <typename HostT, typename PlaneT, int CHANNELS, int XS, int YS, int PREMULTIPLY>
+cudaError_t LaunchRgbInt(const Rgb16Params& rp, int smCount, cudaStream_t stream)
 {
-    const long long groups = static_cast<long long>(rp.groupsPerRow) * ((rp.rowCount + ys) >> ys);
-    long long blocks = (groups + kRgbThreads - 1) / kRgbThreads;
-    const long long cap = static_cast<long long>(smCount) * 16;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    const unsigned grid = static_cast<unsigned>(blocks);
-    if (xs == 1 && ys == 1) EncodeRgbIntPlanarKernel<HostT, PlaneT, CHANNELS, 1, 1, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(rp);
-    else if (xs == 1) EncodeRgbIntPlanarKernel<HostT, PlaneT, CHANNELS, 1, 0, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(rp);
-    else EncodeRgbIntPlanarKernel<HostT, PlaneT, CHANNELS, 0, 0, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(rp);
+    const long long groups = static_cast<long long>(rp.groupsPerRow) * ((rp.rowCount + YS) >> YS);
+    const unsigned grid = GridFor((groups + kRgbThreads - 1) / kRgbThreads, static_cast<long long>(smCount) * kStreamBlocksPerSm);
+    EncodeRgbIntPlanarKernel<HostT, PlaneT, CHANNELS, XS, YS, PREMULTIPLY><<<grid, kRgbThreads, 0, stream>>>(rp);
     return cudaGetLastError();
-}
-
-template <typename HostT, typename PlaneT>
-cudaError_t LaunchRgbIntChannels(const Rgb16Params& rp, int channels, bool premultiply, int xs, int ys, int smCount, cudaStream_t stream)
-{
-    if (channels == 4 && premultiply) return LaunchRgbInt<HostT, PlaneT, 4, 1>(rp, xs, ys, smCount, stream);
-    return channels == 4 ? LaunchRgbInt<HostT, PlaneT, 4, 0>(rp, xs, ys, smCount, stream) : LaunchRgbInt<HostT, PlaneT, 3, 0>(rp, xs, ys, smCount, stream);
 }
 
 } // namespace
@@ -328,19 +312,9 @@ cudaError_t LaunchRgbIntChannels(const Rgb16Params& rp, int channels, bool premu
 // (0 = verified) or -1 on a CUDA error.  Synchronous.
 long long VerifyFastPremultiply(uint32_t maxCode, void* streamHandle)
 {
-    cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
-    unsigned long long* counter = nullptr;
-    if (cudaMalloc(&counter, sizeof(unsigned long long)) != cudaSuccess)
-    {
-        return -1;
-    }
-    cudaMemsetAsync(counter, 0, sizeof(unsigned long long), stream);
-    VerifyFastPremultiplyKernel<<<132 * 8, 256, 0, stream>>>(maxCode, counter);
-    unsigned long long bad = 0;
-    const bool ok = cudaMemcpyAsync(&bad, counter, sizeof(bad), cudaMemcpyDeviceToHost, stream) == cudaSuccess &&
-                    cudaStreamSynchronize(stream) == cudaSuccess;
-    cudaFree(counter);
-    return ok ? static_cast<long long>(bad) : -1;
+    return CountDisagreements(static_cast<cudaStream_t>(streamHandle), [&](unsigned long long* counter, cudaStream_t stream) {
+        VerifyFastPremultiplyKernel<<<132 * 8, 256, 0, stream>>>(maxCode, counter);
+    });
 }
 
 cudaError_t BuildGray16Lut(uint16_t* deviceLut, int smpte428, uint32_t maxCode, void* streamHandle)
@@ -424,8 +398,6 @@ int LaunchEncodeFastInteger(const EncodeParams& p, int hostDepth, void* streamHa
     const Interior inner = EncodeRgbIntInterior(p, hostDepth);
     if (inner.width > 0)
     {
-        const int hostBytes = hostDepth / 8;
-        const int planeBytes = p.imageDepth > 8 ? 2 : 1;
         const int width8 = inner.width;
         const int evenRows = inner.rows;
         Rgb16Params rp = RgbIntShared(p);
@@ -438,17 +410,9 @@ int LaunchEncodeFastInteger(const EncodeParams& p, int hostDepth, void* streamHa
         }
         rp.groupsPerRow = width8 / 8;
         rp.rowCount = evenRows;
-        cudaError_t e;
-        if (hostBytes == 2)
-        {
-            e = planeBytes == 2 ? LaunchRgbIntChannels<uint16_t, uint16_t>(rp, p.channels, p.premultiply != 0, p.xs, p.ys, smCount, stream)
-                                : LaunchRgbIntChannels<uint16_t, uint8_t>(rp, p.channels, p.premultiply != 0, p.xs, p.ys, smCount, stream);
-        }
-        else
-        {
-            e = planeBytes == 2 ? LaunchRgbIntChannels<uint8_t, uint16_t>(rp, p.channels, p.premultiply != 0, p.xs, p.ys, smCount, stream)
-                                : LaunchRgbIntChannels<uint8_t, uint8_t>(rp, p.channels, p.premultiply != 0, p.xs, p.ys, smCount, stream);
-        }
+        const cudaError_t e = WithRgbIntKey(p, hostDepth, [&](auto host, auto plane, auto channels, auto premultiply, auto xs, auto ys) {
+            return LaunchRgbInt<TypeOf<decltype(host)>, TypeOf<decltype(plane)>, channels(), xs(), ys(), premultiply()>(rp, smCount, stream);
+        });
         return CompleteEncode(e, p, hostDepth, width8, evenRows, streamHandle);
     }
     return 0;

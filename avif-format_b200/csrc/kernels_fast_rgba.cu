@@ -7,6 +7,7 @@
 // each, issued one tile ahead) and only the 24 colour samples of a lane -- after the clamp / premultiplication, the
 // values the curve actually sees -- are parked in shared memory for the band-bitmap probes.  One CTA of 16 warps per SM.
 #include "kernels_fast_common.cuh"
+#include "launch_keys.h"
 #include "table_staging.cuh"
 #include "../../include/avifgpu.h"
 
@@ -244,14 +245,6 @@ cudaError_t LaunchRgbaKernel(const FastEncodeParams& fp, int smCount, cudaStream
     return cudaGetLastError();
 }
 
-template <int CURVE>
-cudaError_t DispatchRgbaChroma(const FastEncodeParams& fp, int xs, int ys, int smCount, cudaStream_t stream)
-{
-    if (xs == 1 && ys == 1) return LaunchRgbaKernel<CURVE, 1, 1>(fp, smCount, stream);
-    if (xs == 1) return LaunchRgbaKernel<CURVE, 1, 0>(fp, smCount, stream);
-    return LaunchRgbaKernel<CURVE, 0, 0>(fp, smCount, stream);
-}
-
 } // namespace
 
 // True when the kernel can stage this table's compact image next to its buffers.
@@ -263,8 +256,10 @@ bool RgbaEncodeApplies(const FastEncodeParams& fp)
 
 cudaError_t LaunchFastEncodeRgba(const FastEncodeParams& fp, int curve, int xs, int ys, int smCount, cudaStream_t stream)
 {
-    if (curve == kCurveLinearToPQ) return DispatchRgbaChroma<kCurveLinearToPQ>(fp, xs, ys, smCount, stream);
-    return DispatchRgbaChroma<kCurveLinearToSMPTE428>(fp, xs, ys, smCount, stream);
+    return WithChroma(xs, ys, [&](auto XS, auto YS) {
+        return curve == kCurveLinearToPQ ? LaunchRgbaKernel<kCurveLinearToPQ, XS(), YS()>(fp, smCount, stream)
+                                         : LaunchRgbaKernel<kCurveLinearToSMPTE428, XS(), YS()>(fp, smCount, stream);
+    });
 }
 
 } // namespace avifgpu

@@ -5,6 +5,7 @@
 // they cannot disagree on arithmetic.
 #include "generic_units.cuh"
 #include "kernel_params.h"
+#include "launch_keys.h"
 #include "curve_lookup.cuh"
 #include "../../include/avifgpu.h"
 
@@ -135,22 +136,12 @@ int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* streamH
         const int sitesX = (p.width + p.xs) >> p.xs;
         const int sitesY = (p.rowCount + p.ys) >> p.ys;
         const unsigned grid = static_cast<unsigned>((sitesX + kThreads - 1) / kThreads) * static_cast<unsigned>(sitesY);
-        switch (hostDepth)
-        {
-        case 8: EncodePlanarKernel<uint8_t><<<grid, kThreads, 0, stream>>>(p); break;
-        case 16: EncodePlanarKernel<uint16_t><<<grid, kThreads, 0, stream>>>(p); break;
-        default: EncodePlanarKernel<float><<<grid, kThreads, 0, stream>>>(p); break;
-        }
+        WithHostDepth(hostDepth, [&](auto, auto host) { EncodePlanarKernel<TypeOf<decltype(host)>><<<grid, kThreads, 0, stream>>>(p); });
     }
     else
     {
         const unsigned grid = static_cast<unsigned>((p.width + kThreads - 1) / kThreads) * static_cast<unsigned>(p.rowCount);
-        switch (hostDepth)
-        {
-        case 8: EncodeReferenceLayoutKernel<uint8_t><<<grid, kThreads, 0, stream>>>(p); break;
-        case 16: EncodeReferenceLayoutKernel<uint16_t><<<grid, kThreads, 0, stream>>>(p); break;
-        default: EncodeReferenceLayoutKernel<float><<<grid, kThreads, 0, stream>>>(p); break;
-        }
+        WithHostDepth(hostDepth, [&](auto, auto host) { EncodeReferenceLayoutKernel<TypeOf<decltype(host)>><<<grid, kThreads, 0, stream>>>(p); });
     }
     const cudaError_t launchError = cudaGetLastError();
     return launchError == cudaSuccess ? 1 : ReportLaunchFailure(static_cast<int>(launchError));
@@ -164,12 +155,7 @@ int LaunchDecodeGeneric(const DecodeParams& p, void* streamHandle)
         return 0;
     }
     const unsigned grid = static_cast<unsigned>((p.width + kThreads - 1) / kThreads) * static_cast<unsigned>(p.rowCount);
-    switch (p.hostDepth)
-    {
-    case 8: DecodeKernel<uint8_t, uint8_t><<<grid, kThreads, 0, stream>>>(p); break;
-    case 16: DecodeKernel<uint16_t, uint16_t><<<grid, kThreads, 0, stream>>>(p); break;
-    default: DecodeKernel<uint16_t, float><<<grid, kThreads, 0, stream>>>(p); break;
-    }
+    WithHostDepth(p.hostDepth, [&](auto plane, auto host) { DecodeKernel<TypeOf<decltype(plane)>, TypeOf<decltype(host)>><<<grid, kThreads, 0, stream>>>(p); });
     const cudaError_t launchError = cudaGetLastError();
     return launchError == cudaSuccess ? 1 : ReportLaunchFailure(static_cast<int>(launchError));
 }

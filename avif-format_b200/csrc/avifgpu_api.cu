@@ -712,6 +712,8 @@ AVIFGPU_EXPORT int avifgpu_encode_host_col_bytes(const avifgpu_encode_desc* desc
 
 AVIFGPU_EXPORT int avifgpu_decode_host_col_bytes(const avifgpu_decode_desc* desc)
 {
+    avifgpu_decode_desc full;
+    desc = WidenDecodeDesc(desc, &full);
     int32_t transfer;
     return ValidateDecodeDesc(desc, &transfer, nullptr) == AVIFGPU_OK ? DecodeHostColBytes(*desc) : AVIFGPU_ERR_BAD_PARAM;
 }
@@ -737,6 +739,8 @@ AVIFGPU_EXPORT int avifgpu_encode_plane_geometry(const avifgpu_encode_desc* desc
 
 AVIFGPU_EXPORT int avifgpu_decode_plane_geometry(const avifgpu_decode_desc* desc, int index, int32_t* w, int32_t* h, int32_t* b)
 {
+    avifgpu_decode_desc full;
+    desc = WidenDecodeDesc(desc, &full);
     int32_t transfer;
     const int status = ValidateDecodeDesc(desc, &transfer, nullptr);
     if (status != AVIFGPU_OK || index < 0 || index >= AVIFGPU_MAX_PLANES)
@@ -857,6 +861,8 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_device(avifgpu_context* ctx, const avifgp
     {
         return AVIFGPU_ERR_BAD_PARAM;
     }
+    avifgpu_decode_desc full;
+    desc = WidenDecodeDesc(desc, &full);
     std::string error;
     int32_t transfer;
     int status = ValidateDecodeDesc(desc, &transfer, &error);
@@ -1007,6 +1013,8 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifg
     {
         return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL description or image array");
     }
+    avifgpu_decode_desc full;
+    desc = WidenDecodeDesc(desc, &full);
     // every image is validated before anything is enqueued: the description at the image's size, then its buffers
     avifgpu_decode_desc d = *desc;
     DecodeParams shared;
@@ -1181,6 +1189,8 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_indirect(avifgpu_context* ctx, const avi
     {
         return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL description");
     }
+    avifgpu_decode_desc full;
+    desc = WidenDecodeDesc(desc, &full);
     avifgpu_decode_desc d = *desc;
     d.width = 0;
     d.height = 0;
@@ -1666,12 +1676,18 @@ static int DecodeRowsHost(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
     {
         return AVIFGPU_ERR_BAD_PARAM;
     }
+    avifgpu_decode_desc full;
+    desc = WidenDecodeDesc(desc, &full);
     std::string error;
     int32_t transfer;
     int status = ValidateDecodeDesc(desc, &transfer, &error);
     if (status != AVIFGPU_OK)
     {
         return ctx->Fail(status, error);
+    }
+    if (SourceLayoutOf(*desc) != AVIFGPU_SOURCE_PLANAR)
+    {
+        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "the host-pointer calls read planar, low-bit sources only (libheif's layout)");
     }
     if (src == nullptr || (host_rows == nullptr && nrows > 0 && desc->width > 0))
     {
@@ -2106,6 +2122,10 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_sharded(avifgpu_shard_group* group, const
     {
         return group->Fail(AVIFGPU_ERR_BAD_PARAM, "row block outside the image");
     }
+    if (desc != nullptr && SourceLayoutOf(*desc) != AVIFGPU_SOURCE_PLANAR)
+    {
+        return group->Fail(AVIFGPU_ERR_UNSUPPORTED, "the sharded calls read planar, low-bit sources only (libheif's layout)");
+    }
     std::vector<int32_t> blockY0(n), blockRows(n);
     RowBlocks(y0, nrows, n, blockY0.data(), blockRows.data());
     return group->ForEachMember([&](int r) -> int
@@ -2206,6 +2226,8 @@ AVIFGPU_EXPORT int avifgpu_prepare_decode(avifgpu_context* ctx, const avifgpu_de
     {
         return AVIFGPU_ERR_BAD_PARAM;
     }
+    avifgpu_decode_desc full;
+    desc = WidenDecodeDesc(desc, &full);
     std::string error;
     int32_t transfer;
     const int status = ValidateDecodeDesc(desc, &transfer, &error);

@@ -328,8 +328,27 @@ __device__ __forceinline__ void DecodeChunkPixel(const DecodeParams& p, const Li
         const int uvI = x >> p.xs;
         const int uvJ = (y + p.yPhase) >> p.ys;
         uint32_t unormY = LoadSample<PlaneT>(p.plane[0], p.planeStride[0], x, y);
-        uint32_t unormU = LoadSample<PlaneT>(p.plane[1], p.planeStride[1], uvI, uvJ);
-        uint32_t unormV = LoadSample<PlaneT>(p.plane[2], p.planeStride[2], uvI, uvJ);
+        uint32_t unormU, unormV;
+        if (SourceInterleaved(p.sourceLayout))
+        {
+            // Cb, Cr pairs in plane 1, Cb first
+            unormU = LoadSample<PlaneT>(p.plane[1], p.planeStride[1], 2 * uvI, uvJ);
+            unormV = LoadSample<PlaneT>(p.plane[1], p.planeStride[1], 2 * uvI + 1, uvJ);
+        }
+        else
+        {
+            unormU = LoadSample<PlaneT>(p.plane[1], p.planeStride[1], uvI, uvJ);
+            unormV = LoadSample<PlaneT>(p.plane[2], p.planeStride[2], uvI, uvJ);
+        }
+        if (SourceMsbAligned(p.sourceLayout))
+        {
+            // the code is the top bitDepth bits of the 16-bit sample
+            const int shift = 16 - p.bitDepth;
+            unormY >>= shift;
+            unormU >>= shift;
+            unormV >>= shift;
+            unormA >>= shift;
+        }
         if (!hostIs8)
         {
             unormY = min(unormY, maxCode);

@@ -217,7 +217,7 @@ int ValidateEncodeDesc(const avifgpu_encode_desc* d, std::string* error)
 int ValidateDecodeDesc(const avifgpu_decode_desc* d, int32_t* outTransfer, std::string* error)
 {
     *outTransfer = AVIFGPU_TRANSFER_CLIP;
-    if (d == nullptr || d->struct_size != sizeof(avifgpu_decode_desc)) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "bad decode desc size");
+    if (d == nullptr || (d->struct_size != sizeof(avifgpu_decode_desc) && d->struct_size != AVIFGPU_DECODE_DESC_V9_SIZE)) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "bad decode desc size");
     if (d->width < 0 || d->height < 0) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "negative image size");
     if (d->host_depth != 8 && d->host_depth != 16 && d->host_depth != 32) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "host depth must be 8, 16 or 32");
     if (d->bit_depth != 8 && d->bit_depth != 10 && d->bit_depth != 12 && d->bit_depth != 16) return Fail(error, AVIFGPU_ERR_UNSUPPORTED, "The image has an unsupported bit depth, must be 8, 10, 12 or 16.");
@@ -231,7 +231,29 @@ int ValidateDecodeDesc(const avifgpu_decode_desc* d, int32_t* outTransfer, std::
         if (!TransferFromNclx(d->nclx.transfer_characteristics, outTransfer)) return Fail(error, AVIFGPU_ERR_UNSUPPORTED, "Unsupported NCLX transfer characteristic.");
         if (d->colorspace == AVIFGPU_COLORSPACE_MONOCHROME && *outTransfer != AVIFGPU_TRANSFER_PQ) return Fail(error, AVIFGPU_ERR_UNSUPPORTED, "Unsupported color transfer function.");
     }
+    const int32_t layout = SourceLayoutOf(*d);
+    if (layout != AVIFGPU_SOURCE_PLANAR)
+    {
+        if (layout & ~(AVIFGPU_SOURCE_CHROMA_INTERLEAVED | AVIFGPU_SOURCE_MSB_ALIGNED)) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "unknown source layout bits");
+        if (d->colorspace != AVIFGPU_COLORSPACE_YCBCR) return Fail(error, AVIFGPU_ERR_UNSUPPORTED, "semi-planar and MSB-aligned sources are YCbCr only");
+        if ((layout & AVIFGPU_SOURCE_MSB_ALIGNED) && d->bit_depth != 10 && d->bit_depth != 12) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "MSB-aligned sources need a 10- or 12-bit image");
+    }
     return AVIFGPU_OK;
+}
+
+int32_t SourceLayoutOf(const avifgpu_decode_desc& d) { return d.struct_size == sizeof(avifgpu_decode_desc) ? d.source_layout : AVIFGPU_SOURCE_PLANAR; }
+
+const avifgpu_decode_desc* WidenDecodeDesc(const avifgpu_decode_desc* d, avifgpu_decode_desc* full)
+{
+    if (d == nullptr || d->struct_size != AVIFGPU_DECODE_DESC_V9_SIZE)
+    {
+        return d;
+    }
+    std::memset(full, 0, sizeof(*full));
+    std::memcpy(full, d, AVIFGPU_DECODE_DESC_V9_SIZE);
+    full->struct_size = sizeof(avifgpu_decode_desc);
+    full->source_layout = AVIFGPU_SOURCE_PLANAR;
+    return full;
 }
 
 static void ChromaShifts(int chroma, int* xs, int* ys)
@@ -301,12 +323,14 @@ PlaneGeometry DecodePlaneGeometry(const avifgpu_decode_desc& d, int index)
     }
     else if ((index == 1 || index == 2) && d.colorspace == AVIFGPU_COLORSPACE_YCBCR)
     {
+        // interleaved chroma: plane 1 holds the Cb, Cr pairs and there is no plane 2
+        const bool interleaved = (SourceLayoutOf(d) & AVIFGPU_SOURCE_CHROMA_INTERLEAVED) != 0;
         int xs, ys;
         ChromaShifts(d.chroma, &xs, &ys);
-        g.present = true;
+        g.present = !(interleaved && index == 2);
         g.xs = xs;
         g.ys = ys;
-        g.widthSamples = (d.width + xs) >> xs;
+        g.widthSamples = ((d.width + xs) >> xs) * (interleaved ? 2 : 1);
         g.height = (d.height + ys) >> ys;
     }
     else if ((index == 1 || index == 2) && d.colorspace == AVIFGPU_COLORSPACE_RGB)
@@ -399,6 +423,7 @@ bool FillDecodeParams(const avifgpu_decode_desc& d, int32_t transfer, DecodePara
     p->premultiplied = d.alpha_state == AVIFGPU_ALPHA_PREMULTIPLIED;
     p->bitDepth = d.bit_depth;
     p->maxCode = (1u << d.bit_depth) - 1u;
+    p->sourceLayout = SourceLayoutOf(d);
     p->range = MakeRangeParams(&d.nclx, d.bit_depth, d.colorspace == AVIFGPU_COLORSPACE_MONOCHROME);
     if (d.colorspace == AVIFGPU_COLORSPACE_RGB)
     {

@@ -29,6 +29,12 @@ avifpix::RangeParams MakeRangeParams(const avifgpu_nclx* nclx, int bitDepth, boo
 int ValidateEncodeDesc(const avifgpu_encode_desc* desc, std::string* error);
 int ValidateDecodeDesc(const avifgpu_decode_desc* desc, int32_t* outTransfer, std::string* error);
 
+// The description's avifgpu_source_layout: AVIFGPU_SOURCE_PLANAR for an API-9-sized one, which has no such field.
+int32_t SourceLayoutOf(const avifgpu_decode_desc& desc);
+// An API-9-sized description copied into `full` with source_layout = AVIFGPU_SOURCE_PLANAR, and `full` returned; any other
+// `desc` is returned as it is.  The entry points widen first, so nothing after them reads past a caller's shorter struct.
+const avifgpu_decode_desc* WidenDecodeDesc(const avifgpu_decode_desc* desc, avifgpu_decode_desc* full);
+
 struct PlaneGeometry
 {
     int32_t widthSamples = 0; // samples per row (interleaved: width * channels)

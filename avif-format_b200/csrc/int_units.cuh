@@ -12,6 +12,7 @@
 #include "kernel_params.h"
 #include "packed_f32x2.cuh"
 #include "pixel_math.cuh"
+#include "source_units.cuh"
 
 #include <cuda_runtime.h>
 
@@ -568,8 +569,46 @@ __device__ __forceinline__ YccFactors MakeYccFactors(const InverseMatrix& matrix
     return f;
 }
 
+// The Cb and Cr samples of a lane's chroma sites from interleaved pairs at `address`, as LoadFour (XS) / LoadEight put the
+// planar ones: one load of twice their bytes -- 64 or 128 bits, two 128-bit loads for 16-bit 4:4:4 -- then a byte
+// permutation per word.
+template <typename SampleT, int XS>
+__device__ __forceinline__ void LoadInterleavedChroma(const uint8_t* address, Raw8<SampleT>& rawCb, Raw8<SampleT>& rawCr)
+{
+    rawCb = {};
+    rawCr = {};
+    if constexpr (sizeof(SampleT) == 1 && XS)
+    {
+        const uint2 v = __ldg(reinterpret_cast<const uint2*>(address));
+        rawCb.w[0] = EvenBytes(v.x, v.y);
+        rawCr.w[0] = OddBytes(v.x, v.y);
+    }
+    else if constexpr (sizeof(SampleT) == 1)
+    {
+        const uint4 v = __ldg(reinterpret_cast<const uint4*>(address));
+        rawCb.w[0] = EvenBytes(v.x, v.y);
+        rawCb.w[1] = EvenBytes(v.z, v.w);
+        rawCr.w[0] = OddBytes(v.x, v.y);
+        rawCr.w[1] = OddBytes(v.z, v.w);
+    }
+    else
+    {
+#pragma unroll
+        for (int q = 0; q < (XS ? 1 : 2); ++q)
+        {
+            const uint4 v = __ldg(reinterpret_cast<const uint4*>(address) + q);
+            rawCb.w[2 * q] = LowHalves(v.x, v.y);
+            rawCb.w[2 * q + 1] = LowHalves(v.z, v.w);
+            rawCr.w[2 * q] = HighHalves(v.x, v.y);
+            rawCr.w[2 * q + 1] = HighHalves(v.z, v.w);
+        }
+    }
+}
+
 // A lane's samples of the unit at (unit row `row`, unit column `column`), as loaded; nothing is loaded for an invalid unit or a lane past the width.
-template <typename SampleT, int XS, int YS, int ALPHA>
+// SOURCE (kernel_params.h): interleaved chroma is read in pairs from plane 1; MSB-aligned samples (16-bit planes) are
+// shifted to their codes two at a time as they arrive, so the rest of the unit sees the planar, low-bit samples.
+template <typename SampleT, int XS, int YS, int ALPHA, int SOURCE = 0>
 __device__ __forceinline__ void LoadYccUnit(const IntDecodeParams& p, int lane, int row, int column, bool valid, Raw8<SampleT> (&rawY)[YS ? 2 : 1],
                                             Raw8<SampleT> (&rawA)[YS ? 2 : 1], Raw8<SampleT>& rawCb, Raw8<SampleT>& rawCr)
 {
@@ -582,7 +621,11 @@ __device__ __forceinline__ void LoadYccUnit(const IntDecodeParams& p, int lane, 
     }
     const int64_t chromaRow = YS ? row : y;
     const int64_t chromaColumn = static_cast<int64_t>(XS ? (x >> 1) : x) * sizeof(SampleT);
-    if (XS)
+    if constexpr (SourceInterleaved(SOURCE))
+    {
+        LoadInterleavedChroma<SampleT, XS>(p.plane[1] + chromaRow * p.planeStride[1] + 2 * chromaColumn, rawCb, rawCr);
+    }
+    else if (XS)
     {
         rawCb = LoadFour<SampleT>(p.plane[1] + chromaRow * p.planeStride[1] + chromaColumn);
         rawCr = LoadFour<SampleT>(p.plane[2] + chromaRow * p.planeStride[2] + chromaColumn);
@@ -602,6 +645,25 @@ __device__ __forceinline__ void LoadYccUnit(const IntDecodeParams& p, int lane, 
             {
                 rawA[r] = LoadEight<SampleT>(p.plane[3] + static_cast<int64_t>(y + r) * p.planeStride[3] + static_cast<int64_t>(x) * sizeof(SampleT));
             }
+        }
+    }
+    if constexpr (SourceMsbAligned(SOURCE) && sizeof(SampleT) == 2)
+    {
+        const uint32_t shift = 16u - static_cast<uint32_t>(p.bitDepth);
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+        {
+#pragma unroll
+            for (int r = 0; r < kRows; ++r)
+            {
+                rawY[r].w[i] = MsbPairToCodes(rawY[r].w[i], shift);
+                if (ALPHA)
+                {
+                    rawA[r].w[i] = MsbPairToCodes(rawA[r].w[i], shift);
+                }
+            }
+            rawCb.w[i] = MsbPairToCodes(rawCb.w[i], shift);
+            rawCr.w[i] = MsbPairToCodes(rawCr.w[i], shift);
         }
     }
 }

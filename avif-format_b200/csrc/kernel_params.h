@@ -144,7 +144,13 @@ struct DecodeParams
     int32_t verifiedHlgDivisions; // 1 once the context has verified HLGToLinearUnit's fast divisions on this device
     int32_t verifiedGreenDivision; // 1 once the context has verified the fast `/ kg` of YuvDecode.cpp:308 for this matrix, depth, range
     int32_t verifiedPqRatio;       // 1 once the context has verified the branch-free division inside PQToLinear on this device
+    int32_t sourceLayout;          // avifgpu_source_layout bits (YCbCr only): Cb, Cr pairs in plane 1; codes in the top bits
 };
+
+// The source layout of a decode, as the tuned kernels take it: a template argument SOURCE whose bits are these, 0 being
+// libheif's planar, low-bit layout.
+AVIFGPU_HD constexpr bool SourceInterleaved(int source) { return (source & AVIFGPU_SOURCE_CHROMA_INTERLEAVED) != 0; }
+AVIFGPU_HD constexpr bool SourceMsbAligned(int source) { return (source & AVIFGPU_SOURCE_MSB_ALIGNED) != 0; }
 
 // The block restricted to its sub-rectangle [x0, x0 + width) x [y0, y0 + rows), for the edge strips the tuned
 // launchers leave to the generic kernel.  Plane k moves by (y0 >> ys_k) rows and (x0 >> xs_k) sites of
@@ -176,7 +182,7 @@ AVIFGPU_HD inline EncodeParams EncodeWindow(const EncodeParams& p, int hostDepth
 
 // The same for a decode block, whose first row may be the second of a 4:2:0 row pair (yPhase = 1): the chroma planes
 // move by the chroma rows between the two first rows, and the window's phase is that of its own first row, so y0 may
-// be odd.
+// be odd.  Interleaved chroma (plane 1 only) moves by two samples per site.
 AVIFGPU_HD inline DecodeParams DecodeWindow(const DecodeParams& p, int x0, int y0, int width, int rows)
 {
     DecodeParams w = p;
@@ -191,8 +197,9 @@ AVIFGPU_HD inline DecodeParams DecodeWindow(const DecodeParams& p, int x0, int y
         }
         const bool chroma = k == 1 || k == 2;
         const int planeRows = chroma ? (p.yPhase + y0) >> p.ys : y0;
+        const int samplesPerSite = (k == 1 && SourceInterleaved(p.sourceLayout)) ? 2 : 1;
         w.plane[k] = static_cast<const uint8_t*>(p.plane[k]) + static_cast<int64_t>(planeRows) * p.planeStride[k] +
-                     static_cast<int64_t>(x0 >> (chroma ? p.xs : 0)) * sampleBytes;
+                     static_cast<int64_t>(x0 >> (chroma ? p.xs : 0)) * samplesPerSite * sampleBytes;
     }
     w.width = width;
     w.rowCount = rows;
@@ -256,6 +263,8 @@ Interior EncodeRgbIntInterior(const EncodeParams& p, int hostDepth); // EncodeRg
 
 // The same for the tuned integer YCbCr decode kernel (DecodeYccToRgbIntKernel): 8/16-bit hosts reading 8-bit / 10-12-bit
 // YCbCr (+ straight alpha), a block starting on a 4:2:0 row pair, aligned buffers, at least 8 x (1 << ys) pixels.
+// Interleaved chroma is one plane of Cb, Cr pairs a lane reads in one load of twice the planar chroma's bytes (two 128-bit
+// loads for 16-bit 4:4:4), so it is aligned to that load, at most 16 bytes.
 bool DecodeYccIntTuned(const DecodeParams& p);
 AVIFGPU_HD inline Interior DecodeYccIntBlockInterior(const DecodeParams& p)
 {
@@ -265,8 +274,10 @@ AVIFGPU_HD inline Interior DecodeYccIntBlockInterior(const DecodeParams& p)
     const int lumaAlign = 8 * sampleBytes;
     const int chromaAlign = (p.xs ? 4 : 8) * sampleBytes;
     const int rowAlign = channels == 4 ? 16 : 8 * sampleBytes; // RGB8: 64-bit stores, everything else 128-bit
-    if (!Aligned(p.plane[0], p.planeStride[0], lumaAlign) || !Aligned(p.plane[1], p.planeStride[1], chromaAlign) ||
-        !Aligned(p.plane[2], p.planeStride[2], chromaAlign) || (p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], lumaAlign)) ||
+    const bool interleaved = SourceInterleaved(p.sourceLayout);
+    const bool chromaAligned = interleaved ? Aligned(p.plane[1], p.planeStride[1], 2 * chromaAlign > 16 ? 16 : 2 * chromaAlign)
+                                           : Aligned(p.plane[1], p.planeStride[1], chromaAlign) && Aligned(p.plane[2], p.planeStride[2], chromaAlign);
+    if (!Aligned(p.plane[0], p.planeStride[0], lumaAlign) || !chromaAligned || (p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], lumaAlign)) ||
         !Aligned(p.rows, p.rowStride, rowAlign))
     {
         return none;
@@ -285,18 +296,22 @@ Interior DecodeYccIntInterior(const DecodeParams& p); // DecodeYccIntTuned ? Dec
 // 10/12-bit YCbCr (+ straight alpha) into 32-bit hosts with the PQ, HLG or SMPTE 428 curve; for HLG the context's verified
 // divisions, and with the OOTF an exponent and luma coefficients the branch-free powf covers; for PQ and SMPTE 428 a matrix
 // whose channel sums are never subnormal.  The block's half: a block starting on a 4:2:0 row pair, aligned buffers, equal
-// Cb and Cr strides, at least 4 x (1 << ys) pixels.  width is a multiple of 4, rows of 1 << ys.
+// Cb and Cr strides, at least 4 x (1 << ys) pixels.  width is a multiple of 4, rows of 1 << ys.  Interleaved chroma is one
+// plane of Cb, Cr pairs read in one load of twice the planar chroma's bytes, aligned to it.
 bool DecodeYccF32Tuned(const DecodeParams& p);
 AVIFGPU_HD inline Interior DecodeYccF32BlockInterior(const DecodeParams& p)
 {
     const Interior none = { 0, 0 };
     const int chromaAlign = p.xs ? 4 : 8;
-    if (p.yPhase != 0 || !Aligned(p.plane[0], p.planeStride[0], 8) || !Aligned(p.plane[1], p.planeStride[1], chromaAlign) ||
-        !Aligned(p.plane[2], p.planeStride[2], chromaAlign) || !Aligned(p.rows, p.rowStride, 16) || (p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], 8)))
+    const bool interleaved = SourceInterleaved(p.sourceLayout);
+    const bool chromaAligned = interleaved ? Aligned(p.plane[1], p.planeStride[1], 2 * chromaAlign)
+                                           : Aligned(p.plane[1], p.planeStride[1], chromaAlign) && Aligned(p.plane[2], p.planeStride[2], chromaAlign);
+    if (p.yPhase != 0 || !Aligned(p.plane[0], p.planeStride[0], 8) || !chromaAligned || !Aligned(p.rows, p.rowStride, 16) ||
+        (p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], 8)))
     {
         return none;
     }
-    if (p.planeStride[1] != p.planeStride[2])
+    if (!interleaved && p.planeStride[1] != p.planeStride[2])
     {
         return none; // the single-image kernel walks Cb and Cr with one offset
     }

@@ -355,7 +355,7 @@ __global__ void __launch_bounds__(kBatchEdgeThreads) EncodePlanarBatchKernel(con
     }
 }
 
-template <typename Source, typename SampleT, int XS, int YS, int ALPHA>
+template <typename Source, typename SampleT, int XS, int YS, int ALPHA, int SOURCE>
 __global__ void __launch_bounds__(kRgbThreads, kYccBlocksPerSm) DecodeYccToRgbIntBatchKernel(const __grid_constant__ Source s)
 {
     const typename Source::Walk walk(s);
@@ -391,7 +391,7 @@ __global__ void __launch_bounds__(kRgbThreads, kYccBlocksPerSm) DecodeYccToRgbIn
         const int unitRow = local / unitsX;
         const int unitX = local - unitRow * unitsX;
         Raw8<SampleT> rawY[kRows] = {}, rawA[kRows] = {}, rawCb = {}, rawCr = {};
-        LoadYccUnit<SampleT, XS, YS, ALPHA>(p, lane, unitRow, unitX, true, rawY, rawA, rawCb, rawCr);
+        LoadYccUnit<SampleT, XS, YS, ALPHA, SOURCE>(p, lane, unitRow, unitX, true, rawY, rawA, rawCb, rawCr);
         YccValues<XS, YS> values;
         ExpandYccUnit<SampleT, XS, YS, ALPHA>(p, tables, factors, rawY, rawA, rawCb, rawCr, values);
         const int x0 = unitX * kUnitPixels + lane * 8;
@@ -405,9 +405,10 @@ __global__ void __launch_bounds__(kRgbThreads, kYccBlocksPerSm) DecodeYccToRgbIn
 
 // The single-image kernel's unit -- 128 pixels of a row, or of a row pair for 4:2:0, a lane on 4 pixels of each row -- with
 // 64-bit addresses from the unit's record instead of the 32-bit walk, and no software pipelining: the next unit may belong
-// to another image.  An interior is 4-pixel aligned, so a lane is wholly inside its row or wholly past its end.
-template <typename Source, int XS, int YS, int TRANSFER, int ALPHA, int FASTDIV>
-__global__ void __launch_bounds__(kF32DecodeThreads, kDecodeBlocksPerSm) DecodeYccToRgbF32BatchKernel(const __grid_constant__ Source s)
+// to another image.  An interior is 4-pixel aligned, so a lane is wholly inside its row or wholly past its end.  SOURCE as
+// for the single-image kernel: the body of DecodeYccToRgbF32BatchKernel (SOURCE 0) and DecodeSourceYccF32BatchKernel.
+template <typename Source, int XS, int YS, int TRANSFER, int ALPHA, int FASTDIV, int SOURCE>
+__device__ __forceinline__ void DecodeYccF32BatchBody(const Source& s)
 {
     const typename Source::Walk walk(s);
     if (walk.Idle(static_cast<long long>(blockIdx.x) * kWarps))
@@ -456,9 +457,13 @@ __global__ void __launch_bounds__(kF32DecodeThreads, kDecodeBlocksPerSm) DecodeY
             }
         }
         // chroma row unitRow (one per row, or per 4:2:0 row pair), sites from x >> XS: 2 (XS) or 4 codes
-        const int64_t chromaAt = static_cast<int64_t>(unitRow) * r.planeStride[1] + (x >> XS) * 2;
+        const int64_t chromaAt = static_cast<int64_t>(unitRow) * r.planeStride[1] + (x >> XS) * (SourceInterleaved(SOURCE) ? 4 : 2);
         uint2 cbWords = make_uint2(0u, 0u), crWords = make_uint2(0u, 0u);
-        if (XS)
+        if constexpr (SourceInterleaved(SOURCE))
+        {
+            LoadInterleavedChromaWords<XS>(static_cast<const uint8_t*>(r.plane[1]) + chromaAt, cbWords, crWords);
+        }
+        else if (XS)
         {
             cbWords.x = __ldg(reinterpret_cast<const uint32_t*>(static_cast<const uint8_t*>(r.plane[1]) + chromaAt));
             crWords.x = __ldg(reinterpret_cast<const uint32_t*>(static_cast<const uint8_t*>(r.plane[2]) + chromaAt));
@@ -468,6 +473,18 @@ __global__ void __launch_bounds__(kF32DecodeThreads, kDecodeBlocksPerSm) DecodeY
             cbWords = __ldg(reinterpret_cast<const uint2*>(static_cast<const uint8_t*>(r.plane[1]) + chromaAt));
             crWords = __ldg(reinterpret_cast<const uint2*>(static_cast<const uint8_t*>(r.plane[2]) + chromaAt));
         }
+        if constexpr (SourceMsbAligned(SOURCE))
+        {
+            const uint32_t shift = 16u - static_cast<uint32_t>(s.shared.bitDepth);
+#pragma unroll
+            for (int k = 0; k < kRows; ++k)
+            {
+                yWords[k] = MsbWordsToCodes(yWords[k], shift);
+                aWords[k] = ALPHA ? MsbWordsToCodes(aWords[k], shift) : aWords[k];
+            }
+            cbWords = MsbWordsToCodes(cbWords, shift);
+            crWords = MsbWordsToCodes(crWords, shift);
+        }
         float Yf[kRows][4];
         uint2 aPairs[kRows];
         LookUpLuma<kRows>(yWords, aWords, maxCodePair, tables.sharedY, Yf, aPairs);
@@ -476,6 +493,18 @@ __global__ void __launch_bounds__(kF32DecodeThreads, kDecodeBlocksPerSm) DecodeY
         uint8_t* target = static_cast<uint8_t*>(const_cast<void*>(r.rows)) + y * r.rowStride + static_cast<int64_t>(x) * kOutChannels * 4;
         ConvertRows<XS, YS, TRANSFER, ALPHA, FASTDIV>(s.shared, Yf, aPairs, rOffset, bOffset, gOffset, target, r.rowStride, tables.sharedA, tables.t);
     }
+}
+
+template <typename Source, int XS, int YS, int TRANSFER, int ALPHA, int FASTDIV>
+__global__ void __launch_bounds__(kF32DecodeThreads, kDecodeBlocksPerSm) DecodeYccToRgbF32BatchKernel(const __grid_constant__ Source s)
+{
+    DecodeYccF32BatchBody<Source, XS, YS, TRANSFER, ALPHA, FASTDIV, AVIFGPU_SOURCE_PLANAR>(s);
+}
+
+template <typename Source, int XS, int YS, int TRANSFER, int ALPHA, int FASTDIV, int SOURCE>
+__global__ void __launch_bounds__(kF32DecodeThreads, kDecodeBlocksPerSm) DecodeSourceYccF32BatchKernel(const __grid_constant__ Source s)
+{
+    DecodeYccF32BatchBody<Source, XS, YS, TRANSFER, ALPHA, FASTDIV, SOURCE>(s);
 }
 
 // The pixel `column` (a multiple of 8) and row of a warp's lane in planar-RGB unit `unit` of record `r`: 256 pixels of one row.
@@ -617,18 +646,28 @@ void LaunchPlanar(const Source& s, int hostDepth, unsigned grid, cudaStream_t st
 template <typename Source>
 void LaunchYccInt(const Source& s, const DecodeParams& d, unsigned grid, size_t bytes, cudaStream_t stream)
 {
-    WithYccIntKey(d, [&](auto sample, auto alpha, auto xs, auto ys) {
-        DecodeYccToRgbIntBatchKernel<Source, TypeOf<decltype(sample)>, xs(), ys(), alpha()><<<grid, kRgbThreads, bytes, stream>>>(s);
+    WithYccIntKey(d, [&](auto sample, auto alpha, auto xs, auto ys, auto source) {
+        DecodeYccToRgbIntBatchKernel<Source, TypeOf<decltype(sample)>, xs(), ys(), alpha(), source()><<<grid, kRgbThreads, bytes, stream>>>(s);
     });
 }
 
-template <typename Source, int XS, int YS, int TRANSFER, int ALPHA, int FASTDIV>
+template <typename Source, int XS, int YS, int TRANSFER, int ALPHA, int FASTDIV, int SOURCE>
 void LaunchYccF32One(const Source& s, unsigned grid, size_t bytes, cudaStream_t stream)
 {
     static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
-    if (AllowDynamicShared(DecodeYccToRgbF32BatchKernel<Source, XS, YS, TRANSFER, ALPHA, FASTDIV>, kF32MaxTableBytes, configuredDevices) == cudaSuccess)
+    const auto kernel = [] {
+        if constexpr (SOURCE == AVIFGPU_SOURCE_PLANAR)
+        {
+            return DecodeYccToRgbF32BatchKernel<Source, XS, YS, TRANSFER, ALPHA, FASTDIV>;
+        }
+        else
+        {
+            return DecodeSourceYccF32BatchKernel<Source, XS, YS, TRANSFER, ALPHA, FASTDIV, SOURCE>;
+        }
+    }();
+    if (AllowDynamicShared(kernel, kF32MaxTableBytes, configuredDevices) == cudaSuccess)
     {
-        DecodeYccToRgbF32BatchKernel<Source, XS, YS, TRANSFER, ALPHA, FASTDIV><<<grid, kF32DecodeThreads, bytes, stream>>>(s);
+        kernel<<<grid, kF32DecodeThreads, bytes, stream>>>(s);
     } // else the failed attribute call is the error Launched() finds
 }
 
@@ -636,8 +675,8 @@ void LaunchYccF32One(const Source& s, unsigned grid, size_t bytes, cudaStream_t 
 template <typename Source>
 void LaunchYccF32(const Source& s, const DecodeParams& d, unsigned grid, size_t bytes, cudaStream_t stream)
 {
-    WithYccF32Key(d, [&](auto transfer, auto fastDiv, auto alpha, auto xs, auto ys) {
-        LaunchYccF32One<Source, xs(), ys(), transfer(), alpha(), fastDiv()>(s, grid, bytes, stream);
+    WithYccF32Key(d, [&](auto transfer, auto fastDiv, auto alpha, auto xs, auto ys, auto source) {
+        LaunchYccF32One<Source, xs(), ys(), transfer(), alpha(), fastDiv(), source()>(s, grid, bytes, stream);
     });
 }
 

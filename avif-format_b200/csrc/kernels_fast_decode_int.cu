@@ -33,7 +33,8 @@ namespace
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 
-template <typename SampleT, int XS, int YS, int ALPHA>
+// SOURCE: the avifgpu_source_layout bits the kernel reads (LoadYccUnit); 0 is libheif's planar, low-bit layout.
+template <typename SampleT, int XS, int YS, int ALPHA, int SOURCE>
 __global__ void __launch_bounds__(kThreads, kYccBlocksPerSm) DecodeYccToRgbIntKernel(const IntDecodeParams p)
 {
     constexpr int kRows = YS ? 2 : 1;
@@ -66,7 +67,7 @@ __global__ void __launch_bounds__(kThreads, kYccBlocksPerSm) DecodeYccToRgbIntKe
     }
     rawCb = {};
     rawCr = {};
-    LoadYccUnit<SampleT, XS, YS, ALPHA>(p, lane, unitRow, unitX, firstUnit < unitCount, rawY, rawA, rawCb, rawCr);
+    LoadYccUnit<SampleT, XS, YS, ALPHA, SOURCE>(p, lane, unitRow, unitX, firstUnit < unitCount, rawY, rawA, rawCb, rawCr);
 
 #pragma unroll 1
     for (long long unit = firstUnit; unit < unitCount; unit += warpCount)
@@ -86,7 +87,7 @@ __global__ void __launch_bounds__(kThreads, kYccBlocksPerSm) DecodeYccToRgbIntKe
         YccValues<XS, YS> values;
         ExpandYccUnit<SampleT, XS, YS, ALPHA>(p, tables, factors, rawY, rawA, rawCb, rawCr, values);
 
-        LoadYccUnit<SampleT, XS, YS, ALPHA>(p, lane, nextRow, nextX, unit + warpCount < unitCount, rawY, rawA, rawCb, rawCr);
+        LoadYccUnit<SampleT, XS, YS, ALPHA, SOURCE>(p, lane, nextRow, nextX, unit + warpCount < unitCount, rawY, rawA, rawCb, rawCr);
         unitRow = nextRow;
         unitX = nextX;
         if (!laneActive)
@@ -97,13 +98,13 @@ __global__ void __launch_bounds__(kThreads, kYccBlocksPerSm) DecodeYccToRgbIntKe
     }
 }
 
-template <typename SampleT, int XS, int YS, int ALPHA>
+template <typename SampleT, int XS, int YS, int ALPHA, int SOURCE>
 cudaError_t LaunchOne(const IntDecodeParams& fp, int smCount, cudaStream_t stream)
 {
     const size_t shared = YccTableBytes(fp.bitDepth, ALPHA && sizeof(SampleT) == 2);
     static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
     {
-        const cudaError_t e = AllowDynamicShared(DecodeYccToRgbIntKernel<SampleT, XS, YS, ALPHA>, 64 * 1024, configuredDevices);
+        const cudaError_t e = AllowDynamicShared(DecodeYccToRgbIntKernel<SampleT, XS, YS, ALPHA, SOURCE>, 64 * 1024, configuredDevices);
         if (e != cudaSuccess)
         {
             return e;
@@ -112,7 +113,7 @@ cudaError_t LaunchOne(const IntDecodeParams& fp, int smCount, cudaStream_t strea
     constexpr int rowsPerUnit = YS ? 2 : 1;
     const long long units = static_cast<long long>((fp.width + kUnitPixels - 1) / kUnitPixels) * ((fp.rowCount + rowsPerUnit - 1) / rowsPerUnit);
     const unsigned grid = GridFor((units + kWarps - 1) / kWarps, static_cast<long long>(smCount) * kYccBlocksPerSm);
-    DecodeYccToRgbIntKernel<SampleT, XS, YS, ALPHA><<<grid, kThreads, shared, stream>>>(fp);
+    DecodeYccToRgbIntKernel<SampleT, XS, YS, ALPHA, SOURCE><<<grid, kThreads, shared, stream>>>(fp);
     return cudaGetLastError();
 }
 
@@ -336,8 +337,8 @@ int LaunchDecodeFastInteger(const DecodeParams& p, void* streamHandle)
     fp.rowCount = evenRows;
 
     const int smCount = SmCountOrDefault(p.smCount);
-    const cudaError_t e = WithYccIntKey(p, [&](auto sample, auto alpha, auto xs, auto ys) {
-        return LaunchOne<TypeOf<decltype(sample)>, xs(), ys(), alpha()>(fp, smCount, stream);
+    const cudaError_t e = WithYccIntKey(p, [&](auto sample, auto alpha, auto xs, auto ys, auto source) {
+        return LaunchOne<TypeOf<decltype(sample)>, xs(), ys(), alpha(), source()>(fp, smCount, stream);
     });
     return CompleteDecode(e, p, width8, evenRows, streamHandle);
 }

@@ -41,6 +41,17 @@ auto WithChroma(int xs, int ys, F&& f)
     return f(Int<0>{}, Int<0>{});
 }
 
+// f(SOURCE): the avifgpu_source_layout bits of a YCbCr decode -- interleaved chroma (1), MSB-aligned samples (2), both (3)
+// or libheif's planar, low-bit layout (0).
+template <typename F>
+auto WithSource(int layout, F&& f)
+{
+    if (SourceInterleaved(layout) && SourceMsbAligned(layout)) return f(Int<AVIFGPU_SOURCE_CHROMA_INTERLEAVED | AVIFGPU_SOURCE_MSB_ALIGNED>{});
+    if (SourceMsbAligned(layout)) return f(Int<AVIFGPU_SOURCE_MSB_ALIGNED>{});
+    if (SourceInterleaved(layout)) return f(Int<AVIFGPU_SOURCE_CHROMA_INTERLEAVED>{});
+    return f(Int<AVIFGPU_SOURCE_PLANAR>{});
+}
+
 // f(HostT): the sample type of an integer host -- uint16_t for 16 bits, uint8_t for anything else.
 template <typename F>
 auto WithIntHost(int hostDepth, F&& f)
@@ -87,22 +98,37 @@ auto WithIntDecodeKey(const DecodeParams& d, F&& f)
     return d.hostDepth == 8 ? withSample(Type<uint8_t>{}) : withSample(Type<uint16_t>{});
 }
 
-// Integer YCbCr decode (DecodeYccToRgbIntKernel, DecodeYccToRgbIntBatchKernel).  f(SampleT, ALPHA, XS, YS).
+// Integer YCbCr decode (DecodeYccToRgbIntKernel, DecodeYccToRgbIntBatchKernel).  f(SampleT, ALPHA, XS, YS, SOURCE): 8-bit
+// samples (8-bit hosts) are never MSB-aligned (ValidateDecodeDesc), so they take SOURCE 0 or 1 only.
 template <typename F>
 auto WithYccIntKey(const DecodeParams& d, F&& f)
 {
-    return WithIntDecodeKey(d, [&](auto sample, auto alpha) { return WithChroma(d.xs, d.ys, [&](auto xs, auto ys) { return f(sample, alpha, xs, ys); }); });
+    return WithIntDecodeKey(d, [&](auto sample, auto alpha) {
+        return WithChroma(d.xs, d.ys, [&](auto xs, auto ys) {
+            const auto withSource = [&](auto source) { return f(sample, alpha, xs, ys, source); };
+            if constexpr (sizeof(TypeOf<decltype(sample)>) == 1)
+            {
+                return WithFlag(SourceInterleaved(d.sourceLayout), withSource);
+            }
+            else
+            {
+                return WithSource(d.sourceLayout, withSource);
+            }
+        });
+    });
 }
 
-// Float YCbCr decode (DecodeYccToRgbF32Kernel, DecodeYccToRgbF32BatchKernel).  f(TRANSFER, FASTDIV, ALPHA, XS, YS): PQ with
-// (FASTDIV = 1) or without the context's verified division, HLG, and SMPTE 428 for anything else -- DecodeYccF32Tuned
-// leaves these three.
+// Float YCbCr decode (DecodeYccToRgbF32Kernel, DecodeYccToRgbF32BatchKernel).  f(TRANSFER, FASTDIV, ALPHA, XS, YS, SOURCE):
+// PQ with (FASTDIV = 1) or without the context's verified division, HLG, and SMPTE 428 for anything else --
+// DecodeYccF32Tuned leaves these three.
 template <typename F>
 auto WithYccF32Key(const DecodeParams& d, F&& f)
 {
     const auto withTransfer = [&](auto transfer, auto fastDiv) {
         return WithFlag(d.hasAlpha != 0, [&](auto alpha) {
-            return WithChroma(d.xs, d.ys, [&](auto xs, auto ys) { return f(transfer, fastDiv, alpha, xs, ys); });
+            return WithChroma(d.xs, d.ys, [&](auto xs, auto ys) {
+                return WithSource(d.sourceLayout, [&](auto source) { return f(transfer, fastDiv, alpha, xs, ys, source); });
+            });
         });
     };
     if (d.transfer == AVIFGPU_TRANSFER_PQ && d.verifiedPqRatio) return withTransfer(Int<AVIFGPU_TRANSFER_PQ>{}, Int<1>{});

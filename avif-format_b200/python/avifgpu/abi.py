@@ -8,7 +8,7 @@ import ctypes as C
 
 import numpy as np
 
-API_VERSION = 9
+API_VERSION = 10
 
 # avifgpu_status
 OK = 0
@@ -30,6 +30,8 @@ CHROMA_MONOCHROME, CHROMA_420, CHROMA_422, CHROMA_444 = 0, 1, 2, 3
 COLORSPACE_YCBCR, COLORSPACE_RGB, COLORSPACE_MONOCHROME = 0, 1, 2
 # avifgpu_layout
 LAYOUT_REFERENCE, LAYOUT_PLANAR_YCBCR = 0, 1
+# avifgpu_source_layout (bits of DecodeDesc.source_layout)
+SOURCE_PLANAR, SOURCE_CHROMA_INTERLEAVED, SOURCE_MSB_ALIGNED = 0, 1, 2
 # avifgpu_down_filter
 DOWN_FILTER_BOX, DOWN_FILTER_TOP_LEFT = 0, 1
 # avifgpu_gray16_curve
@@ -145,11 +147,12 @@ class DecodeDesc(C.Structure):
         ("hlg_display_gamma", C.c_float),
         ("hlg_peak_nits", C.c_int32),
         ("pq_peak_nits", C.c_int32),
+        ("source_layout", C.c_int32),
     ]
 
     def __init__(self, width, height, colorspace=COLORSPACE_YCBCR, chroma=CHROMA_444, bit_depth=8,
                  alpha_state=ALPHA_NONE, host_depth=8, nclx=None, hlg_apply_ootf=1, hlg_display_gamma=1.2,
-                 hlg_peak_nits=1000, pq_peak_nits=80):
+                 hlg_peak_nits=1000, pq_peak_nits=80, source_layout=SOURCE_PLANAR):
         super().__init__()
         self.struct_size = C.sizeof(DecodeDesc)
         self.width, self.height = width, height
@@ -162,6 +165,7 @@ class DecodeDesc(C.Structure):
         self.hlg_display_gamma = hlg_display_gamma
         self.hlg_peak_nits = hlg_peak_nits
         self.pq_peak_nits = pq_peak_nits
+        self.source_layout = source_layout
 
     def copy(self, **changes):
         out = DecodeDesc(self.width, self.height)
@@ -234,8 +238,11 @@ def decode_plane_shapes(desc):
     if desc.colorspace == COLORSPACE_YCBCR:
         xs, ys = chroma_shifts(desc.chroma)
         cw, ch = (w + xs) >> xs, (h + ys) >> ys
-        shapes[1] = (ch, cw)
-        shapes[2] = (ch, cw)
+        if desc.source_layout & SOURCE_CHROMA_INTERLEAVED:
+            shapes[1] = (ch, 2 * cw)  # Cb, Cr pairs; no plane 2
+        else:
+            shapes[1] = (ch, cw)
+            shapes[2] = (ch, cw)
     elif desc.colorspace == COLORSPACE_RGB:
         shapes[1] = (h, w)
         shapes[2] = (h, w)

@@ -50,7 +50,7 @@ extern "C" {
 #define AVIFGPU_EXPORT __attribute__((visibility("default")))
 #endif
 
-#define AVIFGPU_API_VERSION 9
+#define AVIFGPU_API_VERSION 10
 
 typedef enum avifgpu_status
 {
@@ -136,7 +136,8 @@ typedef struct avifgpu_nclx
 #define AVIFGPU_MAX_PLANES 4
 
 /* A set of image planes.  stride in BYTES (libheif pads rows: heif_image_get_plane's out_stride).
- * Samples deeper than 8 bit are native-endian uint16 with the value in the low bits. */
+ * Samples deeper than 8 bit are native-endian uint16 with the value in the low bits, unless a decode description's
+ * source_layout says otherwise. */
 typedef struct avifgpu_planes
 {
     void* data[AVIFGPU_MAX_PLANES];
@@ -186,6 +187,26 @@ typedef struct avifgpu_encode_desc
 
 /* Parameter block of the decode direction = heif_image properties + nclx + LoadUIOptions
  * (AvifFormat.h:61-85). */
+/* How a YCbCr decode source sits in memory (avifgpu_decode_desc.source_layout), a bit set.  Hardware video decoders
+ * (NVDEC through the Video Codec SDK or nvImageCodec, D3D12 and Vulkan video) write their frames this way:
+ *   surface format         bit_depth  source_layout
+ *   NV12 (4:2:0), NV16     8          AVIFGPU_SOURCE_CHROMA_INTERLEAVED
+ *   P010 / P016 (4:2:0)    10 or 12   AVIFGPU_SOURCE_CHROMA_INTERLEAVED | AVIFGPU_SOURCE_MSB_ALIGNED
+ *   YUV444 (8-bit planar)  8          AVIFGPU_SOURCE_PLANAR
+ *   YUV444_16Bit           10 or 12   AVIFGPU_SOURCE_MSB_ALIGNED
+ * Every output is, bit for bit, that of the same decode of the equivalent planar, low-bit source. */
+typedef enum avifgpu_source_layout
+{
+    /* libheif's (and dav1d's) layout: planes Y, Cb, Cr, Alpha; deeper codes in the low bits of a uint16.  The default. */
+    AVIFGPU_SOURCE_PLANAR = 0,
+    /* Cb and Cr interleaved in plane 1, Cb first (NV12 / NV16 / P010 / P016 / P210 order): a chroma row holds
+     * 2 * ((width + xs) >> xs) samples.  planes.data[2] is ignored; alpha stays plane 3. */
+    AVIFGPU_SOURCE_CHROMA_INTERLEAVED = 1,
+    /* Every sample of every plane is a uint16 whose top bit_depth bits hold the code, code = sample >> (16 - bit_depth);
+     * the low bits are ignored, whatever they hold.  bit_depth 10 or 12 only. */
+    AVIFGPU_SOURCE_MSB_ALIGNED = 2
+} avifgpu_source_layout;
+
 typedef struct avifgpu_decode_desc
 {
     uint32_t struct_size;   /* sizeof(avifgpu_decode_desc) */
@@ -201,7 +222,17 @@ typedef struct avifgpu_decode_desc
     float hlg_display_gamma;     /* LoadUIOptions.hlg.displayGamma */
     int32_t hlg_peak_nits;       /* LoadUIOptions.hlg.nominalPeakBrightness */
     int32_t pq_peak_nits;        /* LoadUIOptions.pq.nominalPeakBrightness */
+    /* Since API version 10: avifgpu_source_layout bits.  Non-zero only for AVIFGPU_COLORSPACE_YCBCR
+     * (AVIFGPU_ERR_UNSUPPORTED otherwise); AVIFGPU_SOURCE_MSB_ALIGNED needs bit_depth 10 or 12 and unknown bits are
+     * AVIFGPU_ERR_BAD_PARAM.  Only the device-pointer calls read such sources (avifgpu_decode_rows_device,
+     * avifgpu_decode_batch_device, avifgpu_decode_batch_indirect); the host-pointer, asynchronous and sharded calls refuse
+     * a non-zero layout with AVIFGPU_ERR_UNSUPPORTED and launch nothing.  A struct_size of AVIFGPU_DECODE_DESC_V9_SIZE
+     * (a caller built against API version 9, which has no such field) is accepted and means AVIFGPU_SOURCE_PLANAR. */
+    int32_t source_layout;
 } avifgpu_decode_desc;
+
+/* sizeof(avifgpu_decode_desc) up to API version 9: everything before source_layout. */
+#define AVIFGPU_DECODE_DESC_V9_SIZE ((uint32_t)offsetof(avifgpu_decode_desc, source_layout))
 
 typedef struct avifgpu_context avifgpu_context;
 
@@ -312,7 +343,9 @@ AVIFGPU_EXPORT int avifgpu_wait(avifgpu_context* ctx, int64_t ticket);
 /* ---- the hot path: device-pointer variants (no copies, no synchronisation) --------------------------- */
 
 /* Same contracts, but host_rows / planes are DEVICE pointers valid on the context's device and the work is
- * enqueued on `cuda_stream` (a cudaStream_t; NULL = the legacy default stream).
+ * enqueued on `cuda_stream` (a cudaStream_t; NULL = the legacy default stream).  The decode call also reads the
+ * semi-planar and MSB-aligned sources of avifgpu_decode_desc.source_layout, with any row block (an odd y0 of a 4:2:0
+ * image included).
  *
  * CUDA graph capture.  Both calls may be recorded into a CUDA graph (cudaStreamBeginCapture ... cudaStreamEndCapture,
  * or torch.cuda.graph), in any capture mode, global included.  While `cuda_stream` is capturing a call:
@@ -382,8 +415,10 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
  * straight or no alpha, aligned buffers, equal Cb / Cr strides, width >= 4; HLG once its divisions are verified); and,
  * since API version 9, the planar-RGB ones (lossless images: 8-bit planes into 8-bit hosts and 10/12-bit planes into
  * 16-bit hosts, or 10/12-bit planes with PQ, HLG or SMPTE 428 into 32-bit hosts; straight or no alpha, aligned buffers,
- * width >= 8).  Every other image -- monochrome, premultiplied alpha, 16-bit planes, a misaligned buffer -- takes one
- * direct call, after the chunks.  The first-use work (the verified divisions) is done once per call, outside a capture. */
+ * width >= 8).  Since API version 10 the YCbCr routes also take the semi-planar and MSB-aligned sources of
+ * avifgpu_decode_desc.source_layout, an interleaved chroma plane aligned to the pair loads (twice the planar chroma's
+ * alignment, at most 16 bytes).  Every other image -- monochrome, premultiplied alpha, 16-bit planes, a misaligned buffer --
+ * takes one direct call, after the chunks.  The first-use work (the verified divisions) is done once per call, outside a capture. */
 AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
                                                const avifgpu_batch_image* images, int32_t count, void* cuda_stream);
 

@@ -707,6 +707,8 @@ AVIFGPU_EXPORT int avifgpu_host_free(avifgpu_context* ctx, void* ptr)
 
 AVIFGPU_EXPORT int avifgpu_encode_host_col_bytes(const avifgpu_encode_desc* desc)
 {
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
     return ValidateEncodeDesc(desc, nullptr) == AVIFGPU_OK ? EncodeHostColBytes(*desc) : AVIFGPU_ERR_BAD_PARAM;
 }
 
@@ -728,6 +730,8 @@ static int ReportGeometry(const PlaneGeometry& g, int32_t* w, int32_t* h, int32_
 
 AVIFGPU_EXPORT int avifgpu_encode_plane_geometry(const avifgpu_encode_desc* desc, int index, int32_t* w, int32_t* h, int32_t* b)
 {
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
     const int status = ValidateEncodeDesc(desc, nullptr);
     if (status != AVIFGPU_OK || index < 0 || index >= AVIFGPU_MAX_PLANES)
     {
@@ -798,6 +802,8 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_device(avifgpu_context* ctx, const avifgp
     {
         return AVIFGPU_ERR_BAD_PARAM;
     }
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
     std::string error;
     int status = ValidateEncodeDesc(desc, &error);
     if (status != AVIFGPU_OK)
@@ -933,6 +939,8 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
     {
         return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL description or image array");
     }
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
     // every image is validated before anything is enqueued: the description at the image's size, then its buffers
     avifgpu_encode_desc d = *desc;
     EncodeParams shared;
@@ -1135,6 +1143,8 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_indirect(avifgpu_context* ctx, const avi
     {
         return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL description");
     }
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
     avifgpu_encode_desc d = *desc; // the images carry the sizes
     d.width = 0;
     d.height = 0;
@@ -1508,11 +1518,17 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
     {
         return AVIFGPU_ERR_BAD_PARAM;
     }
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
     std::string error;
     int status = ValidateEncodeDesc(desc, &error);
     if (status != AVIFGPU_OK)
     {
         return ctx->Fail(status, error);
+    }
+    if (DestLayoutOf(*desc) != AVIFGPU_SOURCE_PLANAR)
+    {
+        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "the host-pointer calls write planar, low-bit planes only (libheif's layout)");
     }
     if (dst == nullptr || (host_rows == nullptr && nrows > 0 && desc->width > 0))
     {
@@ -2064,6 +2080,8 @@ AVIFGPU_EXPORT int avifgpu_shard_group_prepare_encode(avifgpu_shard_group* group
     {
         return AVIFGPU_ERR_BAD_PARAM;
     }
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
     return group->ForEachMember([&](int r) { return avifgpu_prepare_encode(group->members[r], desc, nullptr); });
 }
 
@@ -2096,6 +2114,12 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_sharded(avifgpu_shard_group* group, const
     if (nrows < 0 || y0 < 0)
     {
         return group->Fail(AVIFGPU_ERR_BAD_PARAM, "row block outside the image");
+    }
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
+    if (desc != nullptr && DestLayoutOf(*desc) != AVIFGPU_SOURCE_PLANAR)
+    {
+        return group->Fail(AVIFGPU_ERR_UNSUPPORTED, "the sharded calls write planar, low-bit planes only (libheif's layout)");
     }
     std::vector<int32_t> blockY0(n), blockRows(n);
     RowBlocks(y0, nrows, n, blockY0.data(), blockRows.data());
@@ -2152,6 +2176,12 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_device(avifgpu_shard_group* group
     {
         return group->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL argument or owner outside the group");
     }
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
+    if (DestLayoutOf(*desc) != AVIFGPU_SOURCE_PLANAR)
+    {
+        return group->Fail(AVIFGPU_ERR_UNSUPPORTED, "the sharded calls write planar, low-bit planes only (libheif's layout)");
+    }
     std::vector<int32_t> blockY0(n), blockRows(n);
     RowBlocks(0, desc->height, n, blockY0.data(), blockRows.data());
     for (int r = 0; r < n; ++r)
@@ -2187,6 +2217,8 @@ AVIFGPU_EXPORT int avifgpu_prepare_encode(avifgpu_context* ctx, const avifgpu_en
     {
         return AVIFGPU_ERR_BAD_PARAM;
     }
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
     std::string error;
     const int status = ValidateEncodeDesc(desc, &error);
     if (status != AVIFGPU_OK)

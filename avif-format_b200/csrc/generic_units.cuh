@@ -197,6 +197,8 @@ __device__ __forceinline__ void EncodePlanarSite(const EncodeParams& p, const Li
     }
     const bool wide = p.imageDepth > 8;
     const int maxCode = static_cast<int>(p.maxCode);
+    // MSB-aligned planes hold every code, alpha included, in the top bits of its uint16 (ValidateEncodeDesc: 10/12 bits)
+    const int shift = SourceMsbAligned(p.destLayout) ? 16 - p.imageDepth : 0;
     float cb[2][2];
     float cr[2][2];
     bool have[2][2] = { { false, false }, { false, false } };
@@ -222,10 +224,10 @@ __device__ __forceinline__ void EncodePlanarSite(const EncodeParams& p, const Li
             float yf;
             ForwardPixel(p.matrix, codes[0], codes[1], codes[2], yf, cb[dy][dx], cr[dy][dx]);
             have[dy][dx] = true;
-            StoreCode(p.plane[0], p.planeStride[0], y, x, wide, QuantiseLuma(yf, maxCode));
+            StoreCode(p.plane[0], p.planeStride[0], y, x, wide, static_cast<uint32_t>(QuantiseLuma(yf, maxCode)) << shift);
             if (p.hasAlpha)
             {
-                StoreCode(p.plane[3], p.planeStride[3], y, x, wide, codes[3]);
+                StoreCode(p.plane[3], p.planeStride[3], y, x, wide, codes[3] << shift);
             }
         }
     }
@@ -256,8 +258,19 @@ __device__ __forceinline__ void EncodePlanarSite(const EncodeParams& p, const Li
         cbv = cb[0][0];
         crv = cr[0][0];
     }
-    StoreCode(p.plane[1], p.planeStride[1], cy, cx, wide, QuantiseChroma(cbv, p.chromaOffset, maxCode));
-    StoreCode(p.plane[2], p.planeStride[2], cy, cx, wide, QuantiseChroma(crv, p.chromaOffset, maxCode));
+    const uint32_t cbCode = static_cast<uint32_t>(QuantiseChroma(cbv, p.chromaOffset, maxCode)) << shift;
+    const uint32_t crCode = static_cast<uint32_t>(QuantiseChroma(crv, p.chromaOffset, maxCode)) << shift;
+    if (SourceInterleaved(p.destLayout))
+    {
+        // Cb, Cr pairs in plane 1, Cb first; plane 2 is not written
+        StoreCode(p.plane[1], p.planeStride[1], cy, 2 * cx, wide, cbCode);
+        StoreCode(p.plane[1], p.planeStride[1], cy, 2 * cx + 1, wide, crCode);
+    }
+    else
+    {
+        StoreCode(p.plane[1], p.planeStride[1], cy, cx, wide, cbCode);
+        StoreCode(p.plane[2], p.planeStride[2], cy, cx, wide, crCode);
+    }
 }
 
 // ---- decode -------------------------------------------------------------------------------------------------

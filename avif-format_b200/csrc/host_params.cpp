@@ -165,7 +165,7 @@ avifpix::RangeParams MakeRangeParams(const avifgpu_nclx* nclx, int bitDepth, boo
 
 int ValidateEncodeDesc(const avifgpu_encode_desc* d, std::string* error)
 {
-    if (d == nullptr || d->struct_size != sizeof(avifgpu_encode_desc)) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "bad encode desc size");
+    if (d == nullptr || (d->struct_size != sizeof(avifgpu_encode_desc) && d->struct_size != AVIFGPU_ENCODE_DESC_V10_SIZE)) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "bad encode desc size");
     if (d->width < 0 || d->height < 0) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "negative image size");
     if (d->host_depth != 8 && d->host_depth != 16 && d->host_depth != 32) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "host depth must be 8, 16 or 32");
     if (d->host_channels < 1 || d->host_channels > 4) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "host channels must be 1..4");
@@ -211,7 +211,29 @@ int ValidateEncodeDesc(const avifgpu_encode_desc* d, std::string* error)
     {
         return Fail(error, AVIFGPU_ERR_BAD_PARAM, "bad layout");
     }
+    const int32_t dest = DestLayoutOf(*d);
+    if (dest != AVIFGPU_SOURCE_PLANAR)
+    {
+        if (dest & ~(AVIFGPU_SOURCE_CHROMA_INTERLEAVED | AVIFGPU_SOURCE_MSB_ALIGNED)) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "unknown destination layout bits");
+        if (d->layout != AVIFGPU_LAYOUT_PLANAR_YCBCR) return Fail(error, AVIFGPU_ERR_UNSUPPORTED, "semi-planar and MSB-aligned destinations are planar YCbCr only");
+        if ((dest & AVIFGPU_SOURCE_MSB_ALIGNED) && d->image_bit_depth == 8) return Fail(error, AVIFGPU_ERR_BAD_PARAM, "MSB-aligned destinations need a 10- or 12-bit image");
+    }
     return AVIFGPU_OK;
+}
+
+int32_t DestLayoutOf(const avifgpu_encode_desc& d) { return d.struct_size == sizeof(avifgpu_encode_desc) ? d.dest_layout : AVIFGPU_SOURCE_PLANAR; }
+
+const avifgpu_encode_desc* WidenEncodeDesc(const avifgpu_encode_desc* d, avifgpu_encode_desc* full)
+{
+    if (d == nullptr || d->struct_size != AVIFGPU_ENCODE_DESC_V10_SIZE)
+    {
+        return d;
+    }
+    std::memset(full, 0, sizeof(*full));
+    std::memcpy(full, d, AVIFGPU_ENCODE_DESC_V10_SIZE);
+    full->struct_size = sizeof(avifgpu_encode_desc);
+    full->dest_layout = AVIFGPU_SOURCE_PLANAR;
+    return full;
 }
 
 int ValidateDecodeDesc(const avifgpu_decode_desc* d, int32_t* outTransfer, std::string* error)
@@ -296,10 +318,12 @@ PlaneGeometry EncodePlaneGeometry(const avifgpu_encode_desc& d, int index)
         }
         else if (index == 1 || index == 2)
         {
-            g.present = true;
+            // interleaved chroma: plane 1 holds the Cb, Cr pairs and there is no plane 2
+            const bool interleaved = (DestLayoutOf(d) & AVIFGPU_SOURCE_CHROMA_INTERLEAVED) != 0;
+            g.present = !(interleaved && index == 2);
             g.xs = xs;
             g.ys = ys;
-            g.widthSamples = (d.width + xs) >> xs;
+            g.widthSamples = ((d.width + xs) >> xs) * (interleaved ? 2 : 1);
             g.height = (d.height + ys) >> ys;
         }
     }
@@ -386,6 +410,7 @@ void FillEncodeParams(const avifgpu_encode_desc& d, EncodeParams* p)
         p->rowMatrix[i] = d.row_matrix[i];
     }
     p->planar = d.layout == AVIFGPU_LAYOUT_PLANAR_YCBCR;
+    p->destLayout = DestLayoutOf(d);
     if (p->planar)
     {
         int xs, ys;

@@ -35,6 +35,11 @@ int32_t SourceLayoutOf(const avifgpu_decode_desc& desc);
 // `desc` is returned as it is.  The entry points widen first, so nothing after them reads past a caller's shorter struct.
 const avifgpu_decode_desc* WidenDecodeDesc(const avifgpu_decode_desc* desc, avifgpu_decode_desc* full);
 
+// The same for encodes: the description's dest_layout (avifgpu_source_layout bits), AVIFGPU_SOURCE_PLANAR for an
+// API-10-sized one; and the widening of an API-10-sized description into `full`.
+int32_t DestLayoutOf(const avifgpu_encode_desc& desc);
+const avifgpu_encode_desc* WidenEncodeDesc(const avifgpu_encode_desc* desc, avifgpu_encode_desc* full);
+
 struct PlaneGeometry
 {
     int32_t widthSamples = 0; // samples per row (interleaved: width * channels)

@@ -129,6 +129,82 @@ __device__ __forceinline__ void StoreFour(uint8_t* address, const uint32_t (&c)[
     }
 }
 
+// DEST != 0: the stores of EncodeRgbIntGroup into semi-planar and MSB-aligned planes, from the codes the planar stores
+// take.  The codes are packed into words as StoreEight / StoreFour pack them (two 16-bit or four 8-bit codes a word);
+// MSB-aligned words are shifted as they stand (CodesToMsbPair), and interleaved chroma is the Cb and Cr words paired by
+// byte permutation into one store of twice the planar bytes -- two 128-bit stores for 16-bit 4:4:4.
+template <int WORDS>
+__device__ __forceinline__ void StoreWords(uint8_t* address, const uint32_t (&w)[WORDS])
+{
+    if constexpr (WORDS == 1)
+    {
+        __stcs(reinterpret_cast<uint32_t*>(address), w[0]);
+    }
+    else if constexpr (WORDS == 2)
+    {
+        __stcs(reinterpret_cast<uint2*>(address), make_uint2(w[0], w[1]));
+    }
+    else
+    {
+#pragma unroll
+        for (int q = 0; q < WORDS / 4; ++q)
+        {
+            __stcs(reinterpret_cast<uint4*>(address) + q, make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]));
+        }
+    }
+}
+
+template <typename PlaneT, int DEST, int N>
+__device__ __forceinline__ void PackDestWords(const uint32_t (&c)[N], uint32_t shift, uint32_t (&w)[N * sizeof(PlaneT) / 4])
+{
+    static_assert(sizeof(PlaneT) == 2 || !SourceMsbAligned(DEST), "8-bit planes are never MSB-aligned");
+#pragma unroll
+    for (int i = 0; i < N * static_cast<int>(sizeof(PlaneT)) / 4; ++i)
+    {
+        w[i] = sizeof(PlaneT) == 2 ? c[2 * i] | (c[2 * i + 1] << 16) : c[4 * i] | (c[4 * i + 1] << 8) | (c[4 * i + 2] << 16) | (c[4 * i + 3] << 24);
+        if (SourceMsbAligned(DEST))
+        {
+            w[i] = CodesToMsbPair(w[i], shift);
+        }
+    }
+}
+
+// N (8 or 4) consecutive luma or alpha codes.
+template <typename PlaneT, int DEST, int N>
+__device__ __forceinline__ void StoreDestCodes(uint8_t* address, const uint32_t (&c)[N], uint32_t shift)
+{
+    uint32_t w[N * sizeof(PlaneT) / 4];
+    PackDestWords<PlaneT, DEST>(c, shift, w);
+    StoreWords(address, w);
+}
+
+// N (8 or 4) consecutive chroma sites: into plane 1 at cbAddress and plane 2 at crAddress, or, interleaved, as Cb, Cr pairs
+// into plane 1 at cbAddress.
+template <typename PlaneT, int DEST, int N>
+__device__ __forceinline__ void StoreDestChroma(uint8_t* cbAddress, uint8_t* crAddress, const uint32_t (&cb)[N], const uint32_t (&cr)[N], uint32_t shift)
+{
+    constexpr int kWords = N * sizeof(PlaneT) / 4;
+    uint32_t cbWords[kWords], crWords[kWords];
+    PackDestWords<PlaneT, DEST>(cb, shift, cbWords);
+    PackDestWords<PlaneT, DEST>(cr, shift, crWords);
+    if constexpr (SourceInterleaved(DEST))
+    {
+        uint32_t pairs[2 * kWords];
+#pragma unroll
+        for (int i = 0; i < kWords; ++i)
+        {
+            pairs[2 * i] = sizeof(PlaneT) == 2 ? LowHalves(cbWords[i], crWords[i]) : LowPairs(cbWords[i], crWords[i]);
+            pairs[2 * i + 1] = sizeof(PlaneT) == 2 ? HighHalves(cbWords[i], crWords[i]) : HighPairs(cbWords[i], crWords[i]);
+        }
+        StoreWords(cbAddress, pairs);
+    }
+    else
+    {
+        StoreWords(cbAddress, cbWords);
+        StoreWords(crAddress, crWords);
+    }
+}
+
 // The fields of the planar launch every group of `p`'s image shares; the launchers add pointers, strides and sizes.
 inline Rgb16Params RgbIntShared(const EncodeParams& p)
 {
@@ -161,10 +237,15 @@ __device__ __forceinline__ void StageHostLut(float* hostLut, uint32_t maxCode)
 // PREMULTIPLY (CHANNELS == 4 only): the colour codes are multiplied by the alpha code in the image's depth before the matrix
 // (WriteHeifImage.cpp:700-718, 760-778, 877-895, 947-965), through FastPremultiplyBiased.
 // One group: pixels [8 column, 8 column + 8) of rows (rowPair << YS) .. (rowPair << YS) + YS.
-template <typename HostT, typename PlaneT, int CHANNELS, int XS, int YS, int PREMULTIPLY>
+// DEST: the avifgpu_source_layout bits of the planes written; 0 stores with StoreEight / StoreFour, anything else with
+// StoreDestCodes / StoreDestChroma.  Nothing before the stores depends on it.
+template <typename HostT, typename PlaneT, int CHANNELS, int XS, int YS, int PREMULTIPLY, int DEST = 0>
 __device__ __forceinline__ void EncodeRgbIntGroup(const Rgb16Params& p, const float* __restrict__ hostLut, long long rowPair, int column)
 {
     constexpr int kRows = 1 + YS;
+    constexpr int kChromaPairs = SourceInterleaved(DEST) ? 2 : 1; // interleaved: Cb, Cr pairs in plane 1
+    // 16 - depth == clz(maxCode) - 16 for MSB-aligned planes (the parameter block has no depth field)
+    const uint32_t msbShift = SourceMsbAligned(DEST) ? static_cast<uint32_t>(__clz(p.maxCode) - 16) : 0u;
     constexpr int kWordsPerRow = CHANNELS * 2 * static_cast<int>(sizeof(HostT)); // 8 pixels x CHANNELS samples / 4 bytes
     constexpr int kVectorWords = (kWordsPerRow % 4 == 0) ? 4 : 2;                 // 128-bit loads where the row chunk allows
     constexpr int kPlaneBytes = static_cast<int>(sizeof(PlaneT));
@@ -323,10 +404,21 @@ __device__ __forceinline__ void EncodeRgbIntGroup(const Rgb16Params& p, const fl
             yCodes[2 * j] = BiasedToCode(luma0);
             yCodes[2 * j + 1] = BiasedToCode(luma1);
         }
-        StoreEight<PlaneT>(p.plane[0] + (y0 + r) * p.stride[0] + static_cast<long long>(column) * (8 * kPlaneBytes), yCodes);
-        if (CHANNELS == 4)
+        if constexpr (DEST == 0)
         {
-            StoreEight<PlaneT>(p.plane[3] + (y0 + r) * p.stride[3] + static_cast<long long>(column) * (8 * kPlaneBytes), aCodes);
+            StoreEight<PlaneT>(p.plane[0] + (y0 + r) * p.stride[0] + static_cast<long long>(column) * (8 * kPlaneBytes), yCodes);
+            if (CHANNELS == 4)
+            {
+                StoreEight<PlaneT>(p.plane[3] + (y0 + r) * p.stride[3] + static_cast<long long>(column) * (8 * kPlaneBytes), aCodes);
+            }
+        }
+        else
+        {
+            StoreDestCodes<PlaneT, DEST>(p.plane[0] + (y0 + r) * p.stride[0] + static_cast<long long>(column) * (8 * kPlaneBytes), yCodes, msbShift);
+            if (CHANNELS == 4)
+            {
+                StoreDestCodes<PlaneT, DEST>(p.plane[3] + (y0 + r) * p.stride[3] + static_cast<long long>(column) * (8 * kPlaneBytes), aCodes, msbShift);
+            }
         }
     }
 
@@ -356,8 +448,16 @@ __device__ __forceinline__ void EncodeRgbIntGroup(const Rgb16Params& p, const fl
                 crCode[2 * j + 1] = chromaClamp(r1);
             }
             const long long offset = static_cast<long long>(column) * (8 * kPlaneBytes);
-            StoreEight<PlaneT>(p.plane[1] + (y0 + r) * p.stride[1] + offset, cbCode);
-            StoreEight<PlaneT>(p.plane[2] + (y0 + r) * p.stride[2] + offset, crCode);
+            if constexpr (DEST == 0)
+            {
+                StoreEight<PlaneT>(p.plane[1] + (y0 + r) * p.stride[1] + offset, cbCode);
+                StoreEight<PlaneT>(p.plane[2] + (y0 + r) * p.stride[2] + offset, crCode);
+            }
+            else
+            {
+                StoreDestChroma<PlaneT, DEST>(p.plane[1] + (y0 + r) * p.stride[1] + offset * kChromaPairs, p.plane[2] + (y0 + r) * p.stride[2] + offset,
+                                              cbCode, crCode, msbShift);
+            }
         }
     }
     else
@@ -408,8 +508,16 @@ __device__ __forceinline__ void EncodeRgbIntGroup(const Rgb16Params& p, const fl
         }
         const long long offset = static_cast<long long>(column) * (4 * kPlaneBytes);
         const long long chromaRow = YS ? rowPair : y0;
-        StoreFour<PlaneT>(p.plane[1] + chromaRow * p.stride[1] + offset, cbCode);
-        StoreFour<PlaneT>(p.plane[2] + chromaRow * p.stride[2] + offset, crCode);
+        if constexpr (DEST == 0)
+        {
+            StoreFour<PlaneT>(p.plane[1] + chromaRow * p.stride[1] + offset, cbCode);
+            StoreFour<PlaneT>(p.plane[2] + chromaRow * p.stride[2] + offset, crCode);
+        }
+        else
+        {
+            StoreDestChroma<PlaneT, DEST>(p.plane[1] + chromaRow * p.stride[1] + offset * kChromaPairs, p.plane[2] + chromaRow * p.stride[2] + offset, cbCode,
+                                          crCode, msbShift);
+        }
     }
 }
 

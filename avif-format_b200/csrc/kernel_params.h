@@ -114,6 +114,7 @@ struct EncodeParams
     const uint16_t* gray16Lut;        // 65536-entry code table for Gray16 hosts (device memory), or nullptr
     int32_t smCount;
     int32_t verifiedPremultiply;      // 1 once the context has verified FastPremultiplyBiased for this image depth on this device
+    int32_t destLayout;               // avifgpu_source_layout bits of the planes written (planar YCbCr only): Cb, Cr pairs in plane 1; codes in the top bits
 };
 
 struct DecodeParams
@@ -147,8 +148,8 @@ struct DecodeParams
     int32_t sourceLayout;          // avifgpu_source_layout bits (YCbCr only): Cb, Cr pairs in plane 1; codes in the top bits
 };
 
-// The source layout of a decode, as the tuned kernels take it: a template argument SOURCE whose bits are these, 0 being
-// libheif's planar, low-bit layout.
+// The source layout of a decode or the destination layout of an encode, as the tuned kernels take it: a template argument
+// (SOURCE, DEST) whose bits are these, 0 being libheif's planar, low-bit layout.
 AVIFGPU_HD constexpr bool SourceInterleaved(int source) { return (source & AVIFGPU_SOURCE_CHROMA_INTERLEAVED) != 0; }
 AVIFGPU_HD constexpr bool SourceMsbAligned(int source) { return (source & AVIFGPU_SOURCE_MSB_ALIGNED) != 0; }
 
@@ -158,7 +159,8 @@ AVIFGPU_HD constexpr bool SourceMsbAligned(int source) { return (source & AVIFGP
 // sub-sampled (FillEncodeParams / FillDecodeParams leave xs = ys = 0 for every other layout), and only plane 0 of the
 // reference layout with three or more channels interleaves `channels` samples per pixel.  A null plane stays null.
 // Blocks carry no column phase, so x0 starts a chroma site (a multiple of 1 << xs); an encode block has no row phase
-// either, so y0 is a multiple of 1 << ys (tests/native/launch_window_check.cpp).
+// either, so y0 is a multiple of 1 << ys (tests/native/launch_window_check.cpp).  Interleaved chroma (plane 1 only) moves
+// by two samples per site.
 AVIFGPU_HD inline EncodeParams EncodeWindow(const EncodeParams& p, int hostDepth, int x0, int y0, int width, int rows)
 {
     EncodeParams w = p;
@@ -171,7 +173,7 @@ AVIFGPU_HD inline EncodeParams EncodeWindow(const EncodeParams& p, int hostDepth
             continue;
         }
         const bool chroma = k == 1 || k == 2;
-        const int samplesPerPixel = (!p.planar && k == 0 && p.channels >= 3) ? p.channels : 1;
+        const int samplesPerPixel = (!p.planar && k == 0 && p.channels >= 3) ? p.channels : (k == 1 && SourceInterleaved(p.destLayout)) ? 2 : 1;
         w.plane[k] = static_cast<uint8_t*>(p.plane[k]) + static_cast<int64_t>(y0 >> (chroma ? p.ys : 0)) * p.planeStride[k] +
                      static_cast<int64_t>(x0 >> (chroma ? p.xs : 0)) * samplesPerPixel * sampleBytes;
     }
@@ -236,7 +238,9 @@ struct Interior
 };
 // EncodeRgbIntInterior in two halves: the description's (host depth, layout, channels, premultiply, depth, matrix --
 // the same for every block of one description, host only) and the block's (buffer alignment, at least 8 pixels and one
-// 4:2:0 row pair).
+// 4:2:0 row pair).  Interleaved chroma is one plane of Cb, Cr pairs a thread writes in one store of twice the planar
+// chroma's bytes (two 128-bit stores for 16-bit 4:4:4), so it is aligned to that store, at most 16 bytes; the
+// destination layout is the block's business only, so the description's half does not read it.
 bool EncodeRgbIntTuned(const EncodeParams& p, int hostDepth);
 AVIFGPU_HD inline Interior EncodeRgbIntBlockInterior(const EncodeParams& p, int hostDepth)
 {
@@ -246,8 +250,10 @@ AVIFGPU_HD inline Interior EncodeRgbIntBlockInterior(const EncodeParams& p, int 
     const int rowAlign = (8 * p.channels * hostBytes) % 16 == 0 ? 16 : 8; // a thread's 8-pixel chunk: 128-bit or 64-bit loads
     const int lumaAlign = 8 * planeBytes;
     const int chromaAlign = (p.xs ? 4 : 8) * planeBytes;
-    if (p.width < 8 || !Aligned(p.rows, p.rowStride, rowAlign) || !Aligned(p.plane[0], p.planeStride[0], lumaAlign) ||
-        !Aligned(p.plane[1], p.planeStride[1], chromaAlign) || !Aligned(p.plane[2], p.planeStride[2], chromaAlign) ||
+    const bool chromaAligned = SourceInterleaved(p.destLayout)
+                                   ? Aligned(p.plane[1], p.planeStride[1], 2 * chromaAlign > 16 ? 16 : 2 * chromaAlign)
+                                   : Aligned(p.plane[1], p.planeStride[1], chromaAlign) && Aligned(p.plane[2], p.planeStride[2], chromaAlign);
+    if (p.width < 8 || !Aligned(p.rows, p.rowStride, rowAlign) || !Aligned(p.plane[0], p.planeStride[0], lumaAlign) || !chromaAligned ||
         (p.channels == 4 && !Aligned(p.plane[3], p.planeStride[3], lumaAlign)))
     {
         return none;
@@ -260,6 +266,32 @@ AVIFGPU_HD inline Interior EncodeRgbIntBlockInterior(const EncodeParams& p, int 
     return Interior{ p.width & ~7, evenRows };
 }
 Interior EncodeRgbIntInterior(const EncodeParams& p, int hostDepth); // EncodeRgbIntTuned ? EncodeRgbIntBlockInterior : none
+
+// The block's half of the tuned float planar encodes (EncodeRgbF32FlatKernel, EncodeRgbaF32FlatKernel,
+// EncodeRgbF32ClipKernel; LaunchEncodeFast has the description's): 10/12-bit planes, a lane on 4 pixels of each of 2 rows,
+// 128-bit row loads, 64-bit luma and alpha stores, 32-bit (4:2:0, 4:2:2) or 64-bit (4:4:4) planar chroma stores -- or,
+// into interleaved chroma, one store of twice those bytes -- and at least 4 x (1 << ys) pixels.  width is a multiple of
+// 4, rows of 1 << ys.
+AVIFGPU_HD inline Interior EncodeRgbF32BlockInterior(const EncodeParams& p)
+{
+    const Interior none = { 0, 0 };
+    const int chromaAlign = p.xs ? 4 : 8;
+    const bool chromaAligned = SourceInterleaved(p.destLayout)
+                                   ? Aligned(p.plane[1], p.planeStride[1], 2 * chromaAlign)
+                                   : Aligned(p.plane[1], p.planeStride[1], chromaAlign) && Aligned(p.plane[2], p.planeStride[2], chromaAlign);
+    if (!Aligned(p.rows, p.rowStride, 16) || !Aligned(p.plane[0], p.planeStride[0], 8) || !chromaAligned ||
+        (p.channels == 4 && p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], 8)))
+    {
+        return none;
+    }
+    const int width4 = p.width & ~3;
+    const int evenRows = p.ys ? (p.rowCount & ~1) : p.rowCount;
+    if (width4 < 4 || evenRows < 1)
+    {
+        return none;
+    }
+    return Interior{ width4, evenRows };
+}
 
 // The same for the tuned integer YCbCr decode kernel (DecodeYccToRgbIntKernel): 8/16-bit hosts reading 8-bit / 10-12-bit
 // YCbCr (+ straight alpha), a block starting on a 4:2:0 row pair, aligned buffers, at least 8 x (1 << ys) pixels.

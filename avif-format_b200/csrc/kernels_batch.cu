@@ -285,7 +285,7 @@ __global__ void __launch_bounds__(kPlanThreads) PlanIndirectKernel(const __grid_
     }
 }
 
-template <typename Source, typename HostT, typename PlaneT, int CHANNELS, int XS, int YS, int PREMULTIPLY>
+template <typename Source, typename HostT, typename PlaneT, int CHANNELS, int XS, int YS, int PREMULTIPLY, int DEST>
 __global__ void __launch_bounds__(kRgbThreads) EncodeRgbIntBatchKernel(const __grid_constant__ Source s)
 {
     const typename Source::Walk walk(s);
@@ -319,7 +319,7 @@ __global__ void __launch_bounds__(kRgbThreads) EncodeRgbIntBatchKernel(const __g
         const int column = (local - rowPair * unitsX) * 32 + lane;
         if (column < p.groupsPerRow)
         {
-            EncodeRgbIntGroup<HostT, PlaneT, CHANNELS, XS, YS, PREMULTIPLY>(p, hostLut, rowPair, column);
+            EncodeRgbIntGroup<HostT, PlaneT, CHANNELS, XS, YS, PREMULTIPLY, DEST>(p, hostLut, rowPair, column);
         }
     }
 }
@@ -630,8 +630,8 @@ __global__ void __launch_bounds__(kBatchEdgeThreads) DecodeBatchKernel(const __g
 template <typename Source>
 void LaunchRgbInt(const Source& s, const EncodeParams& d, int hostDepth, unsigned grid, cudaStream_t stream)
 {
-    WithRgbIntKey(d, hostDepth, [&](auto host, auto plane, auto channels, auto premultiply, auto xs, auto ys) {
-        EncodeRgbIntBatchKernel<Source, TypeOf<decltype(host)>, TypeOf<decltype(plane)>, channels(), xs(), ys(), premultiply()><<<grid, kRgbThreads, 0, stream>>>(s);
+    WithRgbIntKey(d, hostDepth, [&](auto host, auto plane, auto channels, auto premultiply, auto xs, auto ys, auto dest) {
+        EncodeRgbIntBatchKernel<Source, TypeOf<decltype(host)>, TypeOf<decltype(plane)>, channels(), xs(), ys(), premultiply(), dest()><<<grid, kRgbThreads, 0, stream>>>(s);
     });
 }
 

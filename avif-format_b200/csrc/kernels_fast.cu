@@ -28,9 +28,11 @@ constexpr int kClipWarps = kClipThreads / 32;
 constexpr int kClipBlocksPerSm = 3;
 
 // No transfer curve (AVIFGPU_TRANSFER_CLIP): code = trunc(clamp(v * max)) per sample (WriteHeifImage.cpp:1128-1130), then
-// the forward matrix.  No tables, no shared memory; the loads of tile i+1 are issued before tile i's arithmetic.
-template <int XS, int YS>
-__global__ void __launch_bounds__(kClipThreads, kClipBlocksPerSm) EncodeRgbF32ClipKernel(const FastEncodeParams p)
+// the forward matrix.  No tables, no shared memory; the loads of tile i+1 are issued before tile i's arithmetic.  DEST:
+// the avifgpu_source_layout bits of the planes written (StoreTile).  The body of EncodeRgbF32ClipKernel (DEST 0) and of
+// EncodeDestRgbF32ClipKernel (the other layouts).
+template <int XS, int YS, int DEST>
+__device__ __forceinline__ void EncodeRgbF32ClipBody(const FastEncodeParams& p)
 {
     const int lane = threadIdx.x & 31;
     const int warpInBlock = threadIdx.x >> 5;
@@ -98,13 +100,27 @@ __global__ void __launch_bounds__(kClipThreads, kClipBlocksPerSm) EncodeRgbF32Cl
         {
             const int64_t chromaRow = YS ? currentRow : y0;
             const int64_t chromaColumn = static_cast<int64_t>(XS ? (x0 >> 1) : x0) * 2;
-            StoreTile<XS, YS>(p, codeF, p.planeY + static_cast<int64_t>(y0) * p.strideY + static_cast<int64_t>(x0) * 2,
-                              p.planeCb + chromaRow * p.strideCb + chromaColumn, p.planeCr + chromaRow * p.strideCr + chromaColumn, secondRow);
+            StoreTile<XS, YS, DEST>(p, codeF, p.planeY + static_cast<int64_t>(y0) * p.strideY + static_cast<int64_t>(x0) * 2,
+                                    p.planeCb + chromaRow * p.strideCb + chromaColumn * (SourceInterleaved(DEST) ? 2 : 1),
+                                    p.planeCr + chromaRow * p.strideCr + chromaColumn, secondRow);
         }
     }
 }
 
 template <int XS, int YS>
+__global__ void __launch_bounds__(kClipThreads, kClipBlocksPerSm) EncodeRgbF32ClipKernel(const FastEncodeParams p)
+{
+    EncodeRgbF32ClipBody<XS, YS, AVIFGPU_SOURCE_PLANAR>(p);
+}
+
+// The same into semi-planar and MSB-aligned planes (DEST != 0).
+template <int XS, int YS, int DEST>
+__global__ void __launch_bounds__(kClipThreads, kClipBlocksPerSm) EncodeDestRgbF32ClipKernel(const FastEncodeParams p)
+{
+    EncodeRgbF32ClipBody<XS, YS, DEST>(p);
+}
+
+template <int XS, int YS, int DEST>
 cudaError_t LaunchClipKernel(const FastEncodeParams& fp, int smCount, cudaStream_t stream)
 {
     const long long tiles = static_cast<long long>((fp.width + kTilePixels - 1) / kTilePixels) * ((fp.rowCount + 1) / 2);
@@ -113,7 +129,14 @@ cudaError_t LaunchClipKernel(const FastEncodeParams& fp, int smCount, cudaStream
         return cudaErrorInvalidValue;
     }
     const unsigned grid = GridFor((tiles + kClipWarps - 1) / kClipWarps, static_cast<long long>(smCount) * kClipBlocksPerSm);
-    EncodeRgbF32ClipKernel<XS, YS><<<grid, kClipThreads, 0, stream>>>(fp);
+    if constexpr (DEST == AVIFGPU_SOURCE_PLANAR)
+    {
+        EncodeRgbF32ClipKernel<XS, YS><<<grid, kClipThreads, 0, stream>>>(fp);
+    }
+    else
+    {
+        EncodeDestRgbF32ClipKernel<XS, YS, DEST><<<grid, kClipThreads, 0, stream>>>(fp);
+    }
     return cudaGetLastError();
 }
 
@@ -173,22 +196,17 @@ int LaunchEncodeFast(const EncodeParams& p, int hostDepth, void* streamHandle)
     {
         return 0; // an exotic matrix: the generic kernel clamps
     }
-    if (!Aligned(p.rows, p.rowStride, 16) || !Aligned(p.plane[0], p.planeStride[0], 8) ||
-        !Aligned(p.plane[1], p.planeStride[1], p.xs ? 4 : 8) || !Aligned(p.plane[2], p.planeStride[2], p.xs ? 4 : 8) ||
-        (rgba && !Aligned(p.plane[3], p.planeStride[3], 8)))
-    {
-        return 0;
-    }
     if (rgba && (curve == kCurveClip || p.curveTable->compact == nullptr || p.curveTable->bandBits == nullptr))
     {
         return 0; // the RGBA kernel is built on the compact table + band bitmap; everything else with alpha: generic
     }
-    const int width4 = p.width & ~3;
-    const int evenRows = p.ys ? (p.rowCount & ~1) : p.rowCount;
-    if (width4 < 4 || evenRows < 1)
+    const Interior inner = EncodeRgbF32BlockInterior(p); // aligned buffers, at least 4 x (1 << ys) pixels
+    if (inner.width == 0)
     {
         return 0;
     }
+    const int width4 = inner.width;
+    const int evenRows = inner.rows;
 
     FastEncodeParams fp{};
     fp.rows = static_cast<const uint8_t*>(p.rows);
@@ -226,19 +244,21 @@ int LaunchEncodeFast(const EncodeParams& p, int hostDepth, void* streamHandle)
         {
             return 0;
         }
-        e = LaunchFastEncodeRgba(fp, curve, p.xs, p.ys, smCount, stream);
+        e = LaunchFastEncodeRgba(fp, curve, p.xs, p.ys, p.destLayout, smCount, stream);
     }
     else if (curve != kCurveClip)
     {
-        if (!FlatEncodeApplies(fp))
+        if (!FlatEncodeApplies(fp) || !FlatEncodeReaches(fp, curve, p.destLayout))
         {
             return 0; // a table too large to sit beside the staging buffers: the generic kernel looks it up in global memory
         }
-        e = LaunchFastEncodeFlat(fp, curve, p.xs, p.ys, smCount, stream);
+        e = LaunchFastEncodeFlat(fp, curve, p.xs, p.ys, p.destLayout, smCount, stream);
     }
     else
     {
-        e = WithChroma(p.xs, p.ys, [&](auto xs, auto ys) { return LaunchClipKernel<xs(), ys()>(fp, smCount, stream); });
+        e = WithChroma(p.xs, p.ys, [&](auto xs, auto ys) {
+            return WithLayout(p.destLayout, [&](auto dest) { return LaunchClipKernel<xs(), ys(), dest()>(fp, smCount, stream); });
+        });
     }
     return CompleteEncode(e, p, hostDepth, width4, evenRows, streamHandle);
 }

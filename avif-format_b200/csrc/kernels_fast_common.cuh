@@ -6,6 +6,7 @@
 #include "kernel_params.h"
 #include "curve_lookup.cuh"
 #include "packed_f32x2.cuh"
+#include "source_units.cuh"
 
 #include <cuda_runtime.h>
 
@@ -55,7 +56,54 @@ struct FastEncodeParams
 // register pair, so the two chroma sites of a 4:2:0 / 4:2:2 lane are the two halves of one packed value.  The operation
 // sequence per pixel is pixel_math.cuh's ForwardPixelFloat, rounding for rounding; see packed_f32x2.cuh for which
 // operations may be packed (a product's sum is always a scalar add).
-template <int XS, int YS>
+//
+// DEST: the avifgpu_source_layout bits of the planes written (0: libheif's planar, low-bit layout).  Everything up to the
+// stores is the same; then MSB-aligned codes are shifted two at a time as packed words (MsbWord), and with interleaved
+// chroma cbRow points at the lane's first Cb, Cr pair of plane 1: the lane's Cb and Cr words are paired by byte permutation
+// into one store of twice the planar bytes (crRow is not used).
+template <int DEST>
+__device__ __forceinline__ uint32_t MsbWord(uint32_t twoCodes, const FastEncodeParams& p)
+{
+    // 16 - depth == clz(maxCode) - 16 (the parameter block has no depth field)
+    return SourceMsbAligned(DEST) ? CodesToMsbPair(twoCodes, static_cast<uint32_t>(__clz(p.maxCode) - 16)) : twoCodes;
+}
+
+// The Cb and Cr words of one chroma row -- two codes each, sites (0, 1) -- as a lane stores them.
+template <int DEST>
+__device__ __forceinline__ void StoreChromaWords(const FastEncodeParams& p, uint8_t* cbRow, uint8_t* crRow, uint32_t cbWord, uint32_t crWord)
+{
+    cbWord = MsbWord<DEST>(cbWord, p);
+    crWord = MsbWord<DEST>(crWord, p);
+    if (SourceInterleaved(DEST))
+    {
+        __stcs(reinterpret_cast<uint2*>(cbRow), make_uint2(LowHalves(cbWord, crWord), HighHalves(cbWord, crWord)));
+    }
+    else
+    {
+        __stcs(reinterpret_cast<uint32_t*>(cbRow), cbWord);
+        __stcs(reinterpret_cast<uint32_t*>(crRow), crWord);
+    }
+}
+
+// The same for 4:4:4: two words each, sites (0, 1) and (2, 3).
+template <int DEST>
+__device__ __forceinline__ void StoreChromaWords(const FastEncodeParams& p, uint8_t* cbRow, uint8_t* crRow, uint2 cbWords, uint2 crWords)
+{
+    cbWords = make_uint2(MsbWord<DEST>(cbWords.x, p), MsbWord<DEST>(cbWords.y, p));
+    crWords = make_uint2(MsbWord<DEST>(crWords.x, p), MsbWord<DEST>(crWords.y, p));
+    if (SourceInterleaved(DEST))
+    {
+        __stcs(reinterpret_cast<uint4*>(cbRow), make_uint4(LowHalves(cbWords.x, crWords.x), HighHalves(cbWords.x, crWords.x),
+                                                          LowHalves(cbWords.y, crWords.y), HighHalves(cbWords.y, crWords.y)));
+    }
+    else
+    {
+        __stcs(reinterpret_cast<uint2*>(cbRow), cbWords);
+        __stcs(reinterpret_cast<uint2*>(crRow), crWords);
+    }
+}
+
+template <int XS, int YS, int DEST = 0>
 __device__ __forceinline__ void StoreTile(const FastEncodeParams& p, const float (&codeF)[kValuesPerLane], uint8_t* yRow, uint8_t* cbRow, uint8_t* crRow,
                                           bool secondRow)
 {
@@ -102,10 +150,10 @@ __device__ __forceinline__ void StoreTile(const FastEncodeParams& p, const float
         yWord[r][0] = yLow[0] | (yLow[1] << 16);   // pixels 0, 1
         yWord[r][1] = yHigh[0] | (yHigh[1] << 16); // pixels 2, 3
     }
-    __stcs(reinterpret_cast<uint2*>(yRow), make_uint2(yWord[0][0], yWord[0][1]));
+    __stcs(reinterpret_cast<uint2*>(yRow), make_uint2(MsbWord<DEST>(yWord[0][0], p), MsbWord<DEST>(yWord[0][1], p)));
     if (secondRow)
     {
-        __stcs(reinterpret_cast<uint2*>(yRow + p.strideY), make_uint2(yWord[1][0], yWord[1][1]));
+        __stcs(reinterpret_cast<uint2*>(yRow + p.strideY), make_uint2(MsbWord<DEST>(yWord[1][0], p), MsbWord<DEST>(yWord[1][1], p)));
     }
 
     // (chroma + offset) + 0.5 -> code, both halves; `biased` is a scalar-add result or an exact scaling, never a product
@@ -146,8 +194,7 @@ __device__ __forceinline__ void StoreTile(const FastEncodeParams& p, const float
             cbWord = quantisePair(Fma2(cbSum, quarter2, offset2));
             crWord = quantisePair(Fma2(crSum, quarter2, offset2));
         }
-        __stcs(reinterpret_cast<uint32_t*>(cbRow), cbWord);
-        __stcs(reinterpret_cast<uint32_t*>(crRow), crWord);
+        StoreChromaWords<DEST>(p, cbRow, crRow, cbWord, crWord);
     }
     else if (XS == 1)
     {
@@ -166,8 +213,7 @@ __device__ __forceinline__ void StoreTile(const FastEncodeParams& p, const float
                 cbWord = quantisePair(Fma2(addHalves(cb2[r][0], cb2[r][1]), half2, offset2)); // (c0 + c1) * 0.5f + offset, exact scaling
                 crWord = quantisePair(Fma2(addHalves(cr2[r][0], cr2[r][1]), half2, offset2));
             }
-            __stcs(reinterpret_cast<uint32_t*>(cbRow + r * p.strideCb), cbWord);
-            __stcs(reinterpret_cast<uint32_t*>(crRow + r * p.strideCr), crWord);
+            StoreChromaWords<DEST>(p, cbRow + r * p.strideCb, crRow + r * p.strideCr, cbWord, crWord);
         }
     }
     else
@@ -179,21 +225,23 @@ __device__ __forceinline__ void StoreTile(const FastEncodeParams& p, const float
             // pairs hold pixels (0, 2) and (1, 3); the stores want (0, 1) and (2, 3)
             const uint32_t cbEven = quantisePair(addOffset(cb2[r][0])), cbOdd = quantisePair(addOffset(cb2[r][1]));
             const uint32_t crEven = quantisePair(addOffset(cr2[r][0])), crOdd = quantisePair(addOffset(cr2[r][1]));
-            __stcs(reinterpret_cast<uint2*>(cbRow + r * p.strideCb), make_uint2(__byte_perm(cbEven, cbOdd, 0x5410), __byte_perm(cbEven, cbOdd, 0x7632)));
-            __stcs(reinterpret_cast<uint2*>(crRow + r * p.strideCr), make_uint2(__byte_perm(crEven, crOdd, 0x5410), __byte_perm(crEven, crOdd, 0x7632)));
+            StoreChromaWords<DEST>(p, cbRow + r * p.strideCb, crRow + r * p.strideCr,
+                                   make_uint2(__byte_perm(cbEven, cbOdd, 0x5410), __byte_perm(cbEven, cbOdd, 0x7632)),
+                                   make_uint2(__byte_perm(crEven, crOdd, 0x5410), __byte_perm(crEven, crOdd, 0x7632)));
         }
     }
 }
 
 } // namespace fastenc
 
-// kernels_fast_rgba.cu
+// kernels_fast_rgba.cu; `dest` is the description's avifgpu_source_layout bits (EncodeParams::destLayout)
 bool RgbaEncodeApplies(const fastenc::FastEncodeParams& fp);
-cudaError_t LaunchFastEncodeRgba(const fastenc::FastEncodeParams& fp, int curve, int xs, int ys, int smCount, cudaStream_t stream);
+cudaError_t LaunchFastEncodeRgba(const fastenc::FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream);
 
 // kernels_fast_flat.cu
 bool FlatEncodeApplies(const fastenc::FastEncodeParams& fp);
-cudaError_t LaunchFastEncodeFlat(const fastenc::FastEncodeParams& fp, int curve, int xs, int ys, int smCount, cudaStream_t stream);
+bool FlatEncodeReaches(const fastenc::FastEncodeParams& fp, int curve, int dest); // an instantiation exists for the table's form
+cudaError_t LaunchFastEncodeFlat(const fastenc::FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream);
 cudaError_t LaunchFastEncodeFlatInterleaved(const fastenc::FastEncodeParams& fp, int curve, int smCount, cudaStream_t stream);
 
 } // namespace avifgpu

@@ -77,8 +77,11 @@ constexpr int kTableCompact14 = 3;
 
 // INTERLEAVED = 1: the reference's own output layout (heif_channel_interleaved RGB, WriteHeifImage.cpp:1098-1130) -- the
 // codes are stored as they are, 3 x uint16 per pixel into plane Y's buffer, no matrix (XS = YS = 0 then).
-template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED>
-__global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const FastEncodeParams p, const FlatSchedule schedule)
+// DEST: the avifgpu_source_layout bits of the YCbCr planes written (StoreTile); with interleaved chroma the lane's chroma
+// pointer walks plane 1 in steps of twice the bytes.  The body of EncodeRgbF32FlatKernel (DEST 0) and of
+// EncodeDestRgbF32FlatKernel (the other layouts).
+template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED, int DEST>
+__device__ __forceinline__ void EncodeRgbF32FlatBody(const FastEncodeParams& p, const FlatSchedule& schedule)
 {
     constexpr bool kCompact = TABLE != kTableTwoLevel;
     constexpr int kCompactShift = TABLE == kTableCompact14 ? 14 : 0;
@@ -107,7 +110,8 @@ __global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const 
     // fraction of them.
     const int firstItem = warpInBlock * static_cast<int>(gridDim.x) + static_cast<int>(blockIdx.x);
     constexpr int kChromaRowsPerTile = YS ? 1 : 2;
-    constexpr int kChromaTileBytes = XS ? kTilePixels : 2 * kTilePixels;
+    constexpr int kChromaPairs = SourceInterleaved(DEST) ? 2 : 1; // interleaved: Cb, Cr pairs in plane 1
+    constexpr int kChromaTileBytes = (XS ? kTilePixels : 2 * kTilePixels) * kChromaPairs;
 
     // An item's tile column and its run of tile rows [rowBegin, rowEnd).
     auto itemRows = [&](int item, int& column, int& rowBegin, int& rowEnd)
@@ -193,7 +197,7 @@ __global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const 
         int64_t sourceOffset = sourceOffsetOf(rowBegin, column);
         uint8_t* yPointer = p.planeY + static_cast<int64_t>(rowBegin) * 2 * p.strideY +
                             (INTERLEAVED ? static_cast<int64_t>(column) * (6 * kTilePixels) + lane * 24 : static_cast<int64_t>(column) * (2 * kTilePixels) + lane * 8);
-        uint8_t* cbPointer = p.planeCb + static_cast<int64_t>(rowBegin) * kChromaRowsPerTile * p.strideCb + static_cast<int64_t>(column) * kChromaTileBytes + lane * (XS ? 4 : 8);
+        uint8_t* cbPointer = p.planeCb + static_cast<int64_t>(rowBegin) * kChromaRowsPerTile * p.strideCb + static_cast<int64_t>(column) * kChromaTileBytes + lane * (XS ? 4 : 8) * kChromaPairs;
         uint8_t* crPointer = p.planeCr + static_cast<int64_t>(rowBegin) * kChromaRowsPerTile * p.strideCr + static_cast<int64_t>(column) * kChromaTileBytes + lane * (XS ? 4 : 8);
 
 #pragma unroll 1
@@ -339,7 +343,7 @@ __global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const 
             }
             else
             {
-                StoreTile<XS, YS>(p, codeF, yPointer, cbPointer, crPointer, secondRow);
+                StoreTile<XS, YS, DEST>(p, codeF, yPointer, cbPointer, crPointer, secondRow);
             }
         }
         yPointer += 2 * p.strideY;
@@ -349,18 +353,44 @@ __global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const 
     }
 }
 
+template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED>
+__global__ void __launch_bounds__(kFlatThreads, 1) EncodeRgbF32FlatKernel(const FastEncodeParams p, const FlatSchedule schedule)
+{
+    EncodeRgbF32FlatBody<CURVE, XS, YS, TABLE, INTERLEAVED, AVIFGPU_SOURCE_PLANAR>(p, schedule);
+}
+
+// The same into semi-planar and MSB-aligned planes (DEST != 0).
+template <int CURVE, int XS, int YS, int TABLE, int DEST>
+__global__ void __launch_bounds__(kFlatThreads, 1) EncodeDestRgbF32FlatKernel(const FastEncodeParams p, const FlatSchedule schedule)
+{
+    EncodeRgbF32FlatBody<CURVE, XS, YS, TABLE, 0, DEST>(p, schedule);
+}
+
+template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED, int DEST>
+constexpr auto FlatKernelFor()
+{
+    if constexpr (DEST == AVIFGPU_SOURCE_PLANAR)
+    {
+        return EncodeRgbF32FlatKernel<CURVE, XS, YS, TABLE, INTERLEAVED>;
+    }
+    else
+    {
+        return EncodeDestRgbF32FlatKernel<CURVE, XS, YS, TABLE, DEST>;
+    }
+}
+
 inline size_t TableSharedBytes(const FastEncodeParams& fp, int table)
 {
     return table == kTableTwoLevel ? 2048 + static_cast<size_t>(fp.table.bucketCount) * sizeof(uint32_t) : fp.table.compactImageBytes;
 }
 
-template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED = 0>
+template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED = 0, int DEST = AVIFGPU_SOURCE_PLANAR>
 cudaError_t LaunchFlatKernel(const FastEncodeParams& fp, int smCount, cudaStream_t stream)
 {
     const size_t shared = static_cast<size_t>(FlatFixedBytes()) + TableSharedBytes(fp, TABLE);
     static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
     {
-        const cudaError_t e = AllowDynamicShared(EncodeRgbF32FlatKernel<CURVE, XS, YS, TABLE, INTERLEAVED>, kSharedLimit, configuredDevices);
+        const cudaError_t e = AllowDynamicShared(FlatKernelFor<CURVE, XS, YS, TABLE, INTERLEAVED, DEST>(), kSharedLimit, configuredDevices);
         if (e != cudaSuccess)
         {
             return e;
@@ -388,7 +418,7 @@ cudaError_t LaunchFlatKernel(const FastEncodeParams& fp, int smCount, cudaStream
     schedule.longSegments = schedule.tileRows % schedule.segments;
     schedule.lastColumnBytes = (fp.width - (schedule.tilesX - 1) * kTilePixels) * 12;
     schedule.unpairedTileRow = (fp.rowCount & 1) ? fp.rowCount / 2 : -1;
-    EncodeRgbF32FlatKernel<CURVE, XS, YS, TABLE, INTERLEAVED><<<static_cast<unsigned>(blocks), kFlatThreads, shared, stream>>>(fp, schedule);
+    FlatKernelFor<CURVE, XS, YS, TABLE, INTERLEAVED, DEST>()<<<static_cast<unsigned>(blocks), kFlatThreads, shared, stream>>>(fp, schedule);
     return cudaGetLastError();
 }
 
@@ -429,20 +459,39 @@ cudaError_t LaunchFastEncodeFlatInterleaved(const FastEncodeParams& fp, int curv
     return LaunchFlatKernel<kCurveLinearToSMPTE428, 0, 0, kTableTwoLevel, 1>(fp, smCount, stream);
 }
 
-cudaError_t LaunchFastEncodeFlat(const FastEncodeParams& fp, int curve, int xs, int ys, int smCount, cudaStream_t stream)
+// The planar layout keeps every (curve, table) pair.  The other layouts (DEST != 0, picked by WithLayout) instantiate only
+// the pairs the tables built for 10/12-bit encodes reach (DESIGN.md 4.2): PQ with the compact table (kTableCompact14 for
+// flatShift 14, as at 12 bits, kTableCompact for any other shift), SMPTE 428 with the compact table (10 bits) or the
+// two-level one (12 bits, the only form built there).  A PQ table without its compact form has not been built for any
+// configuration so far; it returns false here and the launcher leaves the block to the generic kernel.
+bool FlatEncodeReaches(const FastEncodeParams& fp, int curve, int dest)
+{
+    return dest == AVIFGPU_SOURCE_PLANAR || curve != kCurveLinearToPQ || CompactTableFits(fp);
+}
+
+cudaError_t LaunchFastEncodeFlat(const FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream)
 {
     return WithChroma(xs, ys, [&](auto XS, auto YS) {
-        if (CompactTableFits(fp))
-        {
-            if (curve == kCurveLinearToPQ)
+        return WithLayout(dest, [&](auto DEST) {
+            if (CompactTableFits(fp))
             {
-                return fp.table.flatShift == 14 ? LaunchFlatKernel<kCurveLinearToPQ, XS(), YS(), kTableCompact14>(fp, smCount, stream)
-                                                : LaunchFlatKernel<kCurveLinearToPQ, XS(), YS(), kTableCompact>(fp, smCount, stream);
+                if (curve == kCurveLinearToPQ)
+                {
+                    return fp.table.flatShift == 14 ? LaunchFlatKernel<kCurveLinearToPQ, XS(), YS(), kTableCompact14, 0, DEST()>(fp, smCount, stream)
+                                                    : LaunchFlatKernel<kCurveLinearToPQ, XS(), YS(), kTableCompact, 0, DEST()>(fp, smCount, stream);
+                }
+                return LaunchFlatKernel<kCurveLinearToSMPTE428, XS(), YS(), kTableCompact, 0, DEST()>(fp, smCount, stream);
             }
-            return LaunchFlatKernel<kCurveLinearToSMPTE428, XS(), YS(), kTableCompact>(fp, smCount, stream);
-        }
-        if (curve == kCurveLinearToPQ) return LaunchFlatKernel<kCurveLinearToPQ, XS(), YS(), kTableTwoLevel>(fp, smCount, stream);
-        return LaunchFlatKernel<kCurveLinearToSMPTE428, XS(), YS(), kTableTwoLevel>(fp, smCount, stream);
+            if constexpr (DEST() == AVIFGPU_SOURCE_PLANAR)
+            {
+                if (curve == kCurveLinearToPQ) return LaunchFlatKernel<kCurveLinearToPQ, XS(), YS(), kTableTwoLevel>(fp, smCount, stream);
+            }
+            else if (curve == kCurveLinearToPQ)
+            {
+                return cudaErrorInvalidValue; // FlatEncodeReaches said no: the launcher does not get here
+            }
+            return LaunchFlatKernel<kCurveLinearToSMPTE428, XS(), YS(), kTableTwoLevel, 0, DEST()>(fp, smCount, stream);
+        });
     });
 }
 

@@ -32,9 +32,11 @@ constexpr int kSharedLimit = 227 * 1024;
 constexpr int kTableBarrierBytes = 16; // the table image's mbarrier, padded
 __host__ __device__ constexpr int RgbaFixedBytes() { return kSharedLibm + kTableBarrierBytes + kRgbaWarps * kStagePerWarp; }
 
-// The compact table + first_k array in shared memory (kernels_fast_flat.cu has the commentary).
-template <int CURVE, int XS, int YS>
-__global__ void __launch_bounds__(kRgbaThreads, 1) EncodeRgbaF32FlatKernel(const FastEncodeParams p)
+// The compact table + first_k array in shared memory (kernels_fast_flat.cu has the commentary).  DEST: the
+// avifgpu_source_layout bits of the planes written (StoreTile; the alpha plane is shifted like the others).  The body of
+// EncodeRgbaF32FlatKernel (DEST 0) and of EncodeDestRgbaF32FlatKernel (the other layouts).
+template <int CURVE, int XS, int YS, int DEST>
+__device__ __forceinline__ void EncodeRgbaF32FlatBody(const FastEncodeParams& p)
 {
     extern __shared__ __align__(16) uint8_t sharedBytes[];
     uint64_t* libmStorage = reinterpret_cast<uint64_t*>(sharedBytes);
@@ -205,13 +207,15 @@ __global__ void __launch_bounds__(kRgbaThreads, 1) EncodeRgbaF32FlatKernel(const
         {
             const int64_t chromaRow = YS ? tileRow : y0;
             const int64_t chromaColumn = static_cast<int64_t>(XS ? (x0 >> 1) : x0) * 2;
-            StoreTile<XS, YS>(p, codeF, p.planeY + static_cast<int64_t>(y0) * p.strideY + static_cast<int64_t>(x0) * 2,
-                              p.planeCb + chromaRow * p.strideCb + chromaColumn, p.planeCr + chromaRow * p.strideCr + chromaColumn, secondRow);
+            StoreTile<XS, YS, DEST>(p, codeF, p.planeY + static_cast<int64_t>(y0) * p.strideY + static_cast<int64_t>(x0) * 2,
+                                    p.planeCb + chromaRow * p.strideCb + chromaColumn * (SourceInterleaved(DEST) ? 2 : 1),
+                                    p.planeCr + chromaRow * p.strideCr + chromaColumn, secondRow);
             uint8_t* alphaRow = p.planeA + static_cast<int64_t>(y0) * p.strideA + static_cast<int64_t>(x0) * 2;
-            __stcs(reinterpret_cast<uint2*>(alphaRow), make_uint2(alphaCode[0] | (alphaCode[1] << 16), alphaCode[2] | (alphaCode[3] << 16)));
+            __stcs(reinterpret_cast<uint2*>(alphaRow), make_uint2(MsbWord<DEST>(alphaCode[0] | (alphaCode[1] << 16), p), MsbWord<DEST>(alphaCode[2] | (alphaCode[3] << 16), p)));
             if (secondRow)
             {
-                __stcs(reinterpret_cast<uint2*>(alphaRow + p.strideA), make_uint2(alphaCode[4] | (alphaCode[5] << 16), alphaCode[6] | (alphaCode[7] << 16)));
+                __stcs(reinterpret_cast<uint2*>(alphaRow + p.strideA),
+                       make_uint2(MsbWord<DEST>(alphaCode[4] | (alphaCode[5] << 16), p), MsbWord<DEST>(alphaCode[6] | (alphaCode[7] << 16), p)));
             }
         }
         tileRow = nextRow;
@@ -220,12 +224,38 @@ __global__ void __launch_bounds__(kRgbaThreads, 1) EncodeRgbaF32FlatKernel(const
 }
 
 template <int CURVE, int XS, int YS>
+__global__ void __launch_bounds__(kRgbaThreads, 1) EncodeRgbaF32FlatKernel(const FastEncodeParams p)
+{
+    EncodeRgbaF32FlatBody<CURVE, XS, YS, AVIFGPU_SOURCE_PLANAR>(p);
+}
+
+// The same into semi-planar and MSB-aligned planes (DEST != 0).
+template <int CURVE, int XS, int YS, int DEST>
+__global__ void __launch_bounds__(kRgbaThreads, 1) EncodeDestRgbaF32FlatKernel(const FastEncodeParams p)
+{
+    EncodeRgbaF32FlatBody<CURVE, XS, YS, DEST>(p);
+}
+
+template <int CURVE, int XS, int YS, int DEST>
+constexpr auto RgbaKernelFor()
+{
+    if constexpr (DEST == AVIFGPU_SOURCE_PLANAR)
+    {
+        return EncodeRgbaF32FlatKernel<CURVE, XS, YS>;
+    }
+    else
+    {
+        return EncodeDestRgbaF32FlatKernel<CURVE, XS, YS, DEST>;
+    }
+}
+
+template <int CURVE, int XS, int YS, int DEST>
 cudaError_t LaunchRgbaKernel(const FastEncodeParams& fp, int smCount, cudaStream_t stream)
 {
     const size_t shared = static_cast<size_t>(RgbaFixedBytes()) + fp.table.compactImageBytes;
     static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
     {
-        const cudaError_t e = AllowDynamicShared(EncodeRgbaF32FlatKernel<CURVE, XS, YS>, kSharedLimit, configuredDevices);
+        const cudaError_t e = AllowDynamicShared(RgbaKernelFor<CURVE, XS, YS, DEST>(), kSharedLimit, configuredDevices);
         if (e != cudaSuccess)
         {
             return e;
@@ -241,7 +271,7 @@ cudaError_t LaunchRgbaKernel(const FastEncodeParams& fp, int smCount, cudaStream
     {
         blocks = smCount;
     }
-    EncodeRgbaF32FlatKernel<CURVE, XS, YS><<<static_cast<unsigned>(blocks), kRgbaThreads, shared, stream>>>(fp);
+    RgbaKernelFor<CURVE, XS, YS, DEST>()<<<static_cast<unsigned>(blocks), kRgbaThreads, shared, stream>>>(fp);
     return cudaGetLastError();
 }
 
@@ -254,11 +284,13 @@ bool RgbaEncodeApplies(const FastEncodeParams& fp)
            static_cast<size_t>(RgbaFixedBytes()) + fp.table.compactImageBytes <= static_cast<size_t>(kSharedLimit);
 }
 
-cudaError_t LaunchFastEncodeRgba(const FastEncodeParams& fp, int curve, int xs, int ys, int smCount, cudaStream_t stream)
+cudaError_t LaunchFastEncodeRgba(const FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream)
 {
     return WithChroma(xs, ys, [&](auto XS, auto YS) {
-        return curve == kCurveLinearToPQ ? LaunchRgbaKernel<kCurveLinearToPQ, XS(), YS()>(fp, smCount, stream)
-                                         : LaunchRgbaKernel<kCurveLinearToSMPTE428, XS(), YS()>(fp, smCount, stream);
+        return WithLayout(dest, [&](auto DEST) {
+            return curve == kCurveLinearToPQ ? LaunchRgbaKernel<kCurveLinearToPQ, XS(), YS(), DEST()>(fp, smCount, stream)
+                                             : LaunchRgbaKernel<kCurveLinearToSMPTE428, XS(), YS(), DEST()>(fp, smCount, stream);
+        });
     });
 }
 

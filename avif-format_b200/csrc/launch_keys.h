@@ -41,10 +41,10 @@ auto WithChroma(int xs, int ys, F&& f)
     return f(Int<0>{}, Int<0>{});
 }
 
-// f(SOURCE): the avifgpu_source_layout bits of a YCbCr decode -- interleaved chroma (1), MSB-aligned samples (2), both (3)
-// or libheif's planar, low-bit layout (0).
+// f(LAYOUT): avifgpu_source_layout bits -- the planes a YCbCr decode reads (SOURCE) or a planar encode writes (DEST):
+// interleaved chroma (1), MSB-aligned samples (2), both (3) or libheif's planar, low-bit layout (0).
 template <typename F>
-auto WithSource(int layout, F&& f)
+auto WithLayout(int layout, F&& f)
 {
     if (SourceInterleaved(layout) && SourceMsbAligned(layout)) return f(Int<AVIFGPU_SOURCE_CHROMA_INTERLEAVED | AVIFGPU_SOURCE_MSB_ALIGNED>{});
     if (SourceMsbAligned(layout)) return f(Int<AVIFGPU_SOURCE_MSB_ALIGNED>{});
@@ -70,15 +70,26 @@ auto WithHostDepth(int hostDepth, F&& f)
 }
 
 // Integer planar encode (EncodeRgbIntPlanarKernel, EncodeRgbIntBatchKernel).
-// f(HostT, PlaneT, CHANNELS, PREMULTIPLY, XS, YS): host depth x plane depth (16-bit planes above 8 bits) x channels /
-// premultiply (3, 4 straight, 4 premultiplied) x chroma.
+// f(HostT, PlaneT, CHANNELS, PREMULTIPLY, XS, YS, DEST): host depth x plane depth (16-bit planes above 8 bits) x channels /
+// premultiply (3, 4 straight, 4 premultiplied) x chroma x destination layout.  8-bit planes are never MSB-aligned
+// (ValidateEncodeDesc), so they take DEST 0 or 1 only.
 template <typename F>
 auto WithRgbIntKey(const EncodeParams& d, int hostDepth, F&& f)
 {
     return WithIntHost(hostDepth, [&](auto host) {
         const auto withPlane = [&](auto plane) {
             const auto withChannels = [&](auto channels, auto premultiply) {
-                return WithChroma(d.xs, d.ys, [&](auto xs, auto ys) { return f(host, plane, channels, premultiply, xs, ys); });
+                return WithChroma(d.xs, d.ys, [&](auto xs, auto ys) {
+                    const auto withDest = [&](auto dest) { return f(host, plane, channels, premultiply, xs, ys, dest); };
+                    if constexpr (sizeof(TypeOf<decltype(plane)>) == 1)
+                    {
+                        return WithFlag(SourceInterleaved(d.destLayout), withDest);
+                    }
+                    else
+                    {
+                        return WithLayout(d.destLayout, withDest);
+                    }
+                });
             };
             if (d.channels == 4 && d.premultiply) return withChannels(Int<4>{}, Int<1>{});
             if (d.channels == 4) return withChannels(Int<4>{}, Int<0>{});
@@ -112,7 +123,7 @@ auto WithYccIntKey(const DecodeParams& d, F&& f)
             }
             else
             {
-                return WithSource(d.sourceLayout, withSource);
+                return WithLayout(d.sourceLayout, withSource);
             }
         });
     });
@@ -127,7 +138,7 @@ auto WithYccF32Key(const DecodeParams& d, F&& f)
     const auto withTransfer = [&](auto transfer, auto fastDiv) {
         return WithFlag(d.hasAlpha != 0, [&](auto alpha) {
             return WithChroma(d.xs, d.ys, [&](auto xs, auto ys) {
-                return WithSource(d.sourceLayout, [&](auto source) { return f(transfer, fastDiv, alpha, xs, ys, source); });
+                return WithLayout(d.sourceLayout, [&](auto source) { return f(transfer, fastDiv, alpha, xs, ys, source); });
             });
         });
     };

@@ -8,7 +8,7 @@ import ctypes as C
 
 import numpy as np
 
-API_VERSION = 10
+API_VERSION = 11
 
 # avifgpu_status
 OK = 0
@@ -30,7 +30,7 @@ CHROMA_MONOCHROME, CHROMA_420, CHROMA_422, CHROMA_444 = 0, 1, 2, 3
 COLORSPACE_YCBCR, COLORSPACE_RGB, COLORSPACE_MONOCHROME = 0, 1, 2
 # avifgpu_layout
 LAYOUT_REFERENCE, LAYOUT_PLANAR_YCBCR = 0, 1
-# avifgpu_source_layout (bits of DecodeDesc.source_layout)
+# avifgpu_source_layout (bits of DecodeDesc.source_layout and EncodeDesc.dest_layout)
 SOURCE_PLANAR, SOURCE_CHROMA_INTERLEAVED, SOURCE_MSB_ALIGNED = 0, 1, 2
 # avifgpu_down_filter
 DOWN_FILTER_BOX, DOWN_FILTER_TOP_LEFT = 0, 1
@@ -101,12 +101,13 @@ class EncodeDesc(C.Structure):
         ("hlg_peak_nits", C.c_int32),
         ("row_matrix_enabled", C.c_int32),
         ("row_matrix", C.c_float * 9),
+        ("dest_layout", C.c_int32),
     ]
 
     def __init__(self, width, height, host_depth, host_channels, alpha_state=ALPHA_NONE, image_bit_depth=8,
                  transfer=TRANSFER_CLIP, pq_peak_nits=80, layout=LAYOUT_REFERENCE, chroma=CHROMA_444,
                  down_filter=DOWN_FILTER_BOX, gray16_curve=GRAY16_LUT, nclx=None, hlg_extension=0, hlg_display_gamma=1.2,
-                 hlg_peak_nits=1000):
+                 hlg_peak_nits=1000, *, dest_layout=SOURCE_PLANAR):
         super().__init__()
         self.struct_size = C.sizeof(EncodeDesc)
         self.width, self.height = width, height
@@ -123,6 +124,7 @@ class EncodeDesc(C.Structure):
         self.hlg_extension = hlg_extension
         self.hlg_display_gamma = hlg_display_gamma
         self.hlg_peak_nits = hlg_peak_nits
+        self.dest_layout = dest_layout
 
     def copy(self, **changes):
         out = EncodeDesc(self.width, self.height, self.host_depth, self.host_channels)
@@ -223,8 +225,11 @@ def encode_plane_shapes(desc):
         xs, ys = chroma_shifts(desc.chroma)
         cw, ch = (w + xs) >> xs, (h + ys) >> ys
         shapes[0] = (h, w)
-        shapes[1] = (ch, cw)
-        shapes[2] = (ch, cw)
+        if desc.dest_layout & SOURCE_CHROMA_INTERLEAVED:
+            shapes[1] = (ch, 2 * cw)  # Cb, Cr pairs; no plane 2
+        else:
+            shapes[1] = (ch, cw)
+            shapes[2] = (ch, cw)
         if has_alpha:
             shapes[3] = (h, w)
     return shapes

@@ -50,7 +50,7 @@ extern "C" {
 #define AVIFGPU_EXPORT __attribute__((visibility("default")))
 #endif
 
-#define AVIFGPU_API_VERSION 10
+#define AVIFGPU_API_VERSION 11
 
 typedef enum avifgpu_status
 {
@@ -137,7 +137,7 @@ typedef struct avifgpu_nclx
 
 /* A set of image planes.  stride in BYTES (libheif pads rows: heif_image_get_plane's out_stride).
  * Samples deeper than 8 bit are native-endian uint16 with the value in the low bits, unless a decode description's
- * source_layout says otherwise. */
+ * source_layout or an encode description's dest_layout says otherwise. */
 typedef struct avifgpu_planes
 {
     void* data[AVIFGPU_MAX_PLANES];
@@ -183,27 +183,50 @@ typedef struct avifgpu_encode_desc
      * avifgpu_icc_to_rec2020_linear_matrix() derives it from an ICC profile.  Parity unpinned (lcms2 is not in the tree). */
     int32_t row_matrix_enabled;
     float row_matrix[9];
+    /* Since API version 11: avifgpu_source_layout bits saying how the YCbCr planes are written (the table below).
+     * Non-zero only for AVIFGPU_LAYOUT_PLANAR_YCBCR (AVIFGPU_ERR_UNSUPPORTED otherwise); AVIFGPU_SOURCE_MSB_ALIGNED needs
+     * image_bit_depth 10 or 12 and unknown bits are AVIFGPU_ERR_BAD_PARAM.  Only the device-pointer calls write such
+     * planes (avifgpu_encode_rows_device, avifgpu_encode_batch_device, avifgpu_encode_batch_indirect); the host-pointer,
+     * asynchronous and sharded calls refuse a non-zero layout with AVIFGPU_ERR_UNSUPPORTED and launch nothing.  With
+     * AVIFGPU_SOURCE_CHROMA_INTERLEAVED planes.data[2] is ignored and never written; with AVIFGPU_SOURCE_MSB_ALIGNED every
+     * sample written, alpha included, is code << (16 - image_bit_depth) with the low bits zero.  A struct_size of
+     * AVIFGPU_ENCODE_DESC_V10_SIZE (a caller built against API version 10, which has no such field) is accepted and
+     * means AVIFGPU_SOURCE_PLANAR.
+     *   surface format           image_bit_depth  dest_layout
+     *   NV12 (4:2:0), NV16       8                AVIFGPU_SOURCE_CHROMA_INTERLEAVED
+     *   P010 (4:2:0), P210       10               AVIFGPU_SOURCE_CHROMA_INTERLEAVED | AVIFGPU_SOURCE_MSB_ALIGNED
+     *   P016 (4:2:0)             12               AVIFGPU_SOURCE_CHROMA_INTERLEAVED | AVIFGPU_SOURCE_MSB_ALIGNED
+     *   YUV444_16Bit             10 or 12         AVIFGPU_SOURCE_MSB_ALIGNED
+     * Every sample is, bit for bit, the planar, low-bit encode's code of the same description and rows, moved and
+     * shifted. */
+    int32_t dest_layout;
 } avifgpu_encode_desc;
+
+/* sizeof(avifgpu_encode_desc) up to API version 10: everything before dest_layout. */
+#define AVIFGPU_ENCODE_DESC_V10_SIZE ((uint32_t)offsetof(avifgpu_encode_desc, dest_layout))
 
 /* Parameter block of the decode direction = heif_image properties + nclx + LoadUIOptions
  * (AvifFormat.h:61-85). */
-/* How a YCbCr decode source sits in memory (avifgpu_decode_desc.source_layout), a bit set.  Hardware video decoders
- * (NVDEC through the Video Codec SDK or nvImageCodec, D3D12 and Vulkan video) write their frames this way:
+/* How YCbCr planes sit in memory, a bit set: the planes a decode reads (avifgpu_decode_desc.source_layout) and, since API
+ * version 11, the planes an encode writes (avifgpu_encode_desc.dest_layout).  Hardware video decoders (NVDEC through the
+ * Video Codec SDK or nvImageCodec, D3D12 and Vulkan video) write their frames this way, and hardware video encoders
+ * (NVENC, D3D12 and Vulkan video encode) and HDR swap chains read them:
  *   surface format         bit_depth  source_layout
  *   NV12 (4:2:0), NV16     8          AVIFGPU_SOURCE_CHROMA_INTERLEAVED
  *   P010 / P016 (4:2:0)    10 or 12   AVIFGPU_SOURCE_CHROMA_INTERLEAVED | AVIFGPU_SOURCE_MSB_ALIGNED
  *   YUV444 (8-bit planar)  8          AVIFGPU_SOURCE_PLANAR
  *   YUV444_16Bit           10 or 12   AVIFGPU_SOURCE_MSB_ALIGNED
- * Every output is, bit for bit, that of the same decode of the equivalent planar, low-bit source. */
+ * A decode's output is, bit for bit, that of the same decode of the equivalent planar, low-bit source; an encode's planes
+ * hold, bit for bit, the planar, low-bit encode's codes, moved and shifted. */
 typedef enum avifgpu_source_layout
 {
     /* libheif's (and dav1d's) layout: planes Y, Cb, Cr, Alpha; deeper codes in the low bits of a uint16.  The default. */
     AVIFGPU_SOURCE_PLANAR = 0,
     /* Cb and Cr interleaved in plane 1, Cb first (NV12 / NV16 / P010 / P016 / P210 order): a chroma row holds
-     * 2 * ((width + xs) >> xs) samples.  planes.data[2] is ignored; alpha stays plane 3. */
+     * 2 * ((width + xs) >> xs) samples.  planes.data[2] is ignored (neither read nor written); alpha stays plane 3. */
     AVIFGPU_SOURCE_CHROMA_INTERLEAVED = 1,
-    /* Every sample of every plane is a uint16 whose top bit_depth bits hold the code, code = sample >> (16 - bit_depth);
-     * the low bits are ignored, whatever they hold.  bit_depth 10 or 12 only. */
+    /* Every sample of every plane is a uint16 whose top bit_depth bits hold the code, code = sample >> (16 - bit_depth).
+     * A decode ignores the low bits, whatever they hold; an encode writes them zero.  Bit depth 10 or 12 only. */
     AVIFGPU_SOURCE_MSB_ALIGNED = 2
 } avifgpu_source_layout;
 
@@ -345,7 +368,8 @@ AVIFGPU_EXPORT int avifgpu_wait(avifgpu_context* ctx, int64_t ticket);
 /* Same contracts, but host_rows / planes are DEVICE pointers valid on the context's device and the work is
  * enqueued on `cuda_stream` (a cudaStream_t; NULL = the legacy default stream).  The decode call also reads the
  * semi-planar and MSB-aligned sources of avifgpu_decode_desc.source_layout, with any row block (an odd y0 of a 4:2:0
- * image included).
+ * image included); since API version 11 the encode call writes the semi-planar and MSB-aligned planes of
+ * avifgpu_encode_desc.dest_layout, with any row block the planar layout takes.
  *
  * CUDA graph capture.  Both calls may be recorded into a CUDA graph (cudaStreamBeginCapture ... cudaStreamEndCapture,
  * or torch.cuda.graph), in any capture mode, global included.  While `cuda_stream` is capturing a call:
@@ -402,8 +426,10 @@ typedef struct avifgpu_batch_image
  *     tables) is done once per call, outside a capture, for the batch's pixels.
  * Images the tuned integer planar kernel takes in a direct call (8/16-bit RGB(A) hosts into planar YCbCr, aligned
  * buffers, width >= 8) are converted in chunks of up to 64 images, at most two launches per chunk: one for every
- * image's aligned interior, one for every image's right strip and odd last 4:2:0 row.  Every other image takes one
- * direct call, after the chunks.
+ * image's aligned interior, one for every image's right strip and odd last 4:2:0 row.  Since API version 11 they also
+ * write the semi-planar and MSB-aligned planes of avifgpu_encode_desc.dest_layout, an interleaved chroma plane aligned to
+ * the paired stores (twice the planar chroma's alignment, at most 16 bytes).  Every other image takes one direct call,
+ * after the chunks.
  */
 AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
                                                const avifgpu_batch_image* images, int32_t count, void* cuda_stream);
@@ -438,7 +464,8 @@ AVIFGPU_EXPORT int avifgpu_batch_workspace_bytes(int32_t max_count, size_t* out_
  *   - Host checks, before any launch (each returns its status and launches nothing): ctx, desc, device_images,
  *     device_count or device_workspace NULL; desc invalid (validated as for the other calls, its size ignored);
  *     max_count outside [1, 4096]; workspace_bytes below avifgpu_batch_workspace_bytes(max_count).
- *   - Supported descriptions: encode, 8- or 16-bit RGB(A) hosts into planar YCbCr, any alpha state; decode, 8-, 16- or
+ *   - Supported descriptions: encode, 8- or 16-bit RGB(A) hosts into planar YCbCr, any alpha state (since API version 11
+ *     in any dest_layout); decode, 8-, 16- or
  *     (since API version 8) 32-bit hosts reading YCbCr, or (since API version 9) planar RGB, with no or straight alpha.
  *     Anything else -- monochrome, premultiplied alpha -- is AVIFGPU_ERR_UNSUPPORTED, with no launch.
  *   - Device-side checks.  With n = *device_count: n < 0 or n > max_count converts nothing and sets all max_count

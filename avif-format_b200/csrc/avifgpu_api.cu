@@ -45,42 +45,43 @@ static int TakeLaunchFailure()
 
 int LaunchEncode(const EncodeParams& params, int hostDepth, void* stream)
 {
-    int fast = LaunchEncodeFast(params, hostDepth, stream);
-    if (fast != 0)
+    const EncodeFamily family = EncodeFamilyOf(params, hostDepth);
+    const Interior inner = EncodeBlockInterior(family, params, hostDepth);
+    if (inner.width == 0)
     {
-        return fast;
+        return LaunchEncodeGeneric(params, hostDepth, stream);
     }
-    fast = LaunchEncodeFastInteger(params, hostDepth, stream);
-    if (fast != 0)
+    cudaError_t e;
+    switch (family)
     {
-        return fast;
+    case EncodeFamily::RgbF32Interleaved: e = LaunchEncodeRgbF32Interleaved(params, inner, stream); break;
+    case EncodeFamily::Gray16Lut: e = LaunchEncodeGray16Lut(params, inner, stream); break;
+    case EncodeFamily::GrayInt: e = LaunchEncodeGrayInt(params, hostDepth, inner, stream); break;
+    case EncodeFamily::RgbInt: e = LaunchEncodeRgbInt(params, hostDepth, inner, stream); break;
+    case EncodeFamily::GrayF32: e = LaunchEncodeGrayF32(params, inner, stream); break;
+    default: e = LaunchEncodeRgbF32Planar(family, params, inner, stream); break; // RgbF32Flat, RgbaF32Flat, RgbF32Clip
     }
-    fast = LaunchEncodeFastGray32(params, hostDepth, stream);
-    if (fast != 0)
-    {
-        return fast;
-    }
-    return LaunchEncodeGeneric(params, hostDepth, stream);
+    return CompleteEncode(e, params, hostDepth, inner.width, inner.rows, stream);
 }
 
 int LaunchDecode(const DecodeParams& params, void* stream)
 {
-    int fast = LaunchDecodeFast(params, stream);
-    if (fast != 0)
+    const DecodeFamily family = DecodeFamilyOf(params);
+    const Interior inner = DecodeBlockInterior(family, params);
+    if (inner.width == 0)
     {
-        return fast;
+        return LaunchDecodeGeneric(params, stream);
     }
-    fast = LaunchDecodeFastInteger(params, stream);
-    if (fast != 0)
+    cudaError_t e;
+    switch (family)
     {
-        return fast;
+    case DecodeFamily::YccF32: e = LaunchDecodeYccF32(params, inner, stream); break;
+    case DecodeFamily::YccInt: e = LaunchDecodeYccInt(params, inner, stream); break;
+    case DecodeFamily::MonoInt:
+    case DecodeFamily::PlanarRgbInt: e = LaunchDecodeStream(params, inner, stream); break;
+    default: e = LaunchDecodeTable(params, inner, stream); break; // MonoF32, PlanarRgbF32
     }
-    fast = LaunchDecodeFastTable(params, stream);
-    if (fast != 0)
-    {
-        return fast;
-    }
-    return LaunchDecodeGeneric(params, stream);
+    return CompleteDecode(e, params, inner.width, inner.rows, stream);
 }
 } // namespace avifgpu
 
@@ -1177,7 +1178,7 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_indirect(avifgpu_context* ctx, const avi
     }
     shared.smCount = ctx->smCount;
     ctx->FirstUseEncode(d, 0, capturing, &shared);
-    const int launched = LaunchEncodeIndirect(shared, d.host_depth, EncodeRgbIntTuned(shared, d.host_depth), planeMask, device_images, device_count,
+    const int launched = LaunchEncodeIndirect(shared, d.host_depth, EncodeBatchFamilyOf(shared, d.host_depth), planeMask, device_images, device_count,
                                               max_count, device_workspace, device_status, cuda_stream);
     if (launched < 0)
     {
@@ -1237,7 +1238,7 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_indirect(avifgpu_context* ctx, const avi
     }
     shared.smCount = ctx->smCount;
     ctx->FirstUseDecode(d, transfer, capturing, &shared);
-    const int launched = LaunchDecodeIndirect(shared, DecodeBatchTuned(shared), planeMask, device_images, device_count, max_count, device_workspace,
+    const int launched = LaunchDecodeIndirect(shared, DecodeBatchFamilyOf(shared), planeMask, device_images, device_count, max_count, device_workspace,
                                               device_status, cuda_stream);
     if (launched < 0)
     {

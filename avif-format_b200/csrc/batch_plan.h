@@ -131,11 +131,12 @@ AVIFGPU_HD inline int AdoptBatchImage(Params& p, int planeMask, const avifgpu_ba
     return AVIFGPU_OK;
 }
 
-// The per-image step of both plans.  `shared` is the description's block (FillEncodeParams), `tuned` EncodeRgbIntTuned of
-// it.  An image the tuned kernel takes in a direct call gets its interior and the strips CompleteEncode would hand to
-// the generic kernel; any other non-empty image becomes one whole-image window, which is what the generic kernel
-// converts in a direct call (the device-described batch runs that window; the host-described one makes the direct call).
-AVIFGPU_HD inline BatchImagePlan PlanBatchEncodeImage(const EncodeParams& shared, int hostDepth, bool tuned, int planeMask,
+// The per-image step of both plans.  `shared` is the description's block (FillEncodeParams), `family` the family its
+// interiors take (EncodeBatchFamilyOf: RgbInt or Generic).  An image the tuned kernel takes in a direct call gets its
+// interior and the strips CompleteEncode would hand to the generic kernel; any other non-empty image becomes one
+// whole-image window, which is what the generic kernel converts in a direct call (the device-described batch runs that
+// window; the host-described one makes the direct call).
+AVIFGPU_HD inline BatchImagePlan PlanBatchEncodeImage(const EncodeParams& shared, int hostDepth, EncodeFamily family, int planeMask,
                                                        const avifgpu_batch_image& image)
 {
     BatchImagePlan plan{};
@@ -145,7 +146,7 @@ AVIFGPU_HD inline BatchImagePlan PlanBatchEncodeImage(const EncodeParams& shared
     {
         return plan;
     }
-    const Interior inner = tuned ? EncodeRgbIntBlockInterior(p, hostDepth) : Interior{ 0, 0 };
+    const Interior inner = EncodeBlockInterior(family, p, hostDepth);
     if (inner.width == 0)
     {
         plan.window[0] = RecordOf(EncodeWindow(p, hostDepth, 0, 0, p.width, p.rowCount));
@@ -165,10 +166,9 @@ AVIFGPU_HD inline BatchImagePlan PlanBatchEncodeImage(const EncodeParams& shared
     return plan;
 }
 
-// The same for decodes (`tuned` = DecodeBatchTuned: for planar RGB the planar-RGB kernels' block half; for YCbCr the float
-// kernel's for 32-bit hosts and the integer kernel's otherwise; units of DecodeBatchUnitPixels); edge units are runs of
+// The same for decodes (`family` = DecodeBatchFamilyOf; interior units of DecodeBatchUnitPixels); edge units are runs of
 // pixels of one row.
-AVIFGPU_HD inline BatchImagePlan PlanBatchDecodeImage(const DecodeParams& shared, bool tuned, int planeMask, const avifgpu_batch_image& image)
+AVIFGPU_HD inline BatchImagePlan PlanBatchDecodeImage(const DecodeParams& shared, DecodeFamily family, int planeMask, const avifgpu_batch_image& image)
 {
     BatchImagePlan plan{};
     DecodeParams p = shared;
@@ -178,10 +178,7 @@ AVIFGPU_HD inline BatchImagePlan PlanBatchDecodeImage(const DecodeParams& shared
         return plan;
     }
     p.yPhase = 0;
-    const Interior inner = !tuned                                    ? Interior{ 0, 0 }
-                           : p.colorspace == AVIFGPU_COLORSPACE_RGB ? DecodePlanarRgbBlockInterior(p)
-                           : p.hostDepth == 32                      ? DecodeYccF32BlockInterior(p)
-                                                                    : DecodeYccIntBlockInterior(p);
+    const Interior inner = DecodeBlockInterior(family, p);
     if (inner.width == 0)
     {
         plan.window[0] = RecordOf(DecodeWindow(p, 0, 0, p.width, p.rowCount));
@@ -190,7 +187,7 @@ AVIFGPU_HD inline BatchImagePlan PlanBatchDecodeImage(const DecodeParams& shared
         return plan;
     }
     plan.interior = RecordOf(DecodeWindow(p, 0, 0, inner.width, inner.rows));
-    plan.interiorUnits = BatchInteriorUnits(inner.width, inner.rows, p.ys, DecodeBatchUnitPixels(p.hostDepth, p.colorspace));
+    plan.interiorUnits = BatchInteriorUnits(inner.width, inner.rows, p.ys, DecodeBatchUnitPixels(family));
     Strip strip[2];
     plan.windows = InteriorStrips(p.width, p.rowCount, inner, strip);
     for (int k = 0; k < plan.windows; ++k)
@@ -208,11 +205,11 @@ void PlanEncodeBatch(const EncodeParams& shared, int hostDepth, int planeMask, c
 void PlanDecodeBatch(const DecodeParams& shared, int planeMask, const avifgpu_batch_image* images, int32_t count, BatchPlan* plan);
 
 // The launchers (kernels_batch.cu): the plan, interior and edge kernels of one call on `stream`.  `shared` is the
-// description's block with the context's first-use state; `tuned` its description half of the routing.  Return 3 (the
-// launches) or a negative status.
-int LaunchEncodeIndirect(const EncodeParams& shared, int hostDepth, bool tuned, int planeMask, const avifgpu_batch_image* images,
+// description's block with the context's first-use state; `family` the family its interiors take (EncodeBatchFamilyOf /
+// DecodeBatchFamilyOf).  Return 3 (the launches) or a negative status.
+int LaunchEncodeIndirect(const EncodeParams& shared, int hostDepth, EncodeFamily family, int planeMask, const avifgpu_batch_image* images,
                          const int32_t* count, int maxCount, void* workspace, int32_t* status, void* stream);
-int LaunchDecodeIndirect(const DecodeParams& shared, bool tuned, int planeMask, const avifgpu_batch_image* images, const int32_t* count,
+int LaunchDecodeIndirect(const DecodeParams& shared, DecodeFamily family, int planeMask, const avifgpu_batch_image* images, const int32_t* count,
                          int maxCount, void* workspace, int32_t* status, void* stream);
 
 } // namespace avifgpu

@@ -7,6 +7,7 @@
 #ifndef AVIF_KERNEL_PARAMS_H
 #define AVIF_KERNEL_PARAMS_H
 
+#include <stddef.h>
 #include <stdint.h>
 
 #include <atomic>
@@ -227,21 +228,86 @@ inline unsigned GridFor(long long blocks, long long cap)
     return static_cast<unsigned>(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
-// The aligned interior [0, width) x [0, rows) the tuned integer planar encode kernel (EncodeRgbIntPlanarKernel)
-// converts for this block, or {0, 0} when a direct call of the block takes another route: 8/16-bit RGB(A) hosts into
-// planar YCbCr of at most 12 bits, no alpha, straight alpha or a verified premultiply, a matrix the biased truncation
-// handles, 8-pixel-aligned buffers and at least 8 x (1 << ys) pixels.  width is a multiple of 8, rows of 1 << ys.
 struct Interior
 {
     int32_t width;
     int32_t rows;
 };
-// EncodeRgbIntInterior in two halves: the description's (host depth, layout, channels, premultiply, depth, matrix --
-// the same for every block of one description, host only) and the block's (buffer alignment, at least 8 pixels and one
-// 4:2:0 row pair).  Interleaved chroma is one plane of Cb, Cr pairs a thread writes in one store of twice the planar
-// chroma's bytes (two 128-bit stores for 16-bit 4:4:4), so it is aligned to that store, at most 16 bytes; the
-// destination layout is the block's business only, so the description's half does not read it.
-bool EncodeRgbIntTuned(const EncodeParams& p, int hostDepth);
+
+// ---- routing: which tuned kernel family converts a direct call's block, and on which aligned interior -----------------
+//
+// A route has two halves.  The description's (EncodeFamilyOf / DecodeFamilyOf, host_params.cpp; host only, once per call)
+// names the one tuned family whose conditions the description and the context's first-use state meet (step table, Gray16
+// LUT, verified shortcuts), or generic.  The block's (EncodeBlockInterior / DecodeBlockInterior; also run by the batch plan
+// kernel) gives the interior [0, width) x [0, rows) that family's kernel converts for this block: buffer alignment, enough
+// pixels, a 4:2:0 block starting on a row pair.  An empty interior (width 0) leaves the whole block to the generic kernel;
+// no other tuned family is tried.  LaunchEncode / LaunchDecode launch the family's kernel on the interior and hand the
+// strips around it to the generic kernel (CompleteEncode / CompleteDecode).
+enum class EncodeFamily : int32_t
+{
+    Generic,
+    RgbF32Interleaved, // RGB32f in the reference's interleaved layout through a step table (EncodeRgbF32FlatKernel, INTERLEAVED = 1)
+    RgbF32Flat,        // RGB32f -> planar YCbCr through a step table (EncodeRgbF32FlatKernel)
+    RgbaF32Flat,       // RGBA32f -> planar YCbCr + alpha through the compact table (EncodeRgbaF32FlatKernel)
+    RgbF32Clip,        // RGB32f -> planar YCbCr with no transfer curve (EncodeRgbF32ClipKernel)
+    Gray16Lut,         // Gray16 -> 10/12-bit Y through the context's code table (EncodeGray16LutKernel)
+    GrayInt,           // Gray(+A) 8/16-bit -> Y (+A) (EncodeGrayIntKernel)
+    RgbInt,            // RGB(A) 8/16-bit -> planar YCbCr (EncodeRgbIntPlanarKernel; batched)
+    GrayF32,           // Gray(+A)32f -> Y (+A), PQ through the compact table or clip (EncodeGrayF32Kernel)
+};
+
+enum class DecodeFamily : int32_t
+{
+    Generic,
+    YccF32,       // 10/12-bit YCbCr -> 32-bit hosts (DecodeYccToRgbF32Kernel; batched)
+    YccInt,       // YCbCr -> 8/16-bit hosts (DecodeYccToRgbIntKernel; batched)
+    MonoInt,      // monochrome -> 8/16-bit hosts (StreamDecodeKernel)
+    PlanarRgbInt, // planar RGB -> 8/16-bit hosts (StreamDecodeKernel; batched)
+    MonoF32,      // 10/12-bit monochrome PQ -> 32-bit hosts (TableDecodeF32Kernel)
+    PlanarRgbF32, // 10/12-bit planar RGB -> 32-bit hosts (TableDecodeF32Kernel; batched without premultiplied alpha)
+};
+
+EncodeFamily EncodeFamilyOf(const EncodeParams& p, int hostDepth);
+DecodeFamily DecodeFamilyOf(const DecodeParams& p);
+
+// Shared-memory layouts of the tuned float encode kernels: what the kernels carve their dynamic shared memory into, and
+// what the description's half checks a step table against.  kSharedLimit is the opt-in maximum per CTA on sm_90.
+constexpr int kSharedLimit = 227 * 1024;
+constexpr int kSharedLibm = 768; // avifmath::StageLibmTables' 96 words, first in every float encode kernel's shared memory
+// EncodeRgbF32FlatKernel: libm tables, the warps' barriers (the last slot the table's), a two-row staging buffer per
+// warp, then the step table (compact entries + first_k, or 256 octave entries + the bucket words).
+constexpr int kFlatWarps = 28;
+constexpr int kFlatSharedBarriers = 256;
+constexpr int kFlatStageBytesPerWarp = 2 * 128 * 12; // both rows of a 128-pixel RGB32f tile
+constexpr int kFlatOctaveBytes = 256 * 8;
+AVIFGPU_HD constexpr int FlatFixedBytes() { return kSharedLibm + kFlatSharedBarriers + kFlatWarps * kFlatStageBytesPerWarp; }
+inline size_t FlatTableBytes(const CurveTableView& t, bool twoLevel)
+{
+    return twoLevel ? kFlatOctaveBytes + static_cast<size_t>(t.bucketCount) * sizeof(uint32_t) : t.compactImageBytes;
+}
+inline bool FlatCompactFits(const CurveTableView& t)
+{
+    return t.compact != nullptr && t.firstBits != nullptr && t.bandBits != nullptr &&
+           static_cast<size_t>(FlatFixedBytes()) + FlatTableBytes(t, false) <= static_cast<size_t>(kSharedLimit);
+}
+inline bool FlatTwoLevelFits(const CurveTableView& t)
+{
+    return t.buckets != nullptr && t.octaves != nullptr && static_cast<size_t>(FlatFixedBytes()) + FlatTableBytes(t, true) <= static_cast<size_t>(kSharedLimit);
+}
+// EncodeRgbaF32FlatKernel: libm tables, the table's barrier (padded), 28 words per lane of staged colour samples, the table.
+constexpr int kRgbaWarps = 16;
+constexpr int kRgbaTableBarrierBytes = 16;
+constexpr int kRgbaLaneStrideWords = 28; // 24 colour samples + padding: 16-byte aligned, conflict-free for STS.128
+constexpr int kRgbaStagePerWarp = 32 * kRgbaLaneStrideWords * 4;
+AVIFGPU_HD constexpr int RgbaFixedBytes() { return kSharedLibm + kRgbaTableBarrierBytes + kRgbaWarps * kRgbaStagePerWarp; }
+// EncodeGrayF32Kernel: libm tables, the table's barrier (padded), the compact table (PQ only), within 100 KiB.
+constexpr int kGrayF32FixedBytes = kSharedLibm + 16;
+constexpr int kGrayF32SharedLimit = 100 * 1024;
+
+// The block halves.  8/16-bit RGB(A) hosts into planar YCbCr (EncodeRgbIntPlanarKernel): 8-pixel-aligned buffers and at
+// least 8 x (1 << ys) pixels; width a multiple of 8, rows of 1 << ys.  Interleaved chroma is one plane of Cb, Cr pairs a
+// thread writes in one store of twice the planar chroma's bytes (two 128-bit stores for 16-bit 4:4:4), so it is aligned to
+// that store, at most 16 bytes.
 AVIFGPU_HD inline Interior EncodeRgbIntBlockInterior(const EncodeParams& p, int hostDepth)
 {
     const Interior none = { 0, 0 };
@@ -265,13 +331,11 @@ AVIFGPU_HD inline Interior EncodeRgbIntBlockInterior(const EncodeParams& p, int 
     }
     return Interior{ p.width & ~7, evenRows };
 }
-Interior EncodeRgbIntInterior(const EncodeParams& p, int hostDepth); // EncodeRgbIntTuned ? EncodeRgbIntBlockInterior : none
 
-// The block's half of the tuned float planar encodes (EncodeRgbF32FlatKernel, EncodeRgbaF32FlatKernel,
-// EncodeRgbF32ClipKernel; LaunchEncodeFast has the description's): 10/12-bit planes, a lane on 4 pixels of each of 2 rows,
-// 128-bit row loads, 64-bit luma and alpha stores, 32-bit (4:2:0, 4:2:2) or 64-bit (4:4:4) planar chroma stores -- or,
-// into interleaved chroma, one store of twice those bytes -- and at least 4 x (1 << ys) pixels.  width is a multiple of
-// 4, rows of 1 << ys.
+// The tuned float planar encodes (RgbF32Flat, RgbaF32Flat, RgbF32Clip): 10/12-bit planes, a lane on 4 pixels of each of 2
+// rows, 128-bit row loads, 64-bit luma and alpha stores, 32-bit (4:2:0, 4:2:2) or 64-bit (4:4:4) planar chroma stores --
+// or, into interleaved chroma, one store of twice those bytes -- and at least 4 x (1 << ys) pixels.  width is a multiple
+// of 4, rows of 1 << ys.
 AVIFGPU_HD inline Interior EncodeRgbF32BlockInterior(const EncodeParams& p)
 {
     const Interior none = { 0, 0 };
@@ -293,11 +357,64 @@ AVIFGPU_HD inline Interior EncodeRgbF32BlockInterior(const EncodeParams& p)
     return Interior{ width4, evenRows };
 }
 
-// The same for the tuned integer YCbCr decode kernel (DecodeYccToRgbIntKernel): 8/16-bit hosts reading 8-bit / 10-12-bit
-// YCbCr (+ straight alpha), a block starting on a 4:2:0 row pair, aligned buffers, at least 8 x (1 << ys) pixels.
-// Interleaved chroma is one plane of Cb, Cr pairs a lane reads in one load of twice the planar chroma's bytes (two 128-bit
-// loads for 16-bit 4:4:4), so it is aligned to that load, at most 16 bytes.
-bool DecodeYccIntTuned(const DecodeParams& p);
+// The float kernels that read `rows` with 128-bit loads and write one or two 16-bit planes with 64-bit stores, 4 pixels
+// a thread, no sub-sampling: the interleaved RGB32f encode (plane 0 only) and the gray float one (plane 3 too, with alpha).
+AVIFGPU_HD inline Interior EncodeFourPixelInterior(const EncodeParams& p, bool alphaPlane)
+{
+    const Interior none = { 0, 0 };
+    const int width4 = p.width & ~3;
+    if (width4 < 4 || p.rowCount < 1 || !Aligned(p.rows, p.rowStride, 16) || !Aligned(p.plane[0], p.planeStride[0], 8) ||
+        (alphaPlane && !Aligned(p.plane[3], p.planeStride[3], 8)))
+    {
+        return none;
+    }
+    return Interior{ width4, p.rowCount };
+}
+
+// Gray16 through the code table: a thread looks up 8 samples of one 128-bit load and stores them with one 128-bit store.
+AVIFGPU_HD inline Interior EncodeGray16LutBlockInterior(const EncodeParams& p)
+{
+    const Interior none = { 0, 0 };
+    if (p.width < 8 || !Aligned(p.rows, p.rowStride, 16) || !Aligned(p.plane[0], p.planeStride[0], 16))
+    {
+        return none;
+    }
+    return Interior{ p.width & ~7, p.rowCount };
+}
+
+// Gray(+A) 8/16-bit hosts: a thread's 8 pixels, 64- or 128-bit row loads, 8-sample plane stores.
+AVIFGPU_HD inline Interior EncodeGrayIntBlockInterior(const EncodeParams& p, int hostDepth)
+{
+    const Interior none = { 0, 0 };
+    const int planeBytes = p.imageDepth > 8 ? 2 : 1;
+    const int rowAlign = (8 * p.channels * (hostDepth / 8)) % 16 == 0 ? 16 : 8;
+    if (p.width < 8 || p.rowCount < 1 || !Aligned(p.rows, p.rowStride, rowAlign) || !Aligned(p.plane[0], p.planeStride[0], 8 * planeBytes) ||
+        (p.channels == 2 && !Aligned(p.plane[3], p.planeStride[3], 8 * planeBytes)))
+    {
+        return none;
+    }
+    return Interior{ p.width & ~7, p.rowCount };
+}
+
+AVIFGPU_HD inline Interior EncodeBlockInterior(EncodeFamily family, const EncodeParams& p, int hostDepth)
+{
+    switch (family)
+    {
+    case EncodeFamily::RgbF32Interleaved: return EncodeFourPixelInterior(p, false);
+    case EncodeFamily::RgbF32Flat:
+    case EncodeFamily::RgbF32Clip: return EncodeRgbF32BlockInterior(p);
+    case EncodeFamily::RgbaF32Flat: return p.plane[3] != nullptr ? EncodeRgbF32BlockInterior(p) : Interior{ 0, 0 };
+    case EncodeFamily::Gray16Lut: return EncodeGray16LutBlockInterior(p);
+    case EncodeFamily::GrayInt: return EncodeGrayIntBlockInterior(p, hostDepth);
+    case EncodeFamily::RgbInt: return EncodeRgbIntBlockInterior(p, hostDepth);
+    case EncodeFamily::GrayF32: return EncodeFourPixelInterior(p, p.channels == 2);
+    default: return Interior{ 0, 0 };
+    }
+}
+
+// The integer YCbCr decode (DecodeYccToRgbIntKernel): 8/16-bit hosts, a block starting on a 4:2:0 row pair, aligned
+// buffers, at least 8 x (1 << ys) pixels.  Interleaved chroma is one plane of Cb, Cr pairs a lane reads in one load of
+// twice the planar chroma's bytes (two 128-bit loads for 16-bit 4:4:4), so it is aligned to that load, at most 16 bytes.
 AVIFGPU_HD inline Interior DecodeYccIntBlockInterior(const DecodeParams& p)
 {
     const Interior none = { 0, 0 };
@@ -309,8 +426,8 @@ AVIFGPU_HD inline Interior DecodeYccIntBlockInterior(const DecodeParams& p)
     const bool interleaved = SourceInterleaved(p.sourceLayout);
     const bool chromaAligned = interleaved ? Aligned(p.plane[1], p.planeStride[1], 2 * chromaAlign > 16 ? 16 : 2 * chromaAlign)
                                            : Aligned(p.plane[1], p.planeStride[1], chromaAlign) && Aligned(p.plane[2], p.planeStride[2], chromaAlign);
-    if (!Aligned(p.plane[0], p.planeStride[0], lumaAlign) || !chromaAligned || (p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], lumaAlign)) ||
-        !Aligned(p.rows, p.rowStride, rowAlign))
+    if (p.yPhase != 0 || !Aligned(p.plane[0], p.planeStride[0], lumaAlign) || !chromaAligned ||
+        (p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], lumaAlign)) || !Aligned(p.rows, p.rowStride, rowAlign))
     {
         return none;
     }
@@ -322,15 +439,10 @@ AVIFGPU_HD inline Interior DecodeYccIntBlockInterior(const DecodeParams& p)
     }
     return Interior{ width8, evenRows };
 }
-Interior DecodeYccIntInterior(const DecodeParams& p); // DecodeYccIntTuned ? DecodeYccIntBlockInterior : none
 
-// The same for the tuned float YCbCr decode kernel (DecodeYccToRgbF32Kernel), split the same way.  The description's half:
-// 10/12-bit YCbCr (+ straight alpha) into 32-bit hosts with the PQ, HLG or SMPTE 428 curve; for HLG the context's verified
-// divisions, and with the OOTF an exponent and luma coefficients the branch-free powf covers; for PQ and SMPTE 428 a matrix
-// whose channel sums are never subnormal.  The block's half: a block starting on a 4:2:0 row pair, aligned buffers, equal
-// Cb and Cr strides, at least 4 x (1 << ys) pixels.  width is a multiple of 4, rows of 1 << ys.  Interleaved chroma is one
-// plane of Cb, Cr pairs read in one load of twice the planar chroma's bytes, aligned to it.
-bool DecodeYccF32Tuned(const DecodeParams& p);
+// The float YCbCr decode (DecodeYccToRgbF32Kernel): a block starting on a 4:2:0 row pair, aligned buffers, equal Cb and Cr
+// strides, at least 4 x (1 << ys) pixels.  width is a multiple of 4, rows of 1 << ys.  Interleaved chroma is one plane of
+// Cb, Cr pairs read in one load of twice the planar chroma's bytes, aligned to it.
 AVIFGPU_HD inline Interior DecodeYccF32BlockInterior(const DecodeParams& p)
 {
     const Interior none = { 0, 0 };
@@ -355,14 +467,10 @@ AVIFGPU_HD inline Interior DecodeYccF32BlockInterior(const DecodeParams& p)
     }
     return Interior{ width4, evenRows };
 }
-Interior DecodeYccF32Interior(const DecodeParams& p); // DecodeYccF32Tuned ? DecodeYccF32BlockInterior : none
 
-// The same for the tuned planar-RGB decode kernels (StreamDecodeKernel for 8/16-bit hosts, TableDecodeF32Kernel for 32-bit
-// hosts), split the same way.  The description's half: colour space RGB with no or straight alpha; for 8/16-bit hosts at
-// most 12 bits, 8-bit planes into 8-bit hosts and 10/12-bit planes into 16-bit hosts; for 32-bit hosts 10/12-bit planes
-// with the PQ, HLG or SMPTE 428 curve.  The block's half: planes aligned to a thread's 8 samples, rows to its stores, at
-// least 8 pixels and one row.  width is a multiple of 8 and rows is the block's: the interior only ever leaves a right strip.
-bool DecodePlanarRgbTuned(const DecodeParams& p);
+// The planar-RGB decodes (StreamDecodeKernel for 8/16-bit hosts, TableDecodeF32Kernel for 32-bit hosts): planes aligned to
+// a thread's 8 samples, rows to its stores, at least 8 pixels and one row.  width is a multiple of 8 and rows is the
+// block's: the interior only ever leaves a right strip.
 AVIFGPU_HD inline Interior DecodePlanarRgbBlockInterior(const DecodeParams& p)
 {
     const Interior none = { 0, 0 };
@@ -387,11 +495,58 @@ AVIFGPU_HD inline Interior DecodePlanarRgbBlockInterior(const DecodeParams& p)
     }
     return Interior{ width8, p.rowCount };
 }
-Interior DecodePlanarRgbInterior(const DecodeParams& p); // DecodePlanarRgbTuned ? DecodePlanarRgbBlockInterior : none
 
-// The description half of whichever tuned decode kernel serves the description: the planar-RGB one for colour space RGB,
-// otherwise the float YCbCr one for 32-bit hosts and the integer one for the others.  Both batch APIs route by it.
-bool DecodeBatchTuned(const DecodeParams& p);
+// The monochrome decodes: a thread's 8 samples of plane 0 (and 3), one or two host stores.  Integer hosts align the
+// planes to 8 samples and the rows to the group's stores; float hosts both to 16 bytes.
+AVIFGPU_HD inline Interior DecodeMonoBlockInterior(const DecodeParams& p)
+{
+    const Interior none = { 0, 0 };
+    const bool f32 = p.hostDepth == 32;
+    const int sampleBytes = p.hostDepth == 8 ? 1 : 2;
+    const int planeAlign = f32 ? 16 : 8 * sampleBytes;
+    const int rowAlign = f32 || (8 * (p.hasAlpha ? 2 : 1) * sampleBytes) % 16 == 0 ? 16 : 8;
+    if (!Aligned(p.plane[0], p.planeStride[0], planeAlign) || (p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], planeAlign)) ||
+        !Aligned(p.rows, p.rowStride, rowAlign))
+    {
+        return none;
+    }
+    const int width8 = p.width & ~7;
+    if (width8 < 8 || p.rowCount < 1)
+    {
+        return none;
+    }
+    return Interior{ width8, p.rowCount };
+}
+
+AVIFGPU_HD inline Interior DecodeBlockInterior(DecodeFamily family, const DecodeParams& p)
+{
+    switch (family)
+    {
+    case DecodeFamily::YccF32: return DecodeYccF32BlockInterior(p);
+    case DecodeFamily::YccInt: return DecodeYccIntBlockInterior(p);
+    case DecodeFamily::MonoInt:
+    case DecodeFamily::MonoF32: return DecodeMonoBlockInterior(p);
+    case DecodeFamily::PlanarRgbInt:
+    case DecodeFamily::PlanarRgbF32: return DecodePlanarRgbBlockInterior(p);
+    default: return Interior{ 0, 0 };
+    }
+}
+
+// The family a batch of images of this description runs its interiors on: integer RGB(A) into planar YCbCr for encodes;
+// generic otherwise.
+inline EncodeFamily EncodeBatchFamilyOf(const EncodeParams& p, int hostDepth)
+{
+    return EncodeFamilyOf(p, hostDepth) == EncodeFamily::RgbInt ? EncodeFamily::RgbInt : EncodeFamily::Generic;
+}
+// For decodes: YCbCr and planar RGB into every host depth,
+// except premultiplied alpha, which only the single-image table kernel un-premultiplies; generic otherwise.
+inline DecodeFamily DecodeBatchFamilyOf(const DecodeParams& p)
+{
+    const DecodeFamily family = DecodeFamilyOf(p);
+    const bool batched = family == DecodeFamily::YccF32 || family == DecodeFamily::YccInt || family == DecodeFamily::PlanarRgbInt ||
+                         family == DecodeFamily::PlanarRgbF32;
+    return batched && !(p.hasAlpha && p.premultiplied) ? family : DecodeFamily::Generic;
+}
 
 // The pixel-independent factors of the float decode's channel sums, YuvDecode.cpp:555-557 and :308 -- the reference's
 // float expressions, evaluated once on the host without contraction (host_params.cpp).
@@ -448,11 +603,10 @@ AVIFGPU_HD inline int64_t BatchInteriorUnits(int width, int rows, int ys, int un
 {
     return static_cast<int64_t>((width + unitPixels - 1) / unitPixels) * ((rows + ys) >> ys);
 }
-// The interior unit width of a decode of `colorspace` into `hostDepth`-bit hosts: 128 pixels for YCbCr into 32-bit hosts,
-// 256 for everything else (planar RGB into every host depth).
-AVIFGPU_HD inline int DecodeBatchUnitPixels(int hostDepth, int colorspace)
+// The interior unit width of a batched decode family: 128 pixels for the float YCbCr one, 256 for the others.
+AVIFGPU_HD inline int DecodeBatchUnitPixels(DecodeFamily family)
 {
-    return hostDepth == 32 && colorspace != AVIFGPU_COLORSPACE_RGB ? kF32BatchUnitPixels : kBatchUnitPixels;
+    return family == DecodeFamily::YccF32 ? kF32BatchUnitPixels : kBatchUnitPixels;
 }
 AVIFGPU_HD inline int64_t BatchEdgeUnits(int width, int rows, int xs, int ys)
 {
@@ -504,26 +658,33 @@ inline int BatchChunkLaunches(const BatchChunk& chunk) { return 1 + (chunk.windo
 // of asking CUDA a second time (which would answer cudaSuccess and turn a failed launch into AVIFGPU_OK).
 int ReportLaunchFailure(int cudaErrorCode);
 
-// Launchers implemented in kernels_*.cu.  They only enqueue work on `stream` and return the number of kernels
-// launched (>= 1) or a negative avifgpu_status; the tuned ones (LaunchEncodeFast*, LaunchDecodeFast*) return 0 for a
-// configuration they do not cover.
+// LaunchEncode / LaunchDecode (avifgpu_api.cu) route a direct call (EncodeFamilyOf / DecodeFamilyOf, then the block half),
+// launch the family's kernel on the interior and complete the block.  They only enqueue work on `stream` and return the
+// number of kernels launched (>= 1; 0 for an empty block) or a negative avifgpu_status.
 int LaunchEncode(const EncodeParams& params, int hostDepth, void* stream);
 int LaunchDecode(const DecodeParams& params, void* stream);
 int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* stream);
 int LaunchDecodeGeneric(const DecodeParams& params, void* stream);
-int LaunchEncodeFast(const EncodeParams& params, int hostDepth, void* stream);
-int LaunchEncodeFastInteger(const EncodeParams& params, int hostDepth, void* stream);
-int LaunchEncodeFastGray32(const EncodeParams& params, int hostDepth, void* stream);
-int LaunchDecodeFast(const DecodeParams& params, void* stream);
-int LaunchDecodeFastInteger(const DecodeParams& params, void* stream);
-int LaunchDecodeFastTable(const DecodeParams& params, void* stream);
 int LaunchTransfer(int function, float param, const float* in, float* out, size_t count, void* stream);
 int LaunchHlgOotf(int inverse, const float luma[3], float displayGamma, float peak, const float* in, float* out, size_t pixels, void* stream);
 
-// The end of every tuned launch site.  A tuned kernel converts the block's aligned interior [0, coveredWidth) x
-// [0, coveredRows); `tuned` is its launch status.  On success the generic kernel converts the right strip
-// [coveredWidth, width) x [0, rowCount), then the bottom strip [0, coveredWidth) x [coveredRows, rowCount); an empty
-// strip launches nothing.  Returns 1 + the strip launches, or a negative status.
+// The tuned launchers (kernels_fast*.cu): each fills its kernel's parameters for the interior `inner` of the block `p`
+// that the route gave its family, enqueues the kernel and returns the launch's status.
+cudaError_t LaunchEncodeRgbF32Interleaved(const EncodeParams& p, Interior inner, void* stream);
+cudaError_t LaunchEncodeRgbF32Planar(EncodeFamily family, const EncodeParams& p, Interior inner, void* stream); // RgbF32Flat, RgbaF32Flat, RgbF32Clip
+cudaError_t LaunchEncodeGray16Lut(const EncodeParams& p, Interior inner, void* stream);
+cudaError_t LaunchEncodeGrayInt(const EncodeParams& p, int hostDepth, Interior inner, void* stream);
+cudaError_t LaunchEncodeRgbInt(const EncodeParams& p, int hostDepth, Interior inner, void* stream);
+cudaError_t LaunchEncodeGrayF32(const EncodeParams& p, Interior inner, void* stream);
+cudaError_t LaunchDecodeYccF32(const DecodeParams& p, Interior inner, void* stream);
+cudaError_t LaunchDecodeYccInt(const DecodeParams& p, Interior inner, void* stream);
+cudaError_t LaunchDecodeStream(const DecodeParams& p, Interior inner, void* stream); // MonoInt, PlanarRgbInt
+cudaError_t LaunchDecodeTable(const DecodeParams& p, Interior inner, void* stream);  // MonoF32, PlanarRgbF32
+
+// The end of every tuned launch.  The tuned kernel converts the block's interior [0, coveredWidth) x [0, coveredRows);
+// `tuned` is its launch status.  On success the generic kernel converts the right strip [coveredWidth, width) x
+// [0, rowCount), then the bottom strip [0, coveredWidth) x [coveredRows, rowCount); an empty strip launches nothing.
+// Returns 1 + the strip launches, or a negative status.
 int CompleteEncode(cudaError_t tuned, const EncodeParams& p, int hostDepth, int coveredWidth, int coveredRows, void* stream);
 int CompleteDecode(cudaError_t tuned, const DecodeParams& p, int coveredWidth, int coveredRows, void* stream);
 

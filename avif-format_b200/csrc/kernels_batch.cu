@@ -202,22 +202,22 @@ struct EncodePlanner
 {
     EncodeParams shared;
     int32_t hostDepth;
-    int32_t tuned;
+    EncodeFamily family;
     int32_t planeMask;
     __device__ __forceinline__ BatchImagePlan operator()(const avifgpu_batch_image& image) const
     {
-        return PlanBatchEncodeImage(shared, hostDepth, tuned != 0, planeMask, image);
+        return PlanBatchEncodeImage(shared, hostDepth, family, planeMask, image);
     }
 };
 
 struct DecodePlanner
 {
     DecodeParams shared;
-    int32_t tuned;
+    DecodeFamily family;
     int32_t planeMask;
     __device__ __forceinline__ BatchImagePlan operator()(const avifgpu_batch_image& image) const
     {
-        return PlanBatchDecodeImage(shared, tuned != 0, planeMask, image);
+        return PlanBatchDecodeImage(shared, family, planeMask, image);
     }
 };
 
@@ -767,25 +767,24 @@ int LaunchDecodeBatchChunk(const DecodeParams& shared, const BatchChunk& chunk, 
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
     const int smCount = SmCountOrDefault(shared.smCount);
     const long long warps = (chunk.interiorUnits + kWarps - 1) / kWarps; // one warp per unit
-    if (shared.colorspace == AVIFGPU_COLORSPACE_RGB && shared.hostDepth == 32)
+    switch (DecodeBatchFamilyOf(shared)) // a chunk has interiors: a batched family
     {
+    case DecodeFamily::PlanarRgbF32:
         LaunchPlanarRgbF32(ChunkOf<PlanarRgbF32Chunk>(TableDecodeDescription(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared, warps,
                            smCount, CodeTableBytes(shared.bitDepth, shared.hasAlpha != 0), stream);
-    }
-    else if (shared.colorspace == AVIFGPU_COLORSPACE_RGB)
-    {
+        break;
+    case DecodeFamily::PlanarRgbInt:
         LaunchPlanarRgbInt(ChunkOf<PlanarRgbIntChunk>(StreamDecodeDescription(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared, warps,
                            smCount, stream);
-    }
-    else if (shared.hostDepth == 32)
-    {
+        break;
+    case DecodeFamily::YccF32:
         LaunchYccF32(ChunkOf<YccF32Chunk>(FillF32Description(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared,
                      GridFor(warps, static_cast<long long>(smCount) * kDecodeBlocksPerSm), F32TableBytesOf(shared), stream);
-    }
-    else
-    {
+        break;
+    default:
         LaunchYccInt(ChunkOf<YccIntChunk>(IntDecodeShared(shared), chunk.interior, chunk.images, chunk.interiorUnits), shared,
                      GridFor(warps, static_cast<long long>(smCount) * kYccBlocksPerSm), YccTableBytesOf(shared), stream);
+        break;
     }
     const int interior = Launched(1);
     if (interior < 0 || chunk.windows == 0)
@@ -797,7 +796,7 @@ int LaunchDecodeBatchChunk(const DecodeParams& shared, const BatchChunk& chunk, 
     return Launched(2);
 }
 
-int LaunchEncodeIndirect(const EncodeParams& shared, int hostDepth, bool tuned, int planeMask, const avifgpu_batch_image* images,
+int LaunchEncodeIndirect(const EncodeParams& shared, int hostDepth, EncodeFamily family, int planeMask, const avifgpu_batch_image* images,
                          const int32_t* count, int maxCount, void* workspace, int32_t* status, void* streamHandle)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
@@ -805,7 +804,7 @@ int LaunchEncodeIndirect(const EncodeParams& shared, int hostDepth, bool tuned, 
     EncodePlanner planner{};
     planner.shared = shared;
     planner.hostDepth = hostDepth;
-    planner.tuned = tuned ? 1 : 0;
+    planner.family = family;
     planner.planeMask = planeMask;
     PlanIndirectKernel<EncodePlanner><<<1, kPlanThreads, 0, stream>>>(planner, images, count, maxCount, workspace, status);
     if (Launched(1) < 0)
@@ -821,40 +820,45 @@ int LaunchEncodeIndirect(const EncodeParams& shared, int hostDepth, bool tuned, 
     return Launched(3);
 }
 
-int LaunchDecodeIndirect(const DecodeParams& shared, bool tuned, int planeMask, const avifgpu_batch_image* images, const int32_t* count,
+int LaunchDecodeIndirect(const DecodeParams& shared, DecodeFamily family, int planeMask, const avifgpu_batch_image* images, const int32_t* count,
                          int maxCount, void* workspace, int32_t* status, void* streamHandle)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
     const int smCount = SmCountOrDefault(shared.smCount);
     DecodePlanner planner{};
     planner.shared = shared;
-    planner.tuned = tuned ? 1 : 0;
+    planner.family = family;
     planner.planeMask = planeMask;
     PlanIndirectKernel<DecodePlanner><<<1, kPlanThreads, 0, stream>>>(planner, images, count, maxCount, workspace, status);
     if (Launched(1) < 0)
     {
         return AVIFGPU_ERR_CUDA;
     }
-    // A description the tuned kernel does not take plans no interior unit: its grid returns before staging, so it gets no tables.
-    // The grids are the chunk launchers' caps.
-    if (shared.colorspace == AVIFGPU_COLORSPACE_RGB && shared.hostDepth == 32)
+    // A description no batched family takes plans no interior unit; the call still makes its interior launch, on the batched
+    // kernel of its colour space and host depth, whose grid returns before staging (so it gets no tables).  The grids are the
+    // chunk launchers' caps.
+    const bool tuned = family != DecodeFamily::Generic;
+    const bool rgb = shared.colorspace == AVIFGPU_COLORSPACE_RGB;
+    const DecodeFamily interior = tuned ? family
+                                  : shared.hostDepth == 32 ? (rgb ? DecodeFamily::PlanarRgbF32 : DecodeFamily::YccF32)
+                                                           : (rgb ? DecodeFamily::PlanarRgbInt : DecodeFamily::YccInt);
+    switch (interior)
     {
+    case DecodeFamily::PlanarRgbF32:
         LaunchPlanarRgbF32(WorkspaceSource<TableDecodeParams, 0>{ TableDecodeDescription(shared), workspace, maxCount }, shared, LLONG_MAX, smCount,
                            tuned ? CodeTableBytes(shared.bitDepth, shared.hasAlpha != 0) : 0, stream);
-    }
-    else if (shared.colorspace == AVIFGPU_COLORSPACE_RGB)
-    {
+        break;
+    case DecodeFamily::PlanarRgbInt:
         LaunchPlanarRgbInt(WorkspaceSource<StreamDecodeParams, 0>{ StreamDecodeDescription(shared), workspace, maxCount }, shared, LLONG_MAX, smCount, stream);
-    }
-    else if (shared.hostDepth == 32)
-    {
+        break;
+    case DecodeFamily::YccF32:
         LaunchYccF32(WorkspaceSource<FastDecodeParams, 0>{ FillF32Description(shared), workspace, maxCount }, shared,
                      static_cast<unsigned>(smCount * kDecodeBlocksPerSm), tuned ? F32TableBytesOf(shared) : 0, stream);
-    }
-    else
-    {
+        break;
+    default:
         LaunchYccInt(WorkspaceSource<IntDecodeParams, 0>{ IntDecodeShared(shared), workspace, maxCount }, shared,
                      static_cast<unsigned>(smCount * kYccBlocksPerSm), tuned ? YccTableBytesOf(shared) : 0, stream);
+        break;
     }
     if (Launched(1) < 0)
     {

@@ -20,7 +20,6 @@ using namespace avifpix;
 constexpr int kTilePixels = 128;     // per row
 constexpr int kValuesPerLane = 24;   // 2 rows x 4 pixels x 3 channels
 constexpr int kCurveClip = 2;        // no transfer curve: code = trunc(clamp(v * max))
-constexpr int kSharedLibm = 768;
 
 struct FastEncodeParams
 {
@@ -46,7 +45,7 @@ struct FastEncodeParams
     CurveTableView table;
 };
 
-// The caller (LaunchEncodeFast) has checked ForwardMatrixStaysInRange(): luma needs no upper clamp, chroma only the
+// The route (EncodeFamilyOf) has checked ForwardMatrixStaysInRange(): luma needs no upper clamp, chroma only the
 // H.273 clip of 2^depth (a saturated red / blue) to 2^depth - 1, done on two packed codes at once.
 // A lane's 2 rows x 4 pixels of R'G'B' codes (as floats, row-major, interleaved) -> Y / Cb / Cr codes in the planes:
 // forward matrix, luma quantisation, chroma down-filter (the lane owns whole chroma sites, no cross-lane traffic).
@@ -235,12 +234,9 @@ __device__ __forceinline__ void StoreTile(const FastEncodeParams& p, const float
 } // namespace fastenc
 
 // kernels_fast_rgba.cu; `dest` is the description's avifgpu_source_layout bits (EncodeParams::destLayout)
-bool RgbaEncodeApplies(const fastenc::FastEncodeParams& fp);
 cudaError_t LaunchFastEncodeRgba(const fastenc::FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream);
 
 // kernels_fast_flat.cu
-bool FlatEncodeApplies(const fastenc::FastEncodeParams& fp);
-bool FlatEncodeReaches(const fastenc::FastEncodeParams& fp, int curve, int dest); // an instantiation exists for the table's form
 cudaError_t LaunchFastEncodeFlat(const fastenc::FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream);
 cudaError_t LaunchFastEncodeFlatInterleaved(const fastenc::FastEncodeParams& fp, int curve, int smCount, cudaStream_t stream);
 

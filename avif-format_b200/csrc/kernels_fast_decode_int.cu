@@ -252,42 +252,11 @@ cudaError_t LaunchStream(const StreamDecodeParams& sp, int smCount, cudaStream_t
 
 } // namespace
 
-// The block's aligned interior for the monochrome kernel (no premultiplied alpha, depth <= 12: checked by the caller), or
-// {0, 0} when a direct call takes another route.
-static Interior MonochromeInterior(const DecodeParams& p)
-{
-    const Interior none = { 0, 0 };
-    const int sampleBytes = p.hostDepth == 8 ? 1 : 2;
-    if ((sampleBytes == 1) != (p.bitDepth <= 8))
-    {
-        return none;
-    }
-    const int channels = p.hasAlpha ? 2 : 1;
-    const int planeAlign = 8 * sampleBytes;
-    const int rowAlign = (8 * channels * sampleBytes) % 16 == 0 ? 16 : 8;
-    if (!Aligned(p.plane[0], p.planeStride[0], planeAlign) || (p.hasAlpha && !Aligned(p.plane[3], p.planeStride[3], planeAlign)) ||
-        !Aligned(p.rows, p.rowStride, rowAlign))
-    {
-        return none;
-    }
-    const int width8 = p.width & ~7;
-    if (width8 < 8 || p.rowCount < 1)
-    {
-        return none;
-    }
-    return Interior{ width8, p.rowCount };
-}
-
-// Monochrome and planar-RGB images for the integer hosts; planar RGB routes as the batches do.
-static int LaunchDecodeStream(const DecodeParams& p, void* streamHandle)
+// Monochrome and planar-RGB images for the integer hosts.
+cudaError_t LaunchDecodeStream(const DecodeParams& p, Interior inner, void* streamHandle)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
     const bool mono = p.colorspace == AVIFGPU_COLORSPACE_MONOCHROME;
-    const Interior inner = mono ? MonochromeInterior(p) : DecodePlanarRgbInterior(p);
-    if (inner.width == 0)
-    {
-        return 0;
-    }
     StreamDecodeParams sp = StreamDecodeDescription(p);
     for (int k = 0; k < 4; ++k)
     {
@@ -299,32 +268,15 @@ static int LaunchDecodeStream(const DecodeParams& p, void* streamHandle)
     sp.groupsPerRow = inner.width / 8;
     sp.rowCount = inner.rows;
     const int smCount = SmCountOrDefault(p.smCount);
-    const cudaError_t e = WithIntDecodeKey(p, [&](auto sample, auto alpha) {
+    return WithIntDecodeKey(p, [&](auto sample, auto alpha) {
         using SampleT = TypeOf<decltype(sample)>;
         return mono ? LaunchStream<SampleT, 1 + alpha(), true>(sp, smCount, stream) : LaunchStream<SampleT, 3 + alpha(), false>(sp, smCount, stream);
     });
-    return CompleteDecode(e, p, inner.width, inner.rows, streamHandle);
 }
 
-// Returns the number of kernels launched, 0 if this configuration is not covered, or a negative status.
-int LaunchDecodeFastInteger(const DecodeParams& p, void* streamHandle)
+cudaError_t LaunchDecodeYccInt(const DecodeParams& p, Interior inner, void* streamHandle)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
-    if ((p.hostDepth != 8 && p.hostDepth != 16) || p.bitDepth > 12 || (p.hasAlpha && p.premultiplied))
-    {
-        return 0;
-    }
-    if (p.colorspace != AVIFGPU_COLORSPACE_YCBCR)
-    {
-        return LaunchDecodeStream(p, streamHandle);
-    }
-    const Interior inner = DecodeYccIntInterior(p);
-    if (inner.width == 0)
-    {
-        return 0;
-    }
-    const int width8 = inner.width;
-    const int evenRows = inner.rows;
     IntDecodeParams fp = IntDecodeShared(p);
     for (int k = 0; k < 4; ++k)
     {
@@ -333,14 +285,12 @@ int LaunchDecodeFastInteger(const DecodeParams& p, void* streamHandle)
     }
     fp.rows = static_cast<uint8_t*>(p.rows);
     fp.rowStride = p.rowStride;
-    fp.width = width8;
-    fp.rowCount = evenRows;
-
+    fp.width = inner.width;
+    fp.rowCount = inner.rows;
     const int smCount = SmCountOrDefault(p.smCount);
-    const cudaError_t e = WithYccIntKey(p, [&](auto sample, auto alpha, auto xs, auto ys, auto source) {
+    return WithYccIntKey(p, [&](auto sample, auto alpha, auto xs, auto ys, auto source) {
         return LaunchOne<TypeOf<decltype(sample)>, xs(), ys(), alpha(), source()>(fp, smCount, stream);
     });
-    return CompleteDecode(e, p, width8, evenRows, streamHandle);
 }
 
 } // namespace avifgpu

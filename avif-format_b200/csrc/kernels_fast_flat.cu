@@ -32,19 +32,13 @@ using avifmath::LibmTables;
 namespace
 {
 
-#ifndef AVIF_FLAT_WARPS
-#define AVIF_FLAT_WARPS 28
-#endif
-constexpr int kFlatWarps = AVIF_FLAT_WARPS;
+// The shared-memory layout's sizes (kFlatWarps, FlatFixedBytes, ...) are in kernel_params.h, where the route reads them.
 constexpr int kFlatThreads = kFlatWarps * 32;
-constexpr int kRowSegmentBytes = kTilePixels * 12;      // one tile row of RGB32f
-constexpr int kStageBytesPerWarp = 2 * kRowSegmentBytes; // both rows, linear
+constexpr int kRowSegmentBytes = kTilePixels * 12; // one tile row of RGB32f; a warp stages both rows, linear
+static_assert(kFlatStageBytesPerWarp == 2 * kRowSegmentBytes, "a warp's staging buffer holds both rows of its tile");
 constexpr int kRowSegmentWords = kRowSegmentBytes / 4;
-constexpr int kSharedBarriers = 256;                     // kFlatWarps x 8 bytes, padded; the last slot is the table's barrier
-constexpr int kTableBarrierSlot = kSharedBarriers / 8 - 1;
-static_assert(kFlatWarps <= kTableBarrierSlot, "the warps' barriers and the table's share kSharedBarriers");
-constexpr int kSharedLimit = 227 * 1024;
-__host__ __device__ constexpr int FlatFixedBytes() { return kSharedLibm + kSharedBarriers + kFlatWarps * kStageBytesPerWarp; }
+constexpr int kTableBarrierSlot = kFlatSharedBarriers / 8 - 1; // kFlatWarps x 8 bytes, padded; the last slot is the table's barrier
+static_assert(kFlatWarps <= kTableBarrierSlot, "the warps' barriers and the table's share kFlatSharedBarriers");
 
 // How the persistent warps share the tiles, worked out once on the host (the grid is known at launch).  The image is cut
 // into `items` = tilesX columns x `segments` runs of consecutive tile rows (run lengths differ by at most one), one item
@@ -88,18 +82,18 @@ __device__ __forceinline__ void EncodeRgbF32FlatBody(const FastEncodeParams& p, 
     extern __shared__ __align__(128) uint8_t sharedBytes[];
     uint64_t* libmStorage = reinterpret_cast<uint64_t*>(sharedBytes);
     uint64_t* barriers = reinterpret_cast<uint64_t*>(sharedBytes + kSharedLibm);
-    uint8_t* stageAll = sharedBytes + kSharedLibm + kSharedBarriers;
+    uint8_t* stageAll = sharedBytes + kSharedLibm + kFlatSharedBarriers;
     uint32_t* compactEntries = reinterpret_cast<uint32_t*>(sharedBytes + FlatFixedBytes());  // compact: the entries ...
     const uint32_t* firstBits = compactEntries + ((p.table.flatCount + 3) & ~3);             // ... then first_k per code
     uint2* octaves = reinterpret_cast<uint2*>(sharedBytes + FlatFixedBytes());               // two-level: 256 entries ...
-    uint32_t* bucketWords = reinterpret_cast<uint32_t*>(sharedBytes + FlatFixedBytes() + 2048); // ... then the bucket words
+    uint32_t* bucketWords = reinterpret_cast<uint32_t*>(sharedBytes + FlatFixedBytes() + kFlatOctaveBytes); // ... then the bucket words
 
     const int lane = threadIdx.x & 31;
     // Read through a shuffle so the compiler knows the warp index (and everything derived from it: tile coordinates,
     // copy addresses) is warp-uniform and keeps it in the uniform datapath, which the bulk-copy instruction needs.
     const int warpInBlock = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
     const uint32_t barrier = SharedAddress(barriers + warpInBlock);
-    uint32_t* stage = reinterpret_cast<uint32_t*>(stageAll + warpInBlock * kStageBytesPerWarp);
+    uint32_t* stage = reinterpret_cast<uint32_t*>(stageAll + warpInBlock * kFlatStageBytesPerWarp);
     const uint32_t stageAddress = SharedAddress(stage);
     const uint32_t* myStage = stage + lane * 12; // row 0; row 1 is kRowSegmentWords further
 
@@ -379,15 +373,10 @@ constexpr auto FlatKernelFor()
     }
 }
 
-inline size_t TableSharedBytes(const FastEncodeParams& fp, int table)
-{
-    return table == kTableTwoLevel ? 2048 + static_cast<size_t>(fp.table.bucketCount) * sizeof(uint32_t) : fp.table.compactImageBytes;
-}
-
 template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED = 0, int DEST = AVIFGPU_SOURCE_PLANAR>
 cudaError_t LaunchFlatKernel(const FastEncodeParams& fp, int smCount, cudaStream_t stream)
 {
-    const size_t shared = static_cast<size_t>(FlatFixedBytes()) + TableSharedBytes(fp, TABLE);
+    const size_t shared = static_cast<size_t>(FlatFixedBytes()) + FlatTableBytes(fp.table, TABLE == kTableTwoLevel);
     static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
     {
         const cudaError_t e = AllowDynamicShared(FlatKernelFor<CURVE, XS, YS, TABLE, INTERLEAVED, DEST>(), kSharedLimit, configuredDevices);
@@ -424,29 +413,10 @@ cudaError_t LaunchFlatKernel(const FastEncodeParams& fp, int smCount, cudaStream
 
 } // namespace
 
-static bool CompactTableFits(const FastEncodeParams& fp)
-{
-    return fp.table.compact != nullptr && fp.table.firstBits != nullptr && fp.table.bandBits != nullptr &&
-           static_cast<size_t>(FlatFixedBytes()) + TableSharedBytes(fp, kTableCompact) <= static_cast<size_t>(kSharedLimit);
-}
-
-static bool TwoLevelTableFits(const FastEncodeParams& fp)
-{
-    return fp.table.buckets != nullptr && fp.table.octaves != nullptr &&
-           static_cast<size_t>(FlatFixedBytes()) + TableSharedBytes(fp, kTableTwoLevel) <= static_cast<size_t>(kSharedLimit);
-}
-
-// True when the copy-engine kernel can serve this table: the compact form with its bitmap, else the two-level form, in
-// shared memory next to the staging buffers.
-bool FlatEncodeApplies(const FastEncodeParams& fp)
-{
-    return CompactTableFits(fp) || TwoLevelTableFits(fp);
-}
-
 // The reference's interleaved RGB layout through the same kernel (fp.planeY / strideY = the interleaved buffer).
 cudaError_t LaunchFastEncodeFlatInterleaved(const FastEncodeParams& fp, int curve, int smCount, cudaStream_t stream)
 {
-    if (CompactTableFits(fp))
+    if (FlatCompactFits(fp.table))
     {
         if (curve == kCurveLinearToPQ)
         {
@@ -459,21 +429,17 @@ cudaError_t LaunchFastEncodeFlatInterleaved(const FastEncodeParams& fp, int curv
     return LaunchFlatKernel<kCurveLinearToSMPTE428, 0, 0, kTableTwoLevel, 1>(fp, smCount, stream);
 }
 
-// The planar layout keeps every (curve, table) pair.  The other layouts (DEST != 0, picked by WithLayout) instantiate only
-// the pairs the tables built for 10/12-bit encodes reach (DESIGN.md 4.2): PQ with the compact table (kTableCompact14 for
+// The table's form picks the instantiation: the compact form with its bitmap when it fits, else the two-level form.  The
+// planar layout keeps every (curve, table) pair.  The other layouts (DEST != 0, picked by WithLayout) instantiate only the
+// pairs the tables built for 10/12-bit encodes reach (DESIGN.md 4.2): PQ with the compact table (kTableCompact14 for
 // flatShift 14, as at 12 bits, kTableCompact for any other shift), SMPTE 428 with the compact table (10 bits) or the
 // two-level one (12 bits, the only form built there).  A PQ table without its compact form has not been built for any
-// configuration so far; it returns false here and the launcher leaves the block to the generic kernel.
-bool FlatEncodeReaches(const FastEncodeParams& fp, int curve, int dest)
-{
-    return dest == AVIFGPU_SOURCE_PLANAR || curve != kCurveLinearToPQ || CompactTableFits(fp);
-}
-
+// configuration so far; EncodeFamilyOf leaves such a description with another layout to the generic kernel.
 cudaError_t LaunchFastEncodeFlat(const FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream)
 {
     return WithChroma(xs, ys, [&](auto XS, auto YS) {
         return WithLayout(dest, [&](auto DEST) {
-            if (CompactTableFits(fp))
+            if (FlatCompactFits(fp.table))
             {
                 if (curve == kCurveLinearToPQ)
                 {
@@ -488,7 +454,7 @@ cudaError_t LaunchFastEncodeFlat(const FastEncodeParams& fp, int curve, int xs, 
             }
             else if (curve == kCurveLinearToPQ)
             {
-                return cudaErrorInvalidValue; // FlatEncodeReaches said no: the launcher does not get here
+                return cudaErrorInvalidValue; // EncodeFamilyOf said no: the launcher does not get here
             }
             return LaunchFlatKernel<kCurveLinearToSMPTE428, XS(), YS(), kTableTwoLevel, 0, DEST()>(fp, smCount, stream);
         });

@@ -324,99 +324,69 @@ cudaError_t BuildGray16Lut(uint16_t* deviceLut, int smpte428, uint32_t maxCode, 
     return cudaGetLastError();
 }
 
-// Returns the number of kernels launched, 0 if this configuration is not covered, or a negative status.
-int LaunchEncodeFastInteger(const EncodeParams& p, int hostDepth, void* streamHandle)
+cudaError_t LaunchEncodeGray16Lut(const EncodeParams& p, Interior inner, void* streamHandle)
+{
+    static std::atomic<uint64_t> configuredDevices{ 0 };
+    if (const cudaError_t configured = AllowDynamicShared(EncodeGray16LutKernel, kLutEntries * 2, configuredDevices))
+    {
+        return configured;
+    }
+    Gray16Params gp{};
+    gp.rows = static_cast<const uint8_t*>(p.rows);
+    gp.rowStride = p.rowStride;
+    gp.planeY = static_cast<uint8_t*>(p.plane[0]);
+    gp.strideY = p.planeStride[0];
+    gp.chunksPerRow = inner.width / 8;
+    gp.rowCount = inner.rows;
+    gp.lut = p.gray16Lut;
+    EncodeGray16LutKernel<<<SmCountOrDefault(p.smCount), kLutThreads, kLutEntries * 2, static_cast<cudaStream_t>(streamHandle)>>>(gp);
+    return cudaGetLastError();
+}
+
+// Gray(+A) hosts in the reference layout (Y plane [0], alpha plane [3]).
+cudaError_t LaunchEncodeGrayInt(const EncodeParams& p, int hostDepth, Interior inner, void* streamHandle)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
-    if (hostDepth != 16 && hostDepth != 8)
-    {
-        return 0;
-    }
     const int smCount = SmCountOrDefault(p.smCount);
-
-    if (hostDepth == 16 && p.imageDepth > 8 && p.channels == 1 && !p.planar)
+    Rgb16Params rp{};
+    rp.rows = static_cast<const uint8_t*>(p.rows);
+    rp.rowStride = p.rowStride;
+    for (int k = 0; k < 4; ++k)
     {
-        if (p.gray16Lut == nullptr || p.width < 8 || !Aligned(p.rows, p.rowStride, 16) || !Aligned(p.plane[0], p.planeStride[0], 16))
-        {
-            return 0;
-        }
-        static std::atomic<uint64_t> configuredDevices{ 0 };
-        if (const cudaError_t configured = AllowDynamicShared(EncodeGray16LutKernel, kLutEntries * 2, configuredDevices))
-        {
-            return ReportLaunchFailure(static_cast<int>(configured));
-        }
-        Gray16Params gp{};
-        gp.rows = static_cast<const uint8_t*>(p.rows);
-        gp.rowStride = p.rowStride;
-        gp.planeY = static_cast<uint8_t*>(p.plane[0]);
-        gp.strideY = p.planeStride[0];
-        gp.chunksPerRow = p.width / 8;
-        gp.rowCount = p.rowCount;
-        gp.lut = p.gray16Lut;
-        EncodeGray16LutKernel<<<smCount, kLutThreads, kLutEntries * 2, stream>>>(gp);
-        return CompleteEncode(cudaGetLastError(), p, hostDepth, gp.chunksPerRow * 8, p.rowCount, streamHandle);
+        rp.plane[k] = static_cast<uint8_t*>(p.plane[k]);
+        rp.stride[k] = p.planeStride[k];
     }
-
-    // Gray(+A) hosts in the reference layout (Y plane [0], alpha plane [3]); premultiplication and the Gray16 SMPTE 428
-    // composition stay with the generic kernel (the latter has its own table kernel above for one channel).
-    if (!p.planar && (p.channels == 1 || p.channels == 2) && !p.premultiply && !p.gray16Smpte428 && p.imageDepth <= 12)
+    rp.groupsPerRow = inner.width / 8;
+    rp.rowCount = inner.rows;
+    rp.maxCodeFloat = p.maxCodeFloat;
+    rp.biasedMax = 8388608.0f + p.maxCodeFloat;
+    rp.maxCode = p.maxCode;
+    rp.maxReciprocal = 1.0f / p.maxCodeFloat;
+    const bool widePlanes = p.imageDepth > 8;
+    if (hostDepth == 16)
     {
-        const int hostBytes = hostDepth / 8;
-        const int planeBytes = p.imageDepth > 8 ? 2 : 1;
-        const int rowAlign = (8 * p.channels * hostBytes) % 16 == 0 ? 16 : 8;
-        if (p.width < 8 || p.rowCount < 1 || !Aligned(p.rows, p.rowStride, rowAlign) || !Aligned(p.plane[0], p.planeStride[0], 8 * planeBytes) ||
-            (p.channels == 2 && !Aligned(p.plane[3], p.planeStride[3], 8 * planeBytes)))
-        {
-            return 0;
-        }
-        const int width8 = p.width & ~7;
-        Rgb16Params rp{};
-        rp.rows = static_cast<const uint8_t*>(p.rows);
-        rp.rowStride = p.rowStride;
-        for (int k = 0; k < 4; ++k)
-        {
-            rp.plane[k] = static_cast<uint8_t*>(p.plane[k]);
-            rp.stride[k] = p.planeStride[k];
-        }
-        rp.groupsPerRow = width8 / 8;
-        rp.rowCount = p.rowCount;
-        rp.maxCodeFloat = p.maxCodeFloat;
-        rp.biasedMax = 8388608.0f + p.maxCodeFloat;
-        rp.maxCode = p.maxCode;
-        rp.maxReciprocal = 1.0f / p.maxCodeFloat;
-        cudaError_t e;
-        if (hostBytes == 2)
-        {
-            e = planeBytes == 2 ? LaunchGrayInt<uint16_t, uint16_t>(rp, p.channels, smCount, stream) : LaunchGrayInt<uint16_t, uint8_t>(rp, p.channels, smCount, stream);
-        }
-        else
-        {
-            e = planeBytes == 2 ? LaunchGrayInt<uint8_t, uint16_t>(rp, p.channels, smCount, stream) : LaunchGrayInt<uint8_t, uint8_t>(rp, p.channels, smCount, stream);
-        }
-        return CompleteEncode(e, p, hostDepth, width8, p.rowCount, streamHandle);
+        return widePlanes ? LaunchGrayInt<uint16_t, uint16_t>(rp, p.channels, smCount, stream) : LaunchGrayInt<uint16_t, uint8_t>(rp, p.channels, smCount, stream);
     }
+    return widePlanes ? LaunchGrayInt<uint8_t, uint16_t>(rp, p.channels, smCount, stream) : LaunchGrayInt<uint8_t, uint8_t>(rp, p.channels, smCount, stream);
+}
 
-    const Interior inner = EncodeRgbIntInterior(p, hostDepth);
-    if (inner.width > 0)
+cudaError_t LaunchEncodeRgbInt(const EncodeParams& p, int hostDepth, Interior inner, void* streamHandle)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
+    const int smCount = SmCountOrDefault(p.smCount);
+    Rgb16Params rp = RgbIntShared(p);
+    rp.rows = static_cast<const uint8_t*>(p.rows);
+    rp.rowStride = p.rowStride;
+    for (int k = 0; k < 4; ++k)
     {
-        const int width8 = inner.width;
-        const int evenRows = inner.rows;
-        Rgb16Params rp = RgbIntShared(p);
-        rp.rows = static_cast<const uint8_t*>(p.rows);
-        rp.rowStride = p.rowStride;
-        for (int k = 0; k < 4; ++k)
-        {
-            rp.plane[k] = static_cast<uint8_t*>(p.plane[k]);
-            rp.stride[k] = p.planeStride[k];
-        }
-        rp.groupsPerRow = width8 / 8;
-        rp.rowCount = evenRows;
-        const cudaError_t e = WithRgbIntKey(p, hostDepth, [&](auto host, auto plane, auto channels, auto premultiply, auto xs, auto ys, auto dest) {
-            return LaunchRgbInt<TypeOf<decltype(host)>, TypeOf<decltype(plane)>, channels(), xs(), ys(), premultiply(), dest()>(rp, smCount, stream);
-        });
-        return CompleteEncode(e, p, hostDepth, width8, evenRows, streamHandle);
+        rp.plane[k] = static_cast<uint8_t*>(p.plane[k]);
+        rp.stride[k] = p.planeStride[k];
     }
-    return 0;
+    rp.groupsPerRow = inner.width / 8;
+    rp.rowCount = inner.rows;
+    return WithRgbIntKey(p, hostDepth, [&](auto host, auto plane, auto channels, auto premultiply, auto xs, auto ys, auto dest) {
+        return LaunchRgbInt<TypeOf<decltype(host)>, TypeOf<decltype(plane)>, channels(), xs(), ys(), premultiply(), dest()>(rp, smCount, stream);
+    });
 }
 
 } // namespace avifgpu

@@ -21,16 +21,8 @@ using avifmath::LibmTables;
 namespace
 {
 
-#ifndef AVIF_RGBA_WARPS
-#define AVIF_RGBA_WARPS 16
-#endif
-constexpr int kRgbaWarps = AVIF_RGBA_WARPS;
+// The shared-memory layout's sizes (kRgbaWarps, RgbaFixedBytes, ...) are in kernel_params.h, where the route reads them.
 constexpr int kRgbaThreads = kRgbaWarps * 32;
-constexpr int kLaneStrideWords = 28; // 24 colour samples + padding: 16-byte aligned, conflict-free for STS.128
-constexpr int kStagePerWarp = 32 * kLaneStrideWords * 4;
-constexpr int kSharedLimit = 227 * 1024;
-constexpr int kTableBarrierBytes = 16; // the table image's mbarrier, padded
-__host__ __device__ constexpr int RgbaFixedBytes() { return kSharedLibm + kTableBarrierBytes + kRgbaWarps * kStagePerWarp; }
 
 // The compact table + first_k array in shared memory (kernels_fast_flat.cu has the commentary).  DEST: the
 // avifgpu_source_layout bits of the planes written (StoreTile; the alpha plane is shifted like the others).  The body of
@@ -41,7 +33,7 @@ __device__ __forceinline__ void EncodeRgbaF32FlatBody(const FastEncodeParams& p)
     extern __shared__ __align__(16) uint8_t sharedBytes[];
     uint64_t* libmStorage = reinterpret_cast<uint64_t*>(sharedBytes);
     uint64_t* tableBarrier = reinterpret_cast<uint64_t*>(sharedBytes + kSharedLibm);
-    uint32_t* stageAll = reinterpret_cast<uint32_t*>(sharedBytes + kSharedLibm + kTableBarrierBytes);
+    uint32_t* stageAll = reinterpret_cast<uint32_t*>(sharedBytes + kSharedLibm + kRgbaTableBarrierBytes);
     uint32_t* compactEntries = reinterpret_cast<uint32_t*>(sharedBytes + RgbaFixedBytes());
     const uint32_t* firstBits = compactEntries + ((p.table.flatCount + 3) & ~3);
 
@@ -54,7 +46,7 @@ __device__ __forceinline__ void EncodeRgbaF32FlatBody(const FastEncodeParams& p)
 
     const int lane = threadIdx.x & 31;
     const int warpInBlock = threadIdx.x >> 5;
-    uint32_t* myStage = stageAll + warpInBlock * (32 * kLaneStrideWords) + lane * kLaneStrideWords;
+    uint32_t* myStage = stageAll + warpInBlock * (32 * kRgbaLaneStrideWords) + lane * kRgbaLaneStrideWords;
     const uint32_t flatShift = p.table.flatShift;
     const int32_t negativeLow = -static_cast<int32_t>(p.table.flatLow);
     const int32_t span = static_cast<int32_t>(p.table.flatHigh - p.table.flatLow);
@@ -276,13 +268,6 @@ cudaError_t LaunchRgbaKernel(const FastEncodeParams& fp, int smCount, cudaStream
 }
 
 } // namespace
-
-// True when the kernel can stage this table's compact image next to its buffers.
-bool RgbaEncodeApplies(const FastEncodeParams& fp)
-{
-    return fp.planeA != nullptr && fp.table.compact != nullptr && fp.table.firstBits != nullptr && fp.table.bandBits != nullptr &&
-           static_cast<size_t>(RgbaFixedBytes()) + fp.table.compactImageBytes <= static_cast<size_t>(kSharedLimit);
-}
 
 cudaError_t LaunchFastEncodeRgba(const FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream)
 {

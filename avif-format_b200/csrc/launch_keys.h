@@ -131,7 +131,7 @@ auto WithYccIntKey(const DecodeParams& d, F&& f)
 
 // Float YCbCr decode (DecodeYccToRgbF32Kernel, DecodeYccToRgbF32BatchKernel).  f(TRANSFER, FASTDIV, ALPHA, XS, YS, SOURCE):
 // PQ with (FASTDIV = 1) or without the context's verified division, HLG, and SMPTE 428 for anything else --
-// DecodeYccF32Tuned leaves these three.
+// DecodeFamilyOf leaves these three.
 template <typename F>
 auto WithYccF32Key(const DecodeParams& d, F&& f)
 {

@@ -3,7 +3,7 @@
 // sizes (1 x 1, widths below 8, odd widths and heights) on fake planes, some of them misaligned:
 //   - every pixel and every chroma site of every image is covered exactly once, by an interior, an edge window or a
 //     direct call, read back from the records' rows and plane pointers;
-//   - an image is batched exactly when EncodeRgbIntInterior takes it, and its interior is that rectangle;
+//   - an image is batched exactly when EncodeBlockInterior of EncodeBatchFamilyOf takes it, and its interior is that rectangle;
 //   - chunks hold at most kBatchChunkImages images in increasing order, records' first units are the running sums of
 //     their unit counts, and a chunk has a second launch exactly when one of its images has a strip outside its interior;
 //   - a chunk's kernel parameters fit the 32764-byte limit.
@@ -186,7 +186,7 @@ int main()
                                                 if (i <= previous) Fail("image order", descriptions, static_cast<int>(batches));
                                                 previous = i;
                                                 batched[i] = 1;
-                                                const Interior inner = EncodeRgbIntInterior(fake[i].p, hostDepth);
+                                                const Interior inner = EncodeBlockInterior(EncodeBatchFamilyOf(fake[i].p, hostDepth), fake[i].p, hostDepth);
                                                 const BatchRecord& r = c.interior[j];
                                                 if (r.firstUnit != units || r.width != inner.width || r.rowCount != inner.rows || r.rows != fake[i].p.rows)
                                                 {
@@ -211,7 +211,7 @@ int main()
                                             for (int j = 0; j < c.images; ++j)
                                             {
                                                 const EncodeParams& q = fake[c.imageIndex[j]].p;
-                                                const Interior inner = EncodeRgbIntInterior(q, hostDepth);
+                                                const Interior inner = EncodeBlockInterior(EncodeBatchFamilyOf(q, hostDepth), q, hostDepth);
                                                 edges = edges || inner.width < q.width || inner.rows < q.rowCount;
                                             }
                                             if (BatchChunkLaunches(c) != (edges ? 2 : 1)) Fail("launches", descriptions, static_cast<int>(batches));
@@ -226,7 +226,7 @@ int main()
                                         }
                                         for (int i = 0; i < n; ++i)
                                         {
-                                            const bool eligible = EncodeRgbIntInterior(fake[i].p, hostDepth).width > 0;
+                                            const bool eligible = EncodeBlockInterior(EncodeBatchFamilyOf(fake[i].p, hostDepth), fake[i].p, hostDepth).width > 0;
                                             if (eligible != (batched[i] == 1) || batched[i] == 0)
                                             {
                                                 Fail("eligible / fallback against the predicate", descriptions, static_cast<int>(batches));
@@ -246,7 +246,7 @@ int main()
     std::printf("encode descriptions=%d batches=%lld images=%lld\n", descriptions, batches, images);
 
     // decode: every YCbCr integer-host description; coverage of every pixel from the rows pointers, routing against
-    // DecodeYccIntInterior, launches against the strips
+    // DecodeBlockInterior of DecodeBatchFamilyOf, launches against the strips
     int decodeDescriptions = 0;
     long long decodeImages = 0;
     for (int hostDepth : { 8, 16 })
@@ -337,7 +337,7 @@ int main()
                             {
                                 const int i = c.imageIndex[j];
                                 batched[i] = 1;
-                                const Interior inner = DecodeYccIntInterior(params[i]);
+                                const Interior inner = DecodeBlockInterior(DecodeBatchFamilyOf(params[i]), params[i]);
                                 edges = edges || inner.width < params[i].width || inner.rows < params[i].rowCount;
                                 cover(i, c.interior[j]);
                             }
@@ -351,7 +351,7 @@ int main()
                         }
                         for (int i = 0; i < n; ++i)
                         {
-                            if ((DecodeYccIntInterior(params[i]).width > 0) != (batched[i] == 1)) Fail("decode routing", decodeDescriptions, trial);
+                            if ((DecodeBlockInterior(DecodeBatchFamilyOf(params[i]), params[i]).width > 0) != (batched[i] == 1)) Fail("decode routing", decodeDescriptions, trial);
                             for (int v : count[i])
                                 if (v != 1) { Fail("decode pixel not covered exactly once", decodeDescriptions, trial); break; }
                         }

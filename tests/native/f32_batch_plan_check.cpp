@@ -6,7 +6,7 @@
 // widths below 4, one-row images, some with misaligned rows or Y planes, some with unequal Cb / Cr strides -- on fake
 // padded planes:
 //   host plans     every pixel of every image is covered exactly once by an interior, a window or a direct call; an
-//                  image is batched exactly when DecodeYccF32Interior takes it, with that interior; chunks keep image
+//                  image is batched exactly when DecodeBlockInterior of DecodeBatchFamilyOf takes it, with that interior; chunks keep image
 //                  order and hold at most kBatchChunkImages images; first units are running sums of 128-pixel units; a
 //                  chunk has a second launch exactly when one of its images has a strip outside its interior;
 //   per-image step every pixel covered exactly once by the interior and windows; every record's planes where DecodeWindow
@@ -138,10 +138,11 @@ int main()
                         probe.verifiedHlgDivisions = verified;
                         probe.verifiedGreenDivision = verified;
                         probe.verifiedPqRatio = verified;
-                        const bool tuned = DecodeBatchTuned(probe);
-                        if (tuned != DecodeYccF32Tuned(probe))
+                        const DecodeFamily family = DecodeBatchFamilyOf(probe);
+                        const bool tuned = family != DecodeFamily::Generic;
+                        if (tuned != (DecodeFamilyOf(probe) == DecodeFamily::YccF32))
                         {
-                            Fail("DecodeBatchTuned is not the float predicate for 32-bit hosts", descriptions, -1);
+                            Fail("DecodeBatchFamilyOf is not the float family for 32-bit hosts", descriptions, -1);
                         }
                         const bool expectTuned = bitDepth >= 10 && bitDepth <= 12 && alpha != 2 && (curve.transferCharacteristics != 18 || verified);
                         if (tuned != expectTuned)
@@ -222,7 +223,7 @@ int main()
                                     }
                                     last = i;
                                     batched[i] = 1;
-                                    const Interior inner = DecodeYccF32Interior(params[i]);
+                                    const Interior inner = DecodeBlockInterior(DecodeBatchFamilyOf(params[i]), params[i]);
                                     if (c.interior[j].width != inner.width || c.interior[j].rowCount != inner.rows || c.interior[j].firstUnit != first)
                                     {
                                         Fail("chunk interior", descriptions, trial);
@@ -254,7 +255,7 @@ int main()
                             }
                             for (int i = 0; i < n; ++i)
                             {
-                                if ((DecodeYccF32Interior(params[i]).width > 0) != (batched[i] == 1))
+                                if ((DecodeBlockInterior(DecodeBatchFamilyOf(params[i]), params[i]).width > 0) != (batched[i] == 1))
                                 {
                                     Fail("image routing", descriptions, trial);
                                 }
@@ -270,9 +271,9 @@ int main()
                             int64_t total = 0;
                             for (int i = 0; i < n; ++i)
                             {
-                                const BatchImagePlan step = PlanBatchDecodeImage(probe, tuned, planeMask, batch[i]);
+                                const BatchImagePlan step = PlanBatchDecodeImage(probe, family, planeMask, batch[i]);
                                 std::vector<int> covered(static_cast<size_t>(params[i].width) * params[i].rowCount, 0);
-                                const Interior inner = DecodeYccF32Interior(params[i]);
+                                const Interior inner = DecodeBlockInterior(DecodeBatchFamilyOf(params[i]), params[i]);
                                 if (step.status != AVIFGPU_OK || step.interior.width != inner.width || (inner.width > 0 && step.interior.rowCount != inner.rows))
                                 {
                                     Fail("step interior", descriptions, trial);

@@ -7,7 +7,7 @@
 //     no record, an empty image OK and no record;
 //   - every pixel of an accepted image is covered exactly once by its interior and windows, judged from the records'
 //     rows pointers, and each record's luma and chroma planes sit at its first pixel and chroma site;
-//   - an image has an interior exactly when EncodeRgbIntInterior / DecodeYccIntInterior of its own block (built here as a
+//   - an image has an interior exactly when EncodeBlockInterior / DecodeBlockInterior of the batched family of its own block (built here as a
 //     direct call builds it) takes it, that interior is the predicate's rectangle, and its windows are the strips around
 //     it; any other image is exactly one whole-image window; every unit count matches its record;
 //   - with the records laid out at the exclusive prefix sums of their units (IndirectWorkspaceLayout), FindRecord finds
@@ -255,7 +255,8 @@ int main()
                                 EncodeParams shared;
                                 FillEncodeParams(d, &shared);
                                 shared.verifiedPremultiply = verified;
-                                const bool tuned = EncodeRgbIntTuned(shared, hostDepth);
+                                const EncodeFamily family = EncodeBatchFamilyOf(shared, hostDepth);
+                        const bool tuned = family == EncodeFamily::RgbInt;
                                 const int n = 1 + static_cast<int>(rng() % 120);
                                 std::vector<int> rejected;
                                 const std::vector<avifgpu_batch_image> batch =
@@ -264,7 +265,7 @@ int main()
                                 std::vector<BatchImagePlan> plans(n);
                                 for (int i = 0; i < n; ++i)
                                 {
-                                    const BatchImagePlan& q = plans[i] = PlanBatchEncodeImage(shared, hostDepth, tuned, planeMask, batch[i]);
+                                    const BatchImagePlan& q = plans[i] = PlanBatchEncodeImage(shared, hostDepth, family, planeMask, batch[i]);
                                     if (q.status != (rejected[i] ? AVIFGPU_ERR_BAD_PARAM : AVIFGPU_OK)) Fail("encode status", descriptions, i);
                                     if (rejected[i] || batch[i].width == 0 || batch[i].height == 0)
                                     {
@@ -290,7 +291,7 @@ int main()
                                             p.planeStride[k] = batch[i].planes.stride[k];
                                         }
                                     }
-                                    CheckImagePlan("encode", q, p, EncodeRgbIntInterior(p, hostDepth), EncodeHostColBytes(d), depth > 8 ? 2 : 1, p.xs, p.ys,
+                                    CheckImagePlan("encode", q, p, EncodeBlockInterior(EncodeBatchFamilyOf(p, hostDepth), p, hostDepth), EncodeHostColBytes(d), depth > 8 ? 2 : 1, p.xs, p.ys,
                                                    descriptions, i);
                                 }
                                 CheckLayoutAndSearch(rng, plans, descriptions);
@@ -328,7 +329,8 @@ int main()
                         planeMask |= g.present ? 1 << k : 0;
                         planeXs[k] = g.xs;
                     }
-                    const bool tuned = DecodeYccIntTuned(shared);
+                    const DecodeFamily family = DecodeBatchFamilyOf(shared);
+                    const bool tuned = family == DecodeFamily::YccInt;
                     for (int trial = 0; trial < 4; ++trial)
                     {
                         const int n = 1 + static_cast<int>(rng() % 120);
@@ -338,7 +340,7 @@ int main()
                         std::vector<BatchImagePlan> plans(n);
                         for (int i = 0; i < n; ++i)
                         {
-                            const BatchImagePlan& q = plans[i] = PlanBatchDecodeImage(shared, tuned, planeMask, batch[i]);
+                            const BatchImagePlan& q = plans[i] = PlanBatchDecodeImage(shared, family, planeMask, batch[i]);
                             if (q.status != (rejected[i] ? AVIFGPU_ERR_BAD_PARAM : AVIFGPU_OK)) Fail("decode status", decodeDescriptions, i);
                             if (rejected[i] || batch[i].width == 0 || batch[i].height == 0)
                             {
@@ -362,7 +364,7 @@ int main()
                                     p.planeStride[k] = batch[i].planes.stride[k];
                                 }
                             }
-                            CheckImagePlan("decode", q, p, DecodeYccIntInterior(p), DecodeHostColBytes(d), bitDepth > 8 ? 2 : 1, 0, 0, decodeDescriptions, i);
+                            CheckImagePlan("decode", q, p, DecodeBlockInterior(DecodeBatchFamilyOf(p), p), DecodeHostColBytes(d), bitDepth > 8 ? 2 : 1, 0, 0, decodeDescriptions, i);
                         }
                         CheckLayoutAndSearch(rng, plans, decodeDescriptions);
                     }

@@ -5,10 +5,10 @@
 // HLG with and without the OOTF and SMPTE 428) and seeded random batches of 1 to 300 images of mixed sizes -- widths 1 to
 // 7, 8, 9, 255, 256, 257 and random ones, one-row images, some with rows misaligned by 4 or 8 bytes, some with an R, G, B
 // or alpha plane misaligned by 2 or 8 bytes -- on fake padded planes:
-//   description    DecodeBatchTuned is DecodePlanarRgbTuned, and takes exactly the descriptions with no or straight alpha
+//   description    DecodeBatchFamilyOf is a planar-RGB family, and takes exactly the descriptions with no or straight alpha
 //                  and a depth its kernel reads;
 //   host plans     every pixel of every image is covered exactly once by an interior, a window or a direct call; an
-//                  image is batched exactly when DecodePlanarRgbTuned and DecodePlanarRgbBlockInterior of its own block
+//                  image is batched exactly when the route (DecodeBatchFamilyOf, DecodeBlockInterior) of its own block
 //                  take it, with that interior, which is also the one an independent statement of the kernels' alignment
 //                  rules gives; chunks keep image order and hold at most kBatchChunkImages images; first units are running
 //                  sums of 256-pixel units; the only window of a batched image is its right strip; a chunk has a second
@@ -16,7 +16,7 @@
 //   per-image step every pixel covered exactly once by the interior and windows; every record's planes where DecodeWindow
 //                  puts them; interior units counted with the 256-pixel unit, window units as BatchEdgeUnits; FindRecord
 //                  over the concatenated interior units finds the record that owns each unit.
-// YCbCr and monochrome descriptions route as they did: DecodeBatchTuned is the float YCbCr predicate for 32-bit hosts and
+// YCbCr and monochrome descriptions route as they did: DecodeBatchFamilyOf is the float YCbCr family for 32-bit hosts and
 // the integer one otherwise, with 128- and 256-pixel units; monochrome is never batched.
 // Prints "rgb descriptions=N images=K units=U ycbcr=Y"; exit code 1 on any failure.
 #include "batch_plan.h"
@@ -114,6 +114,8 @@ bool AlignedTo(const void* p, int64_t stride, int alignment)
 // The kernels' block conditions, restated: StreamDecodeKernel reads 8 samples per plane with one 64-bit (8-bit planes) or
 // 128-bit load and stores 8 pixels with 64-bit stores (RGB8) or 128-bit ones; TableDecodeF32Kernel reads 128 bits per
 // plane and stores 128-bit words.  Width rounded down to 8 pixels, at least 8; every row.
+bool IsPlanarRgb(DecodeFamily family) { return family == DecodeFamily::PlanarRgbInt || family == DecodeFamily::PlanarRgbF32; }
+
 Interior ExpectedInterior(const DecodeParams& p)
 {
     const bool tuned = p.colorspace == AVIFGPU_COLORSPACE_RGB && !(p.hasAlpha && p.premultiplied) && p.bitDepth <= 12 &&
@@ -180,8 +182,8 @@ int main()
                                 p.verifiedGreenDivision = verified;
                                 p.verifiedPqRatio = verified;
                                 ++ycbcr;
-                                const bool before = hostDepth == 32 ? DecodeYccF32Tuned(p) : DecodeYccIntTuned(p);
-                                if (DecodeBatchTuned(p) != before || DecodePlanarRgbTuned(p))
+                                const bool before = hostDepth == 32 ? (DecodeFamilyOf(p) == DecodeFamily::YccF32) : (DecodeFamilyOf(p) == DecodeFamily::YccInt);
+                                if ((DecodeBatchFamilyOf(p) != DecodeFamily::Generic) != before || IsPlanarRgb(DecodeBatchFamilyOf(p)))
                                 {
                                     Fail("YCbCr / monochrome description routing changed", ycbcr, -1);
                                 }
@@ -189,7 +191,7 @@ int main()
                                 {
                                     Fail("monochrome batched", ycbcr, -1);
                                 }
-                                if (DecodeBatchUnitPixels(hostDepth, colorspace) != (hostDepth == 32 ? 128 : 256))
+                                if (DecodeBatchUnitPixels(hostDepth == 32 ? DecodeFamily::YccF32 : DecodeFamily::YccInt) != (hostDepth == 32 ? 128 : 256))
                                 {
                                     Fail("YCbCr / monochrome unit width changed", ycbcr, -1);
                                 }
@@ -224,17 +226,18 @@ int main()
                         {
                             continue;
                         }
-                        const bool tuned = DecodeBatchTuned(probe);
-                        if (tuned != DecodePlanarRgbTuned(probe))
+                        const DecodeFamily family = DecodeBatchFamilyOf(probe);
+                        const bool tuned = family != DecodeFamily::Generic;
+                        if (tuned != IsPlanarRgb(DecodeBatchFamilyOf(probe)))
                         {
-                            Fail("DecodeBatchTuned is not the planar-RGB predicate for RGB", descriptions, -1);
+                            Fail("DecodeBatchFamilyOf is not the planar-RGB family for RGB", descriptions, -1);
                         }
                         const bool expectTuned = alpha != 2 && bitDepth <= 12 && (hostDepth == 8 ? bitDepth == 8 : bitDepth >= 10);
                         if (tuned != expectTuned)
                         {
                             Fail("description routing", descriptions, -1);
                         }
-                        if (DecodeBatchUnitPixels(hostDepth, AVIFGPU_COLORSPACE_RGB) != 256)
+                        if (DecodeBatchUnitPixels(hostDepth == 32 ? DecodeFamily::PlanarRgbF32 : DecodeFamily::PlanarRgbInt) != 256)
                         {
                             Fail("planar-RGB unit width", descriptions, -1);
                         }
@@ -278,8 +281,8 @@ int main()
                             {
                                 batch[i] = BatchImageOf(params[i]);
                                 const Interior expected = ExpectedInterior(params[i]);
-                                const Interior inner = DecodePlanarRgbInterior(params[i]);
-                                const Interior split = DecodePlanarRgbTuned(params[i]) ? DecodePlanarRgbBlockInterior(params[i]) : Interior{ 0, 0 };
+                                const Interior inner = DecodeBlockInterior(DecodeBatchFamilyOf(params[i]), params[i]);
+                                const Interior split = IsPlanarRgb(DecodeBatchFamilyOf(params[i])) ? DecodePlanarRgbBlockInterior(params[i]) : Interior{ 0, 0 };
                                 if (inner.width != expected.width || inner.rows != expected.rows || split.width != inner.width || split.rows != inner.rows)
                                 {
                                     Fail("interior against the kernels' restated conditions", descriptions, trial);
@@ -314,7 +317,7 @@ int main()
                                     }
                                     last = i;
                                     batched[i] = 1;
-                                    const Interior inner = DecodePlanarRgbInterior(params[i]);
+                                    const Interior inner = DecodeBlockInterior(DecodeBatchFamilyOf(params[i]), params[i]);
                                     if (c.interior[j].width != inner.width || c.interior[j].rowCount != inner.rows || c.interior[j].firstUnit != first)
                                     {
                                         Fail("chunk interior", descriptions, trial);
@@ -345,7 +348,7 @@ int main()
                             int batchedImages = 0;
                             for (int i = 0; i < n; ++i)
                             {
-                                batchedImages += DecodePlanarRgbInterior(params[i]).width > 0 ? 1 : 0;
+                                batchedImages += DecodeBlockInterior(DecodeBatchFamilyOf(params[i]), params[i]).width > 0 ? 1 : 0;
                             }
                             if (static_cast<int>(plan.chunks.size()) != (batchedImages + kBatchChunkImages - 1) / kBatchChunkImages)
                             {
@@ -361,7 +364,7 @@ int main()
                             }
                             for (int i = 0; i < n; ++i)
                             {
-                                if ((DecodePlanarRgbInterior(params[i]).width > 0) != (batched[i] == 1))
+                                if ((DecodeBlockInterior(DecodeBatchFamilyOf(params[i]), params[i]).width > 0) != (batched[i] == 1))
                                 {
                                     Fail("image routing", descriptions, trial);
                                 }
@@ -377,9 +380,9 @@ int main()
                             int64_t total = 0;
                             for (int i = 0; i < n; ++i)
                             {
-                                const BatchImagePlan step = PlanBatchDecodeImage(probe, tuned, planeMask, batch[i]);
+                                const BatchImagePlan step = PlanBatchDecodeImage(probe, family, planeMask, batch[i]);
                                 std::vector<int> covered(static_cast<size_t>(params[i].width) * params[i].rowCount, 0);
-                                const Interior inner = DecodePlanarRgbInterior(params[i]);
+                                const Interior inner = DecodeBlockInterior(DecodeBatchFamilyOf(params[i]), params[i]);
                                 if (step.status != AVIFGPU_OK || step.interior.width != inner.width || (inner.width > 0 && step.interior.rowCount != inner.rows))
                                 {
                                     Fail("step interior", descriptions, trial);

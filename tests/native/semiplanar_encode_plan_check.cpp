@@ -350,10 +350,11 @@ int main()
                         {
                             Fail("FillEncodeParams does not carry the layout", descriptions, -1);
                         }
-                        const bool tuned = EncodeRgbIntTuned(probe, hostDepth);
+                        const EncodeFamily family = EncodeBatchFamilyOf(probe, hostDepth);
+                        const bool tuned = family == EncodeFamily::RgbInt;
                         EncodeParams planarProbe = probe;
                         planarProbe.destLayout = 0;
-                        if (!tuned || EncodeRgbIntTuned(planarProbe, hostDepth) != tuned)
+                        if (!tuned || (EncodeBatchFamilyOf(planarProbe, hostDepth) == EncodeFamily::RgbInt) != tuned)
                         {
                             Fail("description routing depends on the layout", descriptions, -1);
                         }
@@ -443,7 +444,7 @@ int main()
                                     }
                                     last = i;
                                     batched[i] = 1;
-                                    const Interior inner = EncodeRgbIntInterior(params[i], hostDepth);
+                                    const Interior inner = EncodeBlockInterior(EncodeBatchFamilyOf(params[i], hostDepth), params[i], hostDepth);
                                     if (c.interior[j].width != inner.width || c.interior[j].rowCount != inner.rows || c.interior[j].firstUnit != first)
                                     {
                                         Fail("chunk interior", descriptions, trial);
@@ -482,7 +483,7 @@ int main()
                             for (int i = 0; i < n; ++i)
                             {
                                 const EncodeParams& p = params[i];
-                                const Interior inner = EncodeRgbIntInterior(p, hostDepth);
+                                const Interior inner = EncodeBlockInterior(EncodeBatchFamilyOf(p, hostDepth), p, hostDepth);
                                 if ((inner.width > 0) != (batched[i] == 1))
                                 {
                                     Fail("image routing", descriptions, trial);
@@ -510,9 +511,9 @@ int main()
                             int64_t total = 0;
                             for (int i = 0; i < n; ++i)
                             {
-                                const BatchImagePlan step = PlanBatchEncodeImage(probe, hostDepth, tuned, planeMask, batch[i]);
+                                const BatchImagePlan step = PlanBatchEncodeImage(probe, hostDepth, family, planeMask, batch[i]);
                                 std::vector<int> covered(static_cast<size_t>(params[i].width) * params[i].rowCount, 0);
-                                const Interior inner = EncodeRgbIntInterior(params[i], hostDepth);
+                                const Interior inner = EncodeBlockInterior(EncodeBatchFamilyOf(params[i], hostDepth), params[i], hostDepth);
                                 if (step.status != AVIFGPU_OK || step.interior.width != inner.width || (inner.width > 0 && step.interior.rowCount != inner.rows))
                                 {
                                     Fail("step interior", descriptions, trial);

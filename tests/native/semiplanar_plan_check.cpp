@@ -6,7 +6,7 @@
 //   geometry     interleaved chroma is one plane 1 of 2 * ((width + xs) >> xs) samples and no plane 2;
 //   batches      for every YCbCr description into 8-, 16- and 32-bit hosts in each layout, seeded batches of mixed sizes
 //                (odd widths, one-row images, misaligned rows, Y and interleaved chroma planes): every pixel covered exactly
-//                once; an image batched exactly when the block half (DecodeYccIntInterior / DecodeYccF32Interior) takes it;
+//                once; an image batched exactly when the block half (DecodeBlockInterior of DecodeBatchFamilyOf) takes it;
 //                the interleaved plane's alignment restated; records' planes where DecodeWindow puts them (two samples per
 //                interleaved site); interior units of 256 (128 for 32-bit hosts) pixels; one or two launches per chunk.
 // Prints "semiplanar validations=V descriptions=N images=K units=U"; exit code 1 on any failure.
@@ -116,7 +116,7 @@ bool CoveredOnce(const std::vector<int>& count)
     return true;
 }
 
-Interior BlockHalfInterior(const DecodeParams& p) { return p.hostDepth == 32 ? DecodeYccF32Interior(p) : DecodeYccIntInterior(p); }
+Interior BlockHalfInterior(const DecodeParams& p) { return DecodeBlockInterior(DecodeBatchFamilyOf(p), p); }
 
 // The alignment the tuned kernels' pair loads need of the interleaved plane, restated from the loads: twice the planar
 // chroma's bytes per lane, at most 16 (the integer kernels read 16-bit 4:4:4 in two 128-bit loads).
@@ -235,7 +235,8 @@ int main()
                             {
                                 Fail("FillDecodeParams does not carry the layout", descriptions, -1);
                             }
-                            const bool tuned = DecodeBatchTuned(probe);
+                            const DecodeFamily family = DecodeBatchFamilyOf(probe);
+                        const bool tuned = family != DecodeFamily::Generic;
                             const bool expectTuned = alpha != 2 && (hostDepth == 32 ? bitDepth > 8 : true);
                             if (tuned != expectTuned)
                             {
@@ -309,7 +310,7 @@ int main()
                                 {
                                     count[i].assign(static_cast<size_t>(params[i].width) * params[i].rowCount, 0);
                                 }
-                                const int unitPixels = DecodeBatchUnitPixels(hostDepth, AVIFGPU_COLORSPACE_YCBCR);
+                                const int unitPixels = DecodeBatchUnitPixels(hostDepth == 32 ? DecodeFamily::YccF32 : DecodeFamily::YccInt);
                                 int last = -1;
                                 for (const BatchChunk& c : plan.chunks)
                                 {
@@ -389,7 +390,7 @@ int main()
                                 int64_t total = 0;
                                 for (int i = 0; i < n; ++i)
                                 {
-                                    const BatchImagePlan step = PlanBatchDecodeImage(probe, tuned, planeMask, batch[i]);
+                                    const BatchImagePlan step = PlanBatchDecodeImage(probe, family, planeMask, batch[i]);
                                     std::vector<int> covered(static_cast<size_t>(params[i].width) * params[i].rowCount, 0);
                                     const Interior inner = BlockHalfInterior(params[i]);
                                     if (step.status != AVIFGPU_OK || step.interior.width != inner.width || (inner.width > 0 && step.interior.rowCount != inner.rows))

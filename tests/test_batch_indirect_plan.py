@@ -6,7 +6,7 @@ runs -- with the host compiler.  Over seeded random image sets (sizes 0 to 600, 
 misaligned pointers and strides) for every supported encode and decode description it checks that rejected images get
 BAD_PARAM and no record; that an accepted image's records cover every pixel exactly once, judged from their rows
 pointers, with their planes at their first pixel and chroma site; that an image has an interior exactly when the
-single-image predicate of its own block (EncodeRgbIntInterior / DecodeYccIntInterior) takes it, with the strips around
+single-image predicate of its own block (EncodeBlockInterior / DecodeBlockInterior of the batched family) takes it, with the strips around
 it as windows, and is otherwise one whole-image window; and that FindRecord finds the owner of every unit of the
 prefix-summed layout."""
 import ctypes as C

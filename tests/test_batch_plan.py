@@ -4,7 +4,7 @@ PlanDecodeBatch in csrc/host_params.cpp: chunks packed from the per-image step o
 tests/native/batch_plan_check.cpp plans seeded random batches of 1 to 300 images of mixed sizes (1 x 1, widths below 8,
 odd widths and heights, misaligned rows) for every valid encode description, on fake padded planes, and checks that
 every pixel of every image is covered exactly once by an interior, an edge window or a direct call; that an image is
-batched exactly when the single-image launcher's predicate (EncodeRgbIntInterior) takes it; that chunks keep image
+batched exactly when the single-image launcher's predicate (EncodeBlockInterior of EncodeBatchFamilyOf) takes it; that chunks keep image
 order, hold at most 64 images and fit the kernel parameter limit; and that a chunk costs 1 launch, 2 when one of its images has an edge strip; decode batches
 get the coverage, routing and launch checks too."""
 import ctypes as C

@@ -3,7 +3,7 @@ per-image step PlanBatchDecodeImage (the device-described batch's plan kernel) f
 
 tests/native/f32_batch_plan_check.cpp plans seeded random batches of 1 to 300 images -- widths below 4, one-row images,
 misaligned rows and Y planes, unequal Cb / Cr strides -- for every valid YCbCr float-host description, the verified
-divisions off and on, and checks exact pixel coverage, routing against DecodeYccF32Interior, image order, the launches
+divisions off and on, and checks exact pixel coverage, routing against DecodeBlockInterior of DecodeBatchFamilyOf, image order, the launches
 per chunk, plane placement against DecodeWindow, unit counts with the 128-pixel unit and FindRecord over them."""
 import os
 import re

@@ -3,7 +3,7 @@ PlanBatchDecodeImage (the device-described batch's plan kernel) for 8-, 16- and 
 
 tests/native/rgb_batch_plan_check.cpp plans seeded random batches of 1 to 300 images -- widths 1 to 7, 8, 9, 255 to 257
 and random ones, one-row images, misaligned rows and planes -- for every valid planar-RGB description, and checks exact
-pixel coverage, routing against DecodePlanarRgbTuned + DecodePlanarRgbBlockInterior and against a restatement of the
+pixel coverage, routing against the route (DecodeBatchFamilyOf + DecodeBlockInterior) and against a restatement of the
 kernels' alignment rules, image order, the launches per chunk, plane placement against DecodeWindow, unit counts with the
 256-pixel unit and FindRecord over them.  It also checks that YCbCr and monochrome descriptions route as before."""
 import os

@@ -4,8 +4,8 @@ description, plane geometry, and the planning of both batch APIs for them.
 tests/native/semiplanar_plan_check.cpp checks the validation of every layout bit set x colour space x bit depth, that an
 API-9-sized description is accepted as planar, the interleaved plane's geometry, and, for every YCbCr description into 8-,
 16- and 32-bit hosts in each layout, seeded random batches -- odd widths, one-row images, misaligned rows, Y planes and
-interleaved chroma planes -- for exact pixel coverage, routing against the block halves (DecodeYccIntInterior /
-DecodeYccF32Interior) and a restatement of the interleaved plane's alignment, plane placement against DecodeWindow, unit
+interleaved chroma planes -- for exact pixel coverage, routing against the block halves (DecodeBlockInterior of
+DecodeBatchFamilyOf) and a restatement of the interleaved plane's alignment, plane placement against DecodeWindow, unit
 counts, launches per chunk and FindRecord."""
 import os
 import re

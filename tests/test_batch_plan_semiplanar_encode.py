@@ -6,7 +6,7 @@ layout kind x image depth; that an API-10-sized description, ending against an i
 and laid out without a read past its end and means planar; the interleaved plane's geometry and EncodeWindow offsets; the
 integer and float block halves against a restatement of the stores' alignment rule; and, for every 8/16-bit RGB(A)
 description in each layout, seeded random batches -- odd widths, one-row images, misaligned rows, Y planes and interleaved
-chroma planes -- for exact pixel coverage, routing against EncodeRgbIntInterior, plane placement against EncodeWindow, unit
+chroma planes -- for exact pixel coverage, routing against EncodeBlockInterior of EncodeBatchFamilyOf, plane placement against EncodeWindow, unit
 counts, launches per chunk and FindRecord."""
 import ctypes as C
 import mmap

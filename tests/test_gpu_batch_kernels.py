@@ -147,7 +147,7 @@ def ys_of(desc):
 
 
 def eligible(im, ys):
-    """EncodeRgbIntInterior / DecodeYccIntInterior on these aligned buffers: an 8-px group and a (4:2:0) row pair."""
+    """EncodeBlockInterior / DecodeBlockInterior of the batched family on these aligned buffers: an 8-px group and a (4:2:0) row pair."""
     return im.w >= 8 and im.h >= 1 + ys
 
 

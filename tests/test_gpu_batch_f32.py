@@ -20,13 +20,13 @@ import collections
 import itertools
 import os
 
-import numpy as np
 import pytest
 
 from avifgpu import abi
-from test_gpu_batch import CHUNK, SENTINEL, DecImage, ctx, padded, run_decode_batch, whole  # noqa: F401
-from test_gpu_batch_indirect import Empty, Indirect, launches_of, misaligned_rows
-from test_gpu_multipass import pick
+from gpu_harness import ctx  # noqa: F401
+from gpu_harness import (DECODE_FAULTS, DecodeImage, Empty, Indirect, assert_decode_same_as_direct, assert_passes, captured, capture_and_replay,
+                         chunk_launches, direct_launches, host_or_device, launches_of, padded, pick, rejected_records, replay_sets,
+                         run_decode_batch, sm_count)
 
 C444, C422, C420 = abi.CHROMA_444, abi.CHROMA_422, abi.CHROMA_420
 NONE, STRAIGHT = abi.ALPHA_NONE, abi.ALPHA_STRAIGHT
@@ -89,10 +89,10 @@ def unequal_chroma_strides(im):
 
 
 def mix(desc, seed):
-    images = [DecImage(desc, w, h, f"{seed}_{i}", overshoot=True) for i, (w, h) in enumerate(MIXED)]
-    images.append(misaligned_rows(DecImage(desc, 64, 7, f"{seed}_rows", overshoot=True)))
-    images.append(DecImage(desc, 68, 6, f"{seed}_planes", misalign=2, overshoot=True))
-    images.append(unequal_chroma_strides(DecImage(desc, 72, 8, f"{seed}_strides", overshoot=True)))
+    images = [DecodeImage(desc, w, h, f"{seed}_{i}", overshoot=True) for i, (w, h) in enumerate(MIXED)]
+    images.append(DecodeImage(desc, 64, 7, f"{seed}_rows", overshoot=True, rows_offset=4))
+    images.append(DecodeImage(desc, 68, 6, f"{seed}_planes", overshoot=True, planes_misalign=2))
+    images.append(unequal_chroma_strides(DecodeImage(desc, 72, 8, f"{seed}_strides", overshoot=True)))
     return images
 
 
@@ -110,44 +110,6 @@ def has_edge(im):
     return im.w % 4 != 0 or (ys_of(im.desc) and im.h % 2 != 0)
 
 
-def chunk_launches(images):
-    chosen = [im for im in images if eligible(im)]
-    return sum(1 + any(has_edge(im) for im in chosen[i:i + CHUNK]) for i in range(0, len(chosen), CHUNK))
-
-
-def assert_same_as_direct_and_reference(ctx, images, reference, threads=1):
-    """Each image: its rows (padding included) equal a direct call's, and the reference's floats bit for bit."""
-    import torch
-    for im in images:
-        direct = im.alloc()
-        im.direct(ctx, direct)
-        torch.cuda.synchronize()
-        got = whole(im.rows)
-        assert np.array_equal(got, whole(direct)), (im.w, im.h)
-        assert (got[:, im.row_bytes:] == SENTINEL).all(), ("padding overwritten", im.w, im.h)
-        if im.w and im.h:
-            expected = reference.decode(im.desc, im.codes, threads=threads).view(np.uint32)
-            floats = im.rows.cpu().numpy().view(np.uint32)
-            differ = floats != expected
-            assert not differ.any(), ("reference", im.w, im.h, int(differ.sum()), np.argwhere(differ)[0])
-
-
-def captured(ctx, call):
-    """Captures `call` on a side stream, replays it once, and returns the launches captured."""
-    import torch
-    stream = torch.cuda.Stream()
-    stream.wait_stream(torch.cuda.current_stream())
-    graph = torch.cuda.CUDAGraph()
-    before = ctx.launch_count()
-    with torch.cuda.graph(graph, stream=stream):
-        call(stream.cuda_stream)
-    launches = ctx.launch_count() - before
-    graph.replay()
-    torch.cuda.synchronize()
-    del graph
-    return launches
-
-
 # ---- 1. every instantiation, host-described and device-described ------------------------------------------------------------
 
 @pytest.mark.gpu
@@ -161,16 +123,13 @@ def test_host_described_instantiation(checker, port, name, variant, desc):
         if variant == "pq_ieee":
             # before the PQ division is verified: the IEEE-division kernel; every fallback is one generic launch
             launches = captured(fresh, lambda stream: run_decode_batch(fresh, desc, images, stream))
-            assert launches == chunk_launches(images) + len(fallbacks)
+            assert launches == chunk_launches(images, eligible, has_edge) + len(fallbacks)
         else:
             fresh.prepare_decode(desc)
-            direct = 0
-            for im in fallbacks:  # into the image's own rows: their alignment is part of its route
-                before = fresh.launch_count()
-                im.direct(fresh, im.rows)
-                direct += fresh.launch_count() - before
-            assert launches_of(fresh, lambda: run_decode_batch(fresh, desc, images)) == chunk_launches(images) + direct
-        assert_same_as_direct_and_reference(fresh, images, pick(checker, port, True))
+            # into the image's own rows: their alignment is part of its route
+            direct = direct_launches(fresh, fallbacks, into=lambda im: im.rows)
+            assert launches_of(fresh, lambda: run_decode_batch(fresh, desc, images)) == chunk_launches(images, eligible, has_edge) + direct
+        assert_decode_same_as_direct(fresh, images, pick(checker, port, True))
 
 
 @pytest.mark.gpu
@@ -187,15 +146,10 @@ def test_device_described_instantiation(checker, port, name, variant, desc):
             fresh.prepare_decode(desc)
             assert launches_of(fresh, lambda: batch.decode(fresh, desc)) == 3
         assert (batch.statuses()[:len(images) + 1] == 0).all()
-        assert_same_as_direct_and_reference(fresh, images, pick(checker, port, True))
+        assert_decode_same_as_direct(fresh, images, pick(checker, port, True))
 
 
 # ---- 2. several passes of both grids -------------------------------------------------------------------------------------------
-
-def sm_count():
-    import torch
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
 
 def interior_units(w, h, ys):
     """BatchInteriorUnits of an image's aligned interior with the 128-pixel unit."""
@@ -216,72 +170,31 @@ def test_multipass(ctx, checker, port, api):
     (kernels_batch.cu): both walk their units at least twice."""
     desc = hdr("pq", C420, STRAIGHT, 12, "2020", 0)
     n, w, h = 64, 515, 263
-    sms = sm_count()
-    assert n * interior_units(w, h, 1) >= 2 * sms * 2 * 8
-    assert n * edge_units(w, h, 1) >= 2 * sms * 16
-    images = [DecImage(desc, w, h, f"f32_multipass_{api}_{i}", overshoot=True) for i in range(n)]
+    sms = sm_count(ctx)
+    assert_passes("ycc_f32_interior", n * interior_units(w, h, 1), sms)
+    assert_passes("decode_edge", n * edge_units(w, h, 1), sms)
+    images = [DecodeImage(desc, w, h, f"f32_multipass_{api}_{i}", overshoot=True) for i in range(n)]
     ctx.prepare_decode(desc)
-    if api == "host":
-        assert launches_of(ctx, lambda: run_decode_batch(ctx, desc, images)) == 2
-    else:
-        batch = Indirect(n)
-        batch.load(images)
-        assert launches_of(ctx, lambda: batch.decode(ctx, desc)) == 3
-        assert (batch.statuses() == 0).all()
-    assert_same_as_direct_and_reference(ctx, images, pick(checker, port, True), threads=os.cpu_count())
+    host_or_device(ctx, desc, "decode", api, images,
+                   lambda done: assert_decode_same_as_direct(ctx, done, pick(checker, port, True), threads=os.cpu_count()))
 
 
 # ---- 3. device-described specifics ------------------------------------------------------------------------------------------------
 
 @pytest.mark.gpu
 def test_rejected_images_keep_their_outputs(ctx, checker, port):
-    import avifgpu
     desc = hdr("hlg", C422, STRAIGHT, 10, "709", 1)
-    images = [DecImage(desc, w, h, f"f32_bad_{i}") for i, (w, h) in enumerate([(64, 16), (37, 9), (64, 4), (8, 2), (130, 5), (7, 5)])]
-    records = avifgpu.batch_images_from_tensors([im.record() for im in images])
-    records[1].rows = None
-    records[3].planes.data[3] = None
-    records[5].width = -1
-    batch = Indirect(6)
-    batch.load(records)
+    images = [DecodeImage(desc, w, h, f"f32_bad_{i}") for i, (w, h) in enumerate([(64, 16), (37, 9), (64, 4), (8, 2), (130, 5), (7, 5)])]
     ctx.prepare_decode(desc)
-    assert launches_of(ctx, lambda: batch.decode(ctx, desc)) == 3
-    bad = abi.ERR_BAD_PARAM
-    assert list(batch.statuses()) == [0, bad, 0, bad, 0, bad]
-    import torch
-    torch.cuda.synchronize()
-    assert all((whole(images[i].rows) == SENTINEL).all() for i in (1, 3, 5))
-    assert_same_as_direct_and_reference(ctx, [images[i] for i in (0, 2, 4)], pick(checker, port, True))
+    rejected_records(ctx, desc, "decode", images, DECODE_FAULTS, lambda good: assert_decode_same_as_direct(ctx, good, pick(checker, port, True)))
 
 
 def replay(ctx, desc, tag, reference, prepare):
     """One capture of a device-described call, replayed on 1, 64 and 256 images at new addresses."""
-    import torch
-    batch = Indirect(256)
-    stream = torch.cuda.Stream()
-    with torch.cuda.stream(stream):
-        batch.load([DecImage(desc, 64, 16, f"{tag}_capture")])
-    if prepare:
-        ctx.prepare_decode(desc)
-    stream.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    before = ctx.launch_count()
-    with torch.cuda.graph(graph, stream=stream):
-        batch.decode(ctx, desc, stream.cuda_stream)
-    assert ctx.launch_count() - before == 3
-    sets = [[DecImage(desc, 96, 10, f"{tag}_one", overshoot=True)],
-            [DecImage(desc, 136, 34, f"{tag}_64_{i}", overshoot=True) for i in range(64)],
-            [DecImage(desc, *MIXED[i % len(MIXED)], f"{tag}_256_{i}", overshoot=True) for i in range(256)]]
-    for images in sets:
-        with torch.cuda.stream(stream):
-            batch.load(images)
-            before = ctx.launch_count()
-            graph.replay()
-        torch.cuda.synchronize()
-        assert ctx.launch_count() == before
-        assert (batch.statuses()[:len(images)] == 0).all()
-        assert_same_as_direct_and_reference(ctx, images, reference, threads=os.cpu_count())
-    del graph
+    sets = replay_sets(lambda w, h, seed: DecodeImage(desc, w, h, seed, overshoot=True), tag, (136, 34), MIXED)
+    capture_and_replay(ctx, desc, "decode", DecodeImage(desc, 64, 16, f"{tag}_capture"), sets,
+                       lambda images: assert_decode_same_as_direct(ctx, images, reference, threads=os.cpu_count()),
+                       (lambda: ctx.prepare_decode(desc)) if prepare else None)
 
 
 @pytest.mark.gpu

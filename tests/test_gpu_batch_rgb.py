@@ -18,15 +18,14 @@ compiled reference.  For 32-bit hosts the reference indexes its 2^depth table wi
 maximum are out of its contract: those images are held to the direct call only (test_gpu_multipass.table_planes)."""
 import os
 
-import numpy as np
 import pytest
 
 import cases
 from avifgpu import abi
-from test_gpu_batch import CHUNK, SENTINEL, DecImage, ctx, padded, run_decode_batch, whole  # noqa: F401
-from test_gpu_batch_f32 import captured
-from test_gpu_batch_indirect import Empty, Indirect, launches_of
-from test_gpu_multipass import pick, rgb32_nclx
+from gpu_harness import ctx  # noqa: F401
+from gpu_harness import (DECODE_FAULTS, DecodeImage, Empty, Indirect, assert_decode_same_as_direct, assert_passes, capture_and_replay, captured,
+                         chunk_launches, direct_launches, host_or_device, launches_of, pick, rejected_records, replay_sets, rgb32_nclx,
+                         run_decode_batch, sm_count)
 
 NONE, STRAIGHT, PREMUL = abi.ALPHA_NONE, abi.ALPHA_STRAIGHT, abi.ALPHA_PREMULTIPLIED
 
@@ -67,23 +66,14 @@ def overshoot_ok(desc):
     return desc.host_depth != 32
 
 
-def offset_rows(im, offset):
-    """Moves a decode image's destination rows `offset` bytes off their alignment, keeping the row stride."""
-    import torch
-    stride = padded(im.row_bytes)
-    backing = torch.full(((im.h + 1) * stride,), SENTINEL, dtype=torch.uint8, device="cuda")
-    im.rows = backing[offset:offset + im.h * stride].view(im.h, stride)[:, :im.row_bytes]
-    return im
-
-
 def mix(desc, seed):
     over = overshoot_ok(desc)
-    images = [DecImage(desc, w, h, f"{seed}_{i}", overshoot=over) for i, (w, h) in enumerate(MIXED)]
-    images.append(offset_rows(DecImage(desc, 64, 7, f"{seed}_rows4", overshoot=over), 4))
-    images.append(offset_rows(DecImage(desc, 72, 5, f"{seed}_rows8", overshoot=over), 8))
-    images.append(DecImage(desc, 68, 6, f"{seed}_planes", misalign=2, overshoot=over))
+    images = [DecodeImage(desc, w, h, f"{seed}_{i}", overshoot=over) for i, (w, h) in enumerate(MIXED)]
+    images.append(DecodeImage(desc, 64, 7, f"{seed}_rows4", overshoot=over, rows_offset=4))
+    images.append(DecodeImage(desc, 72, 5, f"{seed}_rows8", overshoot=over, rows_offset=8))
+    images.append(DecodeImage(desc, 68, 6, f"{seed}_planes", overshoot=over, planes_misalign=2))
     if not over:
-        over_image = DecImage(desc, 136, 3, f"{seed}_over", overshoot=True)
+        over_image = DecodeImage(desc, 136, 3, f"{seed}_over", overshoot=True)
         over_image.direct_only = True
         images.append(over_image)
     return images
@@ -102,43 +92,6 @@ def has_edge(im):
     return im.w % 8 != 0
 
 
-def chunk_launches(images):
-    chosen = [im for im in images if eligible(im)]
-    return sum(1 + any(has_edge(im) for im in chosen[i:i + CHUNK]) for i in range(0, len(chosen), CHUNK))
-
-
-def bits(a):
-    return a.view(np.uint32) if a.dtype == np.float32 else a
-
-
-def assert_same_as_direct_and_reference(ctx, images, reference, threads=1):
-    """Each image: its rows (padding included) equal a direct call's, and the reference's output bit for bit."""
-    import torch
-    for im in images:
-        direct = im.alloc()
-        im.direct(ctx, direct)
-        torch.cuda.synchronize()
-        got = whole(im.rows)
-        assert np.array_equal(got, whole(direct)), (im.w, im.h)
-        assert (got[:, im.row_bytes:] == SENTINEL).all(), ("padding overwritten", im.w, im.h)
-        if im.w and im.h and not getattr(im, "direct_only", False):
-            expected = bits(reference.decode(im.desc, im.codes, threads=threads))
-            values = bits(im.rows.cpu().numpy().view(abi.host_dtype(im.desc.host_depth)))
-            differ = values != expected
-            assert not differ.any(), ("reference", im.w, im.h, int(differ.sum()), np.argwhere(differ)[0])
-
-
-def direct_launches(ctx, images):
-    """The launches of one direct call of each image, made into the image's own rows (their alignment is part of its
-    route); the batch overwrites them with the same bits."""
-    total = 0
-    for im in images:
-        before = ctx.launch_count()
-        im.direct(ctx, im.rows)
-        total += ctx.launch_count() - before
-    return total
-
-
 # ---- 1. every instantiation, host-described and device-described ------------------------------------------------------------
 
 @pytest.mark.gpu
@@ -150,9 +103,10 @@ def test_host_described_instantiation(ctx, checker, port, name, desc):
     if desc.host_depth == 8 and desc.alpha_state == NONE:
         assert eligible(images[len(MIXED) + 1])  # RGB8 rows 8 bytes off 16 stay tuned
     ctx.prepare_decode(desc)
-    direct = direct_launches(ctx, fallbacks)
-    assert launches_of(ctx, lambda: run_decode_batch(ctx, desc, images)) == chunk_launches(images) + direct
-    assert_same_as_direct_and_reference(ctx, images, pick(checker, port, True))
+    # into the image's own rows: their alignment is part of its route
+    direct = direct_launches(ctx, fallbacks, into=lambda im: im.rows)
+    assert launches_of(ctx, lambda: run_decode_batch(ctx, desc, images)) == chunk_launches(images, eligible, has_edge) + direct
+    assert_decode_same_as_direct(ctx, images, pick(checker, port, True))
 
 
 @pytest.mark.gpu
@@ -164,24 +118,19 @@ def test_device_described_instantiation(ctx, checker, port, name, desc):
     ctx.prepare_decode(desc)
     assert launches_of(ctx, lambda: batch.decode(ctx, desc)) == 3
     assert (batch.statuses()[:len(images) + 1] == 0).all()
-    assert_same_as_direct_and_reference(ctx, images, pick(checker, port, True))
+    assert_decode_same_as_direct(ctx, images, pick(checker, port, True))
 
 
 @pytest.mark.gpu
 def test_chunks_of_many_images(ctx, checker, port):
     """130 images: three chunks, the last two with right strips, in one host-described call."""
     desc = KERNELS[3][1]
-    images = [DecImage(desc, 64 if i < 64 else 67, 3, f"rgb_chunks_{i}", overshoot=True) for i in range(130)]
+    images = [DecodeImage(desc, 64 if i < 64 else 67, 3, f"rgb_chunks_{i}", overshoot=True) for i in range(130)]
     assert launches_of(ctx, lambda: run_decode_batch(ctx, desc, images)) == 1 + 2 + 2
-    assert_same_as_direct_and_reference(ctx, images, pick(checker, port, True))
+    assert_decode_same_as_direct(ctx, images, pick(checker, port, True))
 
 
 # ---- 2. several passes of both grids -------------------------------------------------------------------------------------------
-
-def sm_count():
-    import torch
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("api", ["host", "device"])
@@ -193,19 +142,13 @@ def test_multipass(ctx, checker, port, api, name):
     desc = dict(KERNELS)[name]
     n, w, h = 64, 525, 300
     assert -(-(w & ~7) // 256) == 3 and w % 8
-    sms = sm_count()
-    assert n * 3 * h >= 2 * sms * 16 * 8
-    assert n * h >= 2 * sms * 16
-    images = [DecImage(desc, w, h, f"rgb_multipass_{api}_{name}_{i}", overshoot=overshoot_ok(desc)) for i in range(n)]
+    sms = sm_count(ctx)
+    assert_passes("rgb_f32_interior" if desc.host_depth == 32 else "rgb_int_interior", n * 3 * h, sms)
+    assert_passes("decode_edge", n * h, sms)
+    images = [DecodeImage(desc, w, h, f"rgb_multipass_{api}_{name}_{i}", overshoot=overshoot_ok(desc)) for i in range(n)]
     ctx.prepare_decode(desc)
-    if api == "host":
-        assert launches_of(ctx, lambda: run_decode_batch(ctx, desc, images)) == 2
-    else:
-        batch = Indirect(n)
-        batch.load(images)
-        assert launches_of(ctx, lambda: batch.decode(ctx, desc)) == 3
-        assert (batch.statuses() == 0).all()
-    assert_same_as_direct_and_reference(ctx, images, pick(checker, port, True), threads=os.cpu_count())
+    host_or_device(ctx, desc, "decode", api, images,
+                   lambda done: assert_decode_same_as_direct(ctx, done, pick(checker, port, True), threads=os.cpu_count()))
 
 
 # ---- 3. device-described specifics ------------------------------------------------------------------------------------------------
@@ -213,23 +156,10 @@ def test_multipass(ctx, checker, port, api, name):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["h8_rgba", "f32_rgba_hlg_ootf_d10"])
 def test_rejected_images_keep_their_outputs(ctx, checker, port, name):
-    import avifgpu
-    import torch
     desc = dict(KERNELS)[name]
-    images = [DecImage(desc, w, h, f"rgb_bad_{name}_{i}") for i, (w, h) in enumerate([(64, 16), (37, 9), (64, 4), (8, 2), (130, 5), (7, 5)])]
-    records = avifgpu.batch_images_from_tensors([im.record() for im in images])
-    records[1].rows = None
-    records[3].planes.data[3] = None
-    records[5].width = -1
-    batch = Indirect(6)
-    batch.load(records)
+    images = [DecodeImage(desc, w, h, f"rgb_bad_{name}_{i}") for i, (w, h) in enumerate([(64, 16), (37, 9), (64, 4), (8, 2), (130, 5), (7, 5)])]
     ctx.prepare_decode(desc)
-    assert launches_of(ctx, lambda: batch.decode(ctx, desc)) == 3
-    bad = abi.ERR_BAD_PARAM
-    assert list(batch.statuses()) == [0, bad, 0, bad, 0, bad]
-    torch.cuda.synchronize()
-    assert all((whole(images[i].rows) == SENTINEL).all() for i in (1, 3, 5))
-    assert_same_as_direct_and_reference(ctx, [images[i] for i in (0, 2, 4)], pick(checker, port, True))
+    rejected_records(ctx, desc, "decode", images, DECODE_FAULTS, lambda good: assert_decode_same_as_direct(ctx, good, pick(checker, port, True)))
 
 
 @pytest.mark.gpu
@@ -237,35 +167,15 @@ def test_rejected_images_keep_their_outputs(ctx, checker, port, name):
 def test_captured_call_replays_new_image_sets(checker, port, name):
     """One capture of a device-described call, replayed on 1, 64 and 256 images at new addresses."""
     import avifgpu
-    import torch
     desc = dict(KERNELS)[name]
     over = overshoot_ok(desc)
     reference = pick(checker, port, True)
+    tag = f"rgb_replay_{name}"
+    sets = replay_sets(lambda w, h, seed: DecodeImage(desc, w, h, seed, overshoot=over), tag, (136, 34), MIXED)
     with avifgpu.Context(0) as fresh:
-        batch = Indirect(256)
-        stream = torch.cuda.Stream()
-        with torch.cuda.stream(stream):
-            batch.load([DecImage(desc, 64, 16, f"rgb_replay_{name}_capture")])
-        fresh.prepare_decode(desc)
-        stream.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        before = fresh.launch_count()
-        with torch.cuda.graph(graph, stream=stream):
-            batch.decode(fresh, desc, stream.cuda_stream)
-        assert fresh.launch_count() - before == 3
-        sets = [[DecImage(desc, 96, 10, f"rgb_replay_{name}_one", overshoot=over)],
-                [DecImage(desc, 136, 34, f"rgb_replay_{name}_64_{i}", overshoot=over) for i in range(64)],
-                [DecImage(desc, *MIXED[i % len(MIXED)], f"rgb_replay_{name}_256_{i}", overshoot=over) for i in range(256)]]
-        for images in sets:
-            with torch.cuda.stream(stream):
-                batch.load(images)
-                before = fresh.launch_count()
-                graph.replay()
-            torch.cuda.synchronize()
-            assert fresh.launch_count() == before
-            assert (batch.statuses()[:len(images)] == 0).all()
-            assert_same_as_direct_and_reference(fresh, images, reference, threads=os.cpu_count())
-        del graph
+        capture_and_replay(fresh, desc, "decode", DecodeImage(desc, 64, 16, f"{tag}_capture"), sets,
+                           lambda images: assert_decode_same_as_direct(fresh, images, reference, threads=os.cpu_count()),
+                           lambda: fresh.prepare_decode(desc))
 
 
 @pytest.mark.gpu
@@ -280,7 +190,7 @@ def test_captured_host_described_call_replays_like_direct_calls(checker, port):
         run_decode_batch(fresh, desc, images)
         calls = fresh.launch_count() - before
         assert captured(fresh, lambda stream: run_decode_batch(fresh, desc, images, stream)) == calls
-        assert_same_as_direct_and_reference(fresh, images, pick(checker, port, True))
+        assert_decode_same_as_direct(fresh, images, pick(checker, port, True))
 
 
 # ---- 4. what stays as it was -----------------------------------------------------------------------------------------------------
@@ -289,11 +199,11 @@ def test_captured_host_described_call_replays_like_direct_calls(checker, port):
 @pytest.mark.parametrize("host_depth", [16, 32])
 def test_premultiplied_planar_rgb_keeps_its_direct_calls(ctx, checker, port, host_depth):
     desc = rgb(16, 10, PREMUL) if host_depth == 16 else rgb(32, 12, PREMUL, "pq")
-    images = [DecImage(desc, w, h, f"rgb_premul_{host_depth}_{i}") for i, (w, h) in enumerate(MIXED)]
+    images = [DecodeImage(desc, w, h, f"rgb_premul_{host_depth}_{i}") for i, (w, h) in enumerate(MIXED)]
     ctx.prepare_decode(desc)
-    direct = direct_launches(ctx, images)
+    direct = direct_launches(ctx, images, into=lambda im: im.rows)
     assert launches_of(ctx, lambda: run_decode_batch(ctx, desc, images)) == direct
-    assert_same_as_direct_and_reference(ctx, images, pick(checker, port, True))
+    assert_decode_same_as_direct(ctx, images, pick(checker, port, True))
 
 
 @pytest.mark.gpu

@@ -13,10 +13,9 @@ import pytest
 import cases
 import encode_spec
 from avifgpu import abi
-from test_gpu_batch import Image, ctx, run_batch  # noqa: F401
-from test_gpu_batch_indirect import Indirect, launches_of
-from test_gpu_batch_kernels import ENCODE_KERNELS, MIXED, assert_batched, ys_of
-from test_gpu_multipass import SENTINEL, Padded, planes_struct, run_counted, strips
+from gpu_harness import ctx  # noqa: F401
+from gpu_harness import (ENCODE_KERNELS, MIXED, SENTINEL, EncodeImage, Indirect, Padded, assert_batched, launches_of, planes_struct, run_batch,
+                         run_counted, strips, whole, ys_of)
 
 pytestmark = pytest.mark.gpu
 
@@ -121,24 +120,13 @@ def test_clip_kernel(gpu, gpu_exact, ref, depth, chroma, down, matrix):
 
 @pytest.mark.parametrize("name,desc", ENCODE_KERNELS, ids=[c[0] for c in ENCODE_KERNELS])
 def test_int_planar_kernel(gpu, ref, name, desc):
-    """Host depth, plane bytes, channels / premultiply and chroma as test_gpu_batch_kernels.ENCODE_KERNELS spreads them,
+    """Host depth, plane bytes, channels / premultiply and chroma as gpu_harness.ENCODE_KERNELS spreads them,
     with its matrices, down-filters and 10 / 12-bit planes; 16-bit random rows carry samples above 32768, extreme rows
     65535."""
     check_all_inputs(ref, ((gpu, True),), desc.copy(width=W, height=H), f"spec_int_{name}", 8)
 
 
 # ---- the batched integer kernels, both APIs -------------------------------------------------------------------------------------
-
-class ExtremeImage(Image):
-    """A batch image whose host rows are extreme_rows()."""
-
-    def __init__(self, desc, w, h, seed):
-        import torch
-        super().__init__(desc, w, h, seed)
-        self.host = encode_spec.extreme_rows(self.desc, w, h, f"spec_batch_{seed}_{w}x{h}")
-        if w and h:
-            self.rows.copy_(torch.from_numpy(self.host.view(np.uint8).reshape(h, -1)).cuda())
-
 
 BATCH_SIZES = MIXED + [(W, H), (520, 9), (16, 2)]
 
@@ -150,15 +138,16 @@ def assert_images_match(ref, images):
             encode_spec.assert_matches(ref, im.desc, im.host, got, f"{im.w} x {im.h} image")
             for p in im.planes:
                 if p is not None:
-                    assert (p.as_strided((p.shape[0], p.stride(0)), (p.stride(0), 1))[:, p.shape[1]:] == SENTINEL).all()
+                    assert (whole(p)[:, p.shape[1]:] == SENTINEL).all()
 
 
 @pytest.mark.parametrize("api", ["device", "indirect"])
 @pytest.mark.parametrize("name,desc", ENCODE_KERNELS, ids=[c[0] for c in ENCODE_KERNELS])
-def test_batch_kernels(ctx, ref, name, desc, api):  # noqa: F811
+def test_batch_kernels(ctx, ref, name, desc, api):
     """Batches of extreme images of several sizes: aligned interiors, right strips, odd 4:2:0 heights, and images too
     small for the interior kernel."""
-    images = [ExtremeImage(desc, w, h, f"{name}_{i}") for i, (w, h) in enumerate(BATCH_SIZES)]
+    # host rows: extreme_rows() of f"spec_batch_{name}_{i}_{w}x{h}"
+    images = [EncodeImage(desc, w, h, f"{name}_{i}_{w}x{h}", prefix="spec_batch_", extreme=True) for i, (w, h) in enumerate(BATCH_SIZES)]
     if api == "device":
         assert_batched(ctx, lambda: run_batch(ctx, desc, images), images, ys_of(desc))
     else:

@@ -23,33 +23,13 @@ import pytest
 
 import cases
 from avifgpu import abi
+from gpu_harness import ctx  # noqa: F401
+from gpu_harness import SENTINEL, capture, pick
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 W, H = 261, 9  # a right strip for every tuned launcher (4- and 8-pixel groups) and an odd last 4:2:0 row
-SENTINEL = 0xCD
-
-
-@pytest.fixture
-def ctx():
-    import avifgpu
-    context = avifgpu.Context(0)
-    yield context
-    context.close()
-
-
-def pick(checker, port, reference_ok):
-    """test_gpu_parity.pick(): the compiled reference wherever the reference has the path; a missing oracle/_ref is a
-    failure unless AVIFGPU_ALLOW_RESTATEMENT=1."""
-    if not reference_ok:
-        return port
-    if checker.kind != "reference":
-        if os.environ.get("AVIFGPU_ALLOW_RESTATEMENT") == "1":
-            return port
-        pytest.fail("oracle/_ref/libavifref.so is not loaded: build it where the reference tree is mounted (make -C oracle) -- "
-                    "or set AVIFGPU_ALLOW_RESTATEMENT=1 to compare against the restatement")
-    return checker
 
 
 # ---- the routes ---------------------------------------------------------------------------------------------------------
@@ -202,16 +182,6 @@ def same(expected, got):
             assert not differ.any(), f"output {k}: {int(differ.sum())} of {e.size} values differ; first at {np.argwhere(differ)[0]}"
 
 
-def capture(ctx, io):
-    """Records one call into a CUDA graph (global capture mode); returns (graph, launches counted at capture)."""
-    import torch
-    graph = torch.cuda.CUDAGraph()
-    before = ctx.launch_count()
-    with torch.cuda.graph(graph):
-        io.call(ctx, torch.cuda.current_stream().cuda_stream)
-    return graph, ctx.launch_count() - before
-
-
 def replay(ctx, graph):
     import torch
     before = ctx.launch_count()
@@ -238,7 +208,7 @@ def test_prepared_capture(ctx, checker, port, name):
     io = DeviceIO(case)
     io.load(case.inputs("capture"))
     case.prepare(ctx, io)
-    graph, captured = capture(ctx, io)
+    graph, captured = capture(ctx, lambda stream: io.call(ctx, stream))
     assert captured >= 2, f"{captured} launch(es) captured: the tuned kernel leaves a right strip to the generic one"
     if name == "flat_pq_420":
         assert captured == 3, "tuned kernel, right strip, odd last row"
@@ -277,7 +247,7 @@ def test_unprepared_capture(ctx, checker, port, kind):
         ctx.set_table_autobuild(0)  # a direct call would build the table at once
     io = DeviceIO(case)
     io.load(case.inputs("capture"))
-    graph, captured = capture(ctx, io)
+    graph, captured = capture(ctx, lambda stream: io.call(ctx, stream))
     assert captured >= 1
     inputs = case.inputs("first")
     io.load(inputs)
@@ -303,7 +273,7 @@ def test_graph_outlives_later_preparation(ctx, checker, port):
     io = DeviceIO(case)
     io.load(case.inputs("capture"))
     case.prepare(ctx, io)
-    graph, _ = capture(ctx, io)
+    graph, _ = capture(ctx, lambda stream: io.call(ctx, stream))
     inputs = case.inputs("first")
     io.load(inputs)
     replay(ctx, graph)

@@ -19,6 +19,7 @@ import pytest
 
 import cases
 from avifgpu import abi
+from gpu_harness import Padded, pick, planes_struct, rgb32_nclx, run_counted, sm_count, strips
 
 pytestmark = pytest.mark.gpu
 
@@ -42,11 +43,6 @@ GRID_CAPS = {
     "table": (256, 8, 1, "kernels_fast_decode_table.cu:146-156 (threads; cudaOccupancyMaxActiveBlocksPerMultiprocessor)"),
     "ycc_int": (8, 3, 1, "kernels_fast_decode_int.cu:377-383 (warps; kWarps = 8, kBlocksPerSm = 3)"),
 }
-
-
-def sm_count(ctx):
-    import torch
-    return torch.cuda.get_device_properties(torch.device("cuda", ctx.device)).multi_processor_count
 
 
 def workers(kernel, units, sms):
@@ -96,69 +92,7 @@ def rows_for(kernel, units_per_row_unit, sms, rows_per_unit=1, factor=1.5, odd=F
     return h | 1 if odd else h
 
 
-# ---- the checker ---------------------------------------------------------------------------------------------------------
-
-def pick(checker, port, reference_ok):
-    """test_gpu_parity.pick(): the compiled reference wherever the reference has the path; a missing oracle/_ref is a
-    failure unless AVIFGPU_ALLOW_RESTATEMENT=1."""
-    if not reference_ok:
-        return port
-    if checker.kind != "reference":
-        if os.environ.get("AVIFGPU_ALLOW_RESTATEMENT") == "1":
-            return port
-        pytest.fail("oracle/_ref/libavifref.so is not loaded: build it where the reference tree is mounted (make -C oracle) -- "
-                    "or set AVIFGPU_ALLOW_RESTATEMENT=1 to compare against the restatement")
-    return checker
-
-
-# ---- device buffers with 256-byte row strides and a sentinel in the padding -----------------------------------------------
-
-SENTINEL = 0xCD
-
-
-class Padded:
-    """A (rows, cols) array of `dtype` on the device, each row 256-byte aligned, the padding filled with SENTINEL."""
-
-    def __init__(self, dev, rows, cols, dtype, source=None):
-        import torch
-        self.dtype = np.dtype(dtype)
-        self.payload = cols * self.dtype.itemsize
-        self.stride = -(-self.payload // 256) * 256
-        self.bytes = torch.full((rows, self.stride), SENTINEL, dtype=torch.uint8, device=dev)
-        if source is not None:
-            assert source.shape == (rows, cols) and source.dtype == self.dtype
-            self.bytes[:, :self.payload] = torch.from_numpy(np.ascontiguousarray(source).view(np.uint8).reshape(rows, self.payload)).to(dev)
-        self.view = self.bytes[:, :self.payload]
-        self.shape = (rows, cols)
-
-    def ptr(self):
-        return self.bytes.data_ptr()
-
-    def host(self):
-        return self.view.contiguous().cpu().numpy().view(self.dtype).reshape(self.shape)
-
-    def padding_intact(self):
-        return self.payload == self.stride or bool((self.bytes[:, self.payload:] == SENTINEL).all().item())
-
-
-def planes_struct(padded):
-    planes = abi.Planes()
-    for k, p in enumerate(padded):
-        planes.data[k] = None if p is None else p.ptr()
-        planes.stride[k] = 0 if p is None else p.stride
-    return planes
-
-
-def run_counted(ctx, call):
-    """Runs `call` twice and returns the launches of the second: table builds and first-use checks happen in the first."""
-    import torch
-    call()
-    torch.cuda.synchronize()
-    before = ctx.launch_count()
-    call()
-    torch.cuda.synchronize()
-    return ctx.launch_count() - before
-
+# ---- device calls on buffers with 256-byte row strides and a sentinel in the padding (gpu_harness.Padded) -------------------
 
 def encode_and_compare(gpu, reference, desc, rows, launches, beyond=None):
     """rows: host array; `launches` = what the tuned launcher makes (1 + strips).  beyond: for Gray16 hosts in the
@@ -214,11 +148,6 @@ def decode_and_compare(gpu, reference, desc, planes, launches, nan_payloads_free
         differ = expected != got
     assert not differ.any(), f"{int(differ.sum())} of {expected.size} samples differ; first at {np.argwhere(differ)[0]}"
     assert out.padding_intact(), "wrote into the row padding"
-
-
-def strips(width, group, odd_rows=False):
-    """Launches of a tuned launcher: the kernel, a right strip when width % group != 0, an odd last 4:2:0 row."""
-    return 1 + (width % group != 0) + bool(odd_rows)
 
 
 _inputs = {}
@@ -402,12 +331,6 @@ def test_ycc_int_decode_multipass(gpu, checker, port, chroma, bit_depth, host_de
 
 
 # ---- float hosts, monochrome and planar-RGB decode (kernels_fast_decode_table.cu) ----------------------------------------------
-
-def rgb32_nclx(transfer_name):
-    nclx = {"pq": cases.NCLX_2020_PQ, "hlg": cases.NCLX_2020_HLG, "428": cases.NCLX_2020_428}[transfer_name]()
-    nclx.matrix_coefficients = abi.MATRIX_GBR
-    return nclx
-
 
 TABLE_CONFIGS = [("rgb", "pq", dict(pq_peak_nits=80)), ("rgb", "pq", dict(pq_peak_nits=1000)), ("rgb", "pq", dict(pq_peak_nits=10000)),
                  ("rgb", "hlg", dict(hlg_apply_ootf=1)), ("rgb", "hlg", dict(hlg_apply_ootf=0)), ("rgb", "428", dict()),

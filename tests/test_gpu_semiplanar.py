@@ -24,10 +24,9 @@ import pytest
 
 import cases
 from avifgpu import abi
-from test_gpu_batch import SENTINEL, ctx, padded, run_decode_batch, whole  # noqa: F401
-from test_gpu_batch_f32 import captured
-from test_gpu_batch_indirect import Indirect, launches_of
-from test_gpu_multipass import pick
+from gpu_harness import ctx  # noqa: F401
+from gpu_harness import (SENTINEL, DecodeImage, Indirect, assert_passes, capture_and_replay, captured, chunk_launches, host_or_device, launches_of,
+                         pick, replay_sets, run_decode_batch, sm_count, whole)
 
 C444, C422, C420 = abi.CHROMA_444, abi.CHROMA_422, abi.CHROMA_420
 NONE, STRAIGHT = abi.ALPHA_NONE, abi.ALPHA_STRAIGHT
@@ -75,101 +74,18 @@ def test_case_table_is_complete():
 
 # ---- images -------------------------------------------------------------------------------------------------------------
 
-def planar_of(desc):
-    d = abi.DecodeDesc.from_buffer_copy(desc)
-    d.source_layout = abi.SOURCE_PLANAR
-    return d
-
-
-class SemiImage:
-    """Seeded codes, the source planes of `desc`'s layout made from them (random low bits under MSB-aligned codes) as byte
-    tensors on the GPU, and sentinel-padded destination rows."""
-
-    def __init__(self, desc, w, h, seed, chroma_misalign=0, low_bits_seed=None):
-        import torch
-        self.w, self.h = w, h
-        d = self.desc = abi.DecodeDesc.from_buffer_copy(desc)
-        d.width, d.height = w, h
-        self.planar_desc = planar_of(d)
-        layout = d.source_layout
-        msb = bool(layout & MSB)
-        rng = cases.rng_for(f"semi_{seed}_{w}x{h}")
-        # an MSB-aligned sample holds no code above the maximum; a low-bit one does
-        self.codes = cases.code_planes(rng, self.planar_desc, overshoot=not msb)
-        shift = 16 - d.bit_depth
-        noise = np.random.default_rng(low_bits_seed if low_bits_seed is not None else rng.integers(1 << 31))
-        source = []
-        for c in self.codes:
-            if c is None or not msb:
-                source.append(c)
-            else:
-                source.append(((c.astype(np.uint32) << shift) | noise.integers(0, 1 << shift, c.shape)).astype(np.uint16))
-        if layout & NV:
-            pairs = np.empty((source[1].shape[0], 2 * source[1].shape[1]), dtype=source[1].dtype)
-            pairs[:, 0::2], pairs[:, 1::2] = source[1], source[2]
-            source[1], source[2] = pairs, None
-        self.planes = []
-        for k, s in enumerate(source):
-            if s is None:
-                self.planes.append(None)
-                continue
-            raw = np.ascontiguousarray(s).view(np.uint8)
-            misalign = chroma_misalign if k == 1 else 0
-            backing = torch.zeros((max(raw.shape[0], 1), padded(raw.shape[1]) + misalign), dtype=torch.uint8, device="cuda")
-            plane = backing[:raw.shape[0], misalign:misalign + raw.shape[1]]
-            plane.copy_(torch.from_numpy(raw).cuda())
-            self.planes.append(plane)
-        self.row_bytes = w * abi.decode_host_channels(d) * d.host_depth // 8
-        self.rows = self.alloc()
-
-    def alloc(self):
-        import torch
-        return torch.full((max(self.h, 1), padded(self.row_bytes)), SENTINEL, dtype=torch.uint8, device="cuda")[:self.h, :self.row_bytes]
-
-    def record(self):
-        return (self.w, self.h, self.rows, self.planes)
-
-    def direct(self, ctx, rows, y0=0, nrows=None, stream=0):
-        import avifgpu
-        nrows = self.h - y0 if nrows is None else nrows
-        pointer = rows.data_ptr() + y0 * rows.stride(0)
-        ctx.decode_device(self.desc, avifgpu.planes_from_tensors(self.planes), pointer, rows.stride(0), y0, nrows, stream)
-
-    def torch_planar(self):
-        """The planar, low-bit planes of the same image, made on the GPU by torch: de-interleave, then shift."""
-        import torch
-        wide = self.desc.bit_depth > 8
-        dtype = torch.int16 if wide else torch.uint8
-        samples = [None if p is None else p.contiguous().view(dtype) for p in self.planes]
-        if self.desc.source_layout & NV:
-            samples[1], samples[2] = samples[1][:, 0::2], samples[1][:, 1::2]
-        if self.desc.source_layout & MSB:
-            shift = 16 - self.desc.bit_depth
-            samples = [None if s is None else ((s.to(torch.int32) & 0xFFFF) >> shift).to(torch.int16) for s in samples]
-        out = []
-        for s in samples:
-            if s is None:
-                out.append(None)
-                continue
-            raw = torch.empty(s.shape, dtype=s.dtype, device="cuda").copy_(s).view(torch.uint8)  # dense, whatever s's strides
-            backing = torch.zeros((max(raw.shape[0], 1), padded(raw.shape[1])), dtype=torch.uint8, device="cuda")
-            backing[:raw.shape[0], :raw.shape[1]].copy_(raw)
-            out.append(backing[:raw.shape[0], :raw.shape[1]])
-        return out
+def image(desc, w, h, seed, **kwargs):
+    """A DecodeImage of seed "semi_...": codes above the maximum where the layout holds them (low-bit samples)."""
+    return DecodeImage(desc, w, h, seed, prefix="semi_", overshoot=not desc.source_layout & MSB, **kwargs)
 
 
 def mix(desc, seed):
     # odd widths (odd chroma pair counts), odd 4:2:0 heights, right strips, a 1 x 1 image; one image whose interleaved
     # plane is 2 bytes off the pair loads' alignment, one with misaligned rows
     sizes = [(8, 2), (37, 5), (64, 7), (129, 4), (256, 3), (7, 3), (1, 1), (100, 6)]
-    images = [SemiImage(desc, w, h, f"{seed}_{i}") for i, (w, h) in enumerate(sizes)]
-    images.append(SemiImage(desc, 70, 6, f"{seed}_chroma", chroma_misalign=2))
-    rows = SemiImage(desc, 64, 5, f"{seed}_rows")
-    import torch
-    stride = padded(rows.row_bytes)
-    backing = torch.full(((rows.h + 1) * stride,), SENTINEL, dtype=torch.uint8, device="cuda")
-    rows.rows = backing[4:4 + rows.h * stride].view(rows.h, stride)[:, :rows.row_bytes]
-    images.append(rows)
+    images = [image(desc, w, h, f"{seed}_{i}") for i, (w, h) in enumerate(sizes)]
+    images.append(image(desc, 70, 6, f"{seed}_chroma", chroma_misalign=2))
+    images.append(image(desc, 64, 5, f"{seed}_rows", rows_offset=4))
     return images
 
 
@@ -210,11 +126,6 @@ def direct_launches(im):
         return 1
     step = 4 if im.desc.host_depth == 32 else 8
     return 1 + (im.w % step != 0) + (ys_of(im.desc) and im.h % 2 != 0)
-
-
-def chunk_launches(images):
-    chosen = [im for im in images if eligible(im)]
-    return sum(1 + any(has_edge(im) for im in chosen[i:i + 64]) for i in range(0, len(chosen), 64))
 
 
 def assert_planar_and_reference(ctx, images, reference, threads=1):
@@ -258,7 +169,7 @@ def test_instantiation(checker, port, name, variant, desc):
             im.rows.fill_(0)
         # the host-described batch: one chunk of one or two launches, then one direct call per image it does not take
         direct = sum(1 for im in fallbacks if im.w and im.h)
-        assert run(lambda stream: run_decode_batch(fresh, desc, images, stream)) == chunk_launches(images) + direct
+        assert run(lambda stream: run_decode_batch(fresh, desc, images, stream)) == chunk_launches(images, eligible, has_edge) + direct
         assert_planar_and_reference(fresh, images, reference)
         for im in images:
             im.rows.fill_(0)
@@ -282,8 +193,8 @@ NV12 = ycc(8, 8, C420, STRAIGHT, NV, abi.MATRIX_BT709, 0)
 def test_low_bits_change_nothing(ctx, desc):
     import torch
     ctx.prepare_decode(desc)
-    a = [SemiImage(desc, w, h, "lowbits", low_bits_seed=1) for w, h in ((136, 10), (37, 5))]
-    b = [SemiImage(desc, w, h, "lowbits", low_bits_seed=2) for w, h in ((136, 10), (37, 5))]
+    a = [image(desc, w, h, "lowbits", low_bits_seed=1) for w, h in ((136, 10), (37, 5))]
+    b = [image(desc, w, h, "lowbits", low_bits_seed=2) for w, h in ((136, 10), (37, 5))]
     assert not all(torch.equal(x, y) for x, y in zip(a[0].planes, b[0].planes) if x is not None)
     for images in (a, b):
         run_decode_batch(ctx, desc, images)
@@ -300,15 +211,10 @@ def test_low_bits_change_nothing(ctx, desc):
 @pytest.mark.parametrize("desc", [NV12, P010, P016_F32], ids=["nv12", "p010", "p016_f32"])
 def test_row_blocks_with_odd_y0(ctx, checker, port, desc):
     ctx.prepare_decode(desc)
-    im = SemiImage(desc, 203, 21, "blocks")
+    im = image(desc, 203, 21, "blocks")
     for y0, y1 in ((0, 3), (3, 8), (8, 9), (9, 16), (16, 21)):
         im.direct(ctx, im.rows, y0, y1 - y0)
     assert_planar_and_reference(ctx, [im], pick(checker, port, True))
-
-
-def sm_count():
-    import torch
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 @pytest.mark.gpu
@@ -320,51 +226,24 @@ def test_multipass(ctx, checker, port, api, desc):
     n, w, h = 64, 515, 263
     f32 = desc.host_depth == 32
     interior = -(-(w & ~(3 if f32 else 7)) // (128 if f32 else 256)) * (h // 2)
-    assert n * interior >= 2 * sm_count() * (2 if f32 else 3) * 8 and n * (h + 1) >= 2 * sm_count() * 16
-    images = [SemiImage(desc, w, h, f"multipass_{api}_{i}") for i in range(n)]
+    assert_passes("ycc_f32_interior" if f32 else "ycc_int_interior", n * interior, sm_count(ctx))
+    assert_passes("decode_edge", n * (h + 1), sm_count(ctx))
+    images = [image(desc, w, h, f"multipass_{api}_{i}") for i in range(n)]
     ctx.prepare_decode(desc)
-    if api == "host":
-        assert launches_of(ctx, lambda: run_decode_batch(ctx, desc, images)) == 2
-    else:
-        batch = Indirect(n)
-        batch.load(images)
-        assert launches_of(ctx, lambda: batch.decode(ctx, desc)) == 3
-        assert (batch.statuses() == 0).all()
-    assert_planar_and_reference(ctx, images, pick(checker, port, True), threads=os.cpu_count())
+    host_or_device(ctx, desc, "decode", api, images, lambda done: assert_planar_and_reference(ctx, done, pick(checker, port, True), threads=os.cpu_count()))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("desc", [NV12, P016_F32], ids=["nv12", "p016_f32"])
 def test_captured_call_replays_new_image_sets(checker, port, desc):
     import avifgpu
-    import torch
     reference = pick(checker, port, True)
+    sizes = [(8, 2), (37, 5), (129, 4), (7, 3), (100, 6)]
+    sets = replay_sets(lambda w, h, seed: image(desc, w, h, seed), "replay", (136, 34), sizes)
     with avifgpu.Context(0) as fresh:
-        batch = Indirect(256)
-        stream = torch.cuda.Stream()
-        with torch.cuda.stream(stream):
-            batch.load([SemiImage(desc, 64, 16, "replay_capture")])
-        fresh.prepare_decode(desc)
-        stream.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        before = fresh.launch_count()
-        with torch.cuda.graph(graph, stream=stream):
-            batch.decode(fresh, desc, stream.cuda_stream)
-        assert fresh.launch_count() - before == 3
-        sizes = [(8, 2), (37, 5), (129, 4), (7, 3), (100, 6)]
-        sets = [[SemiImage(desc, 96, 10, "replay_one")],
-                [SemiImage(desc, 136, 34, f"replay_64_{i}") for i in range(64)],
-                [SemiImage(desc, *sizes[i % len(sizes)], f"replay_256_{i}") for i in range(256)]]
-        for images in sets:
-            with torch.cuda.stream(stream):
-                batch.load(images)
-                before = fresh.launch_count()
-                graph.replay()
-            torch.cuda.synchronize()
-            assert fresh.launch_count() == before
-            assert (batch.statuses()[:len(images)] == 0).all()
-            assert_planar_and_reference(fresh, images, reference, threads=os.cpu_count())
-        del graph
+        capture_and_replay(fresh, desc, "decode", image(desc, 64, 16, "replay_capture"), sets,
+                           lambda images: assert_planar_and_reference(fresh, images, reference, threads=os.cpu_count()),
+                           lambda: fresh.prepare_decode(desc))
 
 
 # ---- 3. refusals and the API-9-sized description ----------------------------------------------------------------------------
@@ -375,7 +254,9 @@ def test_host_async_and_sharded_calls_refuse_a_layout(ctx, call):
     import avifgpu
     desc = abi.DecodeDesc.from_buffer_copy(P010)
     desc.width, desc.height = 32, 8
-    planes = cases.code_planes(cases.rng_for("refuse"), planar_of(desc))
+    planar = abi.DecodeDesc.from_buffer_copy(desc)
+    planar.source_layout = abi.SOURCE_PLANAR
+    planes = cases.code_planes(cases.rng_for("refuse"), planar)
     planes = [planes[0], np.repeat(planes[1], 2, axis=1), None, planes[3]]
     out = np.zeros((8, 32 * 4), dtype=np.uint16)
     before = ctx.launch_count()
@@ -397,7 +278,7 @@ def test_api9_sized_description_decodes(ctx, checker, port):
     import avifgpu
     import torch
     desc = ycc(16, 10, C420, STRAIGHT, abi.SOURCE_PLANAR, abi.MATRIX_BT709, 1)
-    images = [SemiImage(desc, 77, 9, "v9")]
+    images = [image(desc, 77, 9, "v9")]
     old = abi.DecodeDesc.from_buffer_copy(images[0].desc)
     old.struct_size = C.sizeof(abi.DecodeDesc) - 4
     old.source_layout = NVMSB  # past the end of an API-9 struct: never read

@@ -27,8 +27,9 @@ import pytest
 import cases
 import encode_spec
 from avifgpu import abi
-from test_gpu_batch import SENTINEL, ctx, padded, run_batch, whole  # noqa: F401
-from test_gpu_batch_indirect import Indirect, launches_of
+from gpu_harness import ctx  # noqa: F401
+from gpu_harness import (SENTINEL, EncodeImage, Indirect, assert_passes, capture_and_replay, chunk_launches, host_or_device, launches_of,
+                         replay_sets, run_batch, sm_count, whole)
 
 C444, C422, C420 = abi.CHROMA_444, abi.CHROMA_422, abi.CHROMA_420
 NONE, STRAIGHT, PREMUL = abi.ALPHA_NONE, abi.ALPHA_STRAIGHT, abi.ALPHA_PREMULTIPLIED
@@ -88,86 +89,9 @@ def test_case_table_is_complete():
 
 # ---- images -------------------------------------------------------------------------------------------------------------
 
-def planar_of(desc):
-    d = abi.EncodeDesc.from_buffer_copy(desc)
-    d.dest_layout = abi.SOURCE_PLANAR
-    return d
-
-
-class EncImage:
-    """Seeded host rows on the GPU and sentinel-padded destination planes of `desc`'s layout (byte tensors); with
-    interleaved chroma also a sentinel-filled plane-2 buffer, passed to every call, that must stay untouched."""
-
-    def __init__(self, desc, w, h, seed, chroma_misalign=0, rows_misalign=0, extreme=False):
-        import torch
-        self.w, self.h = w, h
-        d = self.desc = abi.EncodeDesc.from_buffer_copy(desc)
-        d.width, d.height = w, h
-        self.planar_desc = planar_of(d)
-        rng = cases.rng_for(f"semi_encode_{seed}_{w}x{h}")
-        if extreme:
-            self.host = encode_spec.extreme_rows(d, w, h, f"semi_encode_{seed}")
-        elif d.host_depth == 32:
-            self.host = cases.float_host_rows(rng, h, w, d.host_channels)
-        else:
-            self.host = cases.int_host_rows(rng, h, w, d.host_channels, d.host_depth, beyond=True)
-        self.row_bytes = w * d.host_channels * d.host_depth // 8
-        backing = torch.zeros((max(h, 1), padded(self.row_bytes) + rows_misalign), dtype=torch.uint8, device="cuda")
-        self.rows = backing[:h, rows_misalign:rows_misalign + self.row_bytes]
-        if w and h:
-            self.rows.copy_(torch.from_numpy(np.ascontiguousarray(self.host).view(np.uint8).reshape(h, self.row_bytes)).cuda())
-        self.sample_bytes = 2 if d.image_bit_depth > 8 else 1
-        shapes = abi.encode_plane_shapes(d)
-        self.planes = [self.alloc(s, chroma_misalign if k == 1 else 0) for k, s in enumerate(shapes)]
-        if d.dest_layout & NV:
-            self.planes[2] = self.alloc(abi.encode_plane_shapes(self.planar_desc)[2])  # ignored: must stay sentinel
-
-    def alloc(self, shape, misalign=0):
-        import torch
-        if shape is None:
-            return None
-        rows, cols = shape
-        # one spare row: whole() reads a full stride from the view's first byte, `misalign` bytes past the last row
-        backing = torch.full((max(rows, 1) + 1, padded(cols * self.sample_bytes) + misalign), SENTINEL, dtype=torch.uint8, device="cuda")
-        return backing[:rows, misalign:misalign + cols * self.sample_bytes]
-
-    def record(self):
-        return (self.w, self.h, self.rows, self.planes)
-
-    def direct(self, ctx, desc=None, planes=None, y0=0, nrows=None, stream=0):
-        import avifgpu
-        nrows = self.h - y0 if nrows is None else nrows
-        ctx.encode_device(desc or self.desc, self.rows.data_ptr() + y0 * self.rows.stride(0), self.rows.stride(0),
-                          avifgpu.planes_from_tensors(planes or self.planes), y0, nrows, stream)
-
-    def expected(self, ctx):
-        """The planar encode of the same description and rows, then re-interleaved and shifted by torch: per plane of the
-        layout, its visible bytes (numpy, uint8)."""
-        import torch
-        planar = [self.alloc(s) for s in abi.encode_plane_shapes(self.planar_desc)]
-        self.direct(ctx, self.planar_desc, planar)
-        torch.cuda.synchronize()
-        wide = self.sample_bytes == 2
-        codes = [None if p is None else p.contiguous().view(torch.int16 if wide else torch.uint8).to(torch.int32) & (0xFFFF if wide else 0xFF)
-                 for p in planar]
-        if self.desc.dest_layout & MSB:
-            shift = 16 - self.desc.image_bit_depth
-            codes = [None if c is None else c << shift for c in codes]
-        if self.desc.dest_layout & NV:
-            codes[1] = torch.stack([codes[1], codes[2]], dim=-1).reshape(codes[1].shape[0], -1)
-            codes[2] = None
-        dtype = np.uint16 if wide else np.uint8
-        return [None if c is None else c.cpu().numpy().astype(dtype).view(np.uint8).reshape(c.shape[0], -1) for c in codes]
-
-    def codes_of_output(self):
-        """The output turned back into planar, low-bit codes (numpy), for the independent model."""
-        wide = self.sample_bytes == 2
-        out = [None if p is None else p.cpu().numpy().view(np.uint16 if wide else np.uint8).astype(np.int64) for p in self.planes]
-        if self.desc.dest_layout & NV:
-            out[1], out[2] = out[1][:, 0::2], out[1][:, 1::2]
-        if self.desc.dest_layout & MSB:
-            out = [None if c is None else c >> (16 - self.desc.image_bit_depth) for c in out]
-        return out
+def image(desc, w, h, seed, **kwargs):
+    """An EncodeImage of seed "semi_encode_...", 16-bit hosts with samples above 32768."""
+    return EncodeImage(desc, w, h, seed, prefix="semi_encode_", beyond=True, **kwargs)
 
 
 def assert_layout_of_planar(ctx, images):
@@ -199,9 +123,9 @@ def mix(desc, seed):
     # right strips and odd chroma pair counts, odd 4:2:0 heights, narrow images, a 1 x 1 image; one image whose
     # interleaved plane is 2 bytes off the paired stores' alignment, one with misaligned rows
     sizes = [(8, 2), (37, 5), (64, 7), (129, 4), (256, 3), (7, 3), (1, 1), (100, 6)]
-    images = [EncImage(desc, w, h, f"{seed}_{i}") for i, (w, h) in enumerate(sizes)]
-    images.append(EncImage(desc, 70, 6, f"{seed}_chroma", chroma_misalign=2))
-    images.append(EncImage(desc, 64, 5, f"{seed}_rows", rows_misalign=4))
+    images = [image(desc, w, h, f"{seed}_{i}") for i, (w, h) in enumerate(sizes)]
+    images.append(image(desc, 70, 6, f"{seed}_chroma", chroma_misalign=2))
+    images.append(image(desc, 64, 5, f"{seed}_rows", rows_misalign=4))
     return images
 
 
@@ -238,11 +162,6 @@ def direct_launches(im):
         return 1
     step = 4 if im.desc.host_depth == 32 else 8
     return 1 + (im.w % step != 0) + (ys_of(im.desc) and im.h % 2 != 0)
-
-
-def chunk_launches(images):
-    chosen = [im for im in images if eligible(im)]
-    return sum(1 + any(has_edge(im) for im in chosen[i:i + 64]) for i in range(0, len(chosen), 64))
 
 
 @pytest.fixture(scope="module")
@@ -283,7 +202,7 @@ def test_instantiation(tables, request, name, family, desc):
         reset(images)
         # the host-described batch: one chunk of one or two launches (integer hosts), one direct call per other image
         direct = sum(direct_launches(im) for im in images if im.w and im.h and (family != "int" or not eligible(im)))
-        chunks = chunk_launches(images) if family == "int" else 0
+        chunks = chunk_launches(images, eligible, has_edge) if family == "int" else 0
         assert launches_of(ctx, lambda: run_batch(ctx, desc, images)) == chunks + direct
         assert_layout_of_planar(ctx, images)
         reset(images)
@@ -303,7 +222,7 @@ def test_instantiation(tables, request, name, family, desc):
         if name in SPEC_CASES:
             ref = request.getfixturevalue("ref")
             for extreme in (False, True):
-                im = EncImage(desc, 259, 37, f"{name}_spec", extreme=extreme)
+                im = image(desc, 259, 37, f"{name}_spec", extreme=extreme)
                 im.direct(ctx)
                 import torch
                 torch.cuda.synchronize()
@@ -330,7 +249,7 @@ def test_untuned_descriptions_take_the_generic_kernel(tables, kind):
         desc.row_matrix_enabled = 1
         desc.row_matrix[:] = [0.9, 0.05, 0.05, 0.1, 0.8, 0.1, 0.0, 0.1, 0.9]
     tables.prepare_encode(desc)
-    images = [EncImage(desc, w, h, f"untuned_{kind}") for w, h in ((136, 10), (37, 5))]
+    images = [image(desc, w, h, f"untuned_{kind}") for w, h in ((136, 10), (37, 5))]
     for im in images:
         assert launches_of(tables, lambda: im.direct(tables)) == 1
     assert_layout_of_planar(tables, images)
@@ -340,15 +259,10 @@ def test_untuned_descriptions_take_the_generic_kernel(tables, kind):
 @pytest.mark.parametrize("desc", [NV12, P010, P016_F32], ids=["nv12", "p010", "p016_f32"])
 def test_row_blocks(tables, desc):
     tables.prepare_encode(desc)
-    im = EncImage(desc, 203, 21, "blocks")
+    im = image(desc, 203, 21, "blocks")
     for y0, y1 in ((0, 4), (4, 10), (10, 12), (12, 20), (20, 21)):
         im.direct(tables, y0=y0, nrows=y1 - y0)
     assert_layout_of_planar(tables, [im])
-
-
-def sm_count():
-    import torch
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 @pytest.mark.gpu
@@ -358,51 +272,23 @@ def test_multipass(ctx, api, desc):
     """64 images of 1031 x 300 (4:2:0): 4 interior units x 150 row pairs and 150 edge units per image; the interior grid
     has 16 CTAs of 8 warps per SM, the edge grid 16 one-CTA workers per SM -- both walk at least twice."""
     n, w, h = 64, 1031, 300
-    assert n * 4 * (h // 2) >= 2 * sm_count() * 16 * 8 and n * (h // 2) >= 2 * sm_count() * 16
-    images = [EncImage(desc, w, h, f"multipass_{api}_{i}") for i in range(n)]
+    assert_passes("encode_interior", n * 4 * (h // 2), sm_count(ctx))
+    assert_passes("encode_edge", n * (h // 2), sm_count(ctx))
+    images = [image(desc, w, h, f"multipass_{api}_{i}") for i in range(n)]
     images[0].direct(ctx)
-    if api == "host":
-        assert launches_of(ctx, lambda: run_batch(ctx, desc, images)) == 2
-    else:
-        batch = Indirect(n)
-        batch.load(images)
-        assert launches_of(ctx, lambda: batch.encode(ctx, desc)) == 3
-        assert (batch.statuses() == 0).all()
-    assert_layout_of_planar(ctx, images)
+    host_or_device(ctx, desc, "encode", api, images, lambda done: assert_layout_of_planar(ctx, done))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("desc", [NV12, P010], ids=["nv12", "p010"])
 def test_captured_call_replays_new_image_sets(desc):
     import avifgpu
-    import torch
+    sizes = [(8, 2), (37, 5), (129, 4), (7, 3), (100, 6)]
+    sets = replay_sets(lambda w, h, seed: image(desc, w, h, seed), "replay", (136, 34), sizes)
+    warm = image(desc, 64, 16, "replay_capture")
     with avifgpu.Context(0) as fresh:
-        batch = Indirect(256)
-        stream = torch.cuda.Stream()
-        warm = EncImage(desc, 64, 16, "replay_capture")
-        warm.direct(fresh)  # the premultiply check, outside the capture
-        with torch.cuda.stream(stream):
-            batch.load([warm])
-        stream.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        before = fresh.launch_count()
-        with torch.cuda.graph(graph, stream=stream):
-            batch.encode(fresh, desc, stream.cuda_stream)
-        assert fresh.launch_count() - before == 3
-        sizes = [(8, 2), (37, 5), (129, 4), (7, 3), (100, 6)]
-        sets = [[EncImage(desc, 96, 10, "replay_one")],
-                [EncImage(desc, 136, 34, f"replay_64_{i}") for i in range(64)],
-                [EncImage(desc, *sizes[i % len(sizes)], f"replay_256_{i}") for i in range(256)]]
-        for images in sets:
-            with torch.cuda.stream(stream):
-                batch.load(images)
-                before = fresh.launch_count()
-                graph.replay()
-            torch.cuda.synchronize()
-            assert fresh.launch_count() == before
-            assert (batch.statuses()[:len(images)] == 0).all()
-            assert_layout_of_planar(fresh, images)
-        del graph
+        # the premultiply check, outside the capture
+        capture_and_replay(fresh, desc, "encode", warm, sets, lambda images: assert_layout_of_planar(fresh, images), lambda: warm.direct(fresh))
 
 
 # ---- 3. refusals and the API-10-sized description ---------------------------------------------------------------------------
@@ -427,7 +313,7 @@ def test_host_async_and_sharded_calls_refuse_a_layout(ctx, call):
                     if call == "sharded":
                         group.encode(desc, rows, planes=planes)
                     else:
-                        im = EncImage(desc, 32, 8, "refuse_device")
+                        im = image(desc, 32, 8, "refuse_device")
                         group.encode_device(desc, [im.rows.data_ptr()], [im.rows.stride(0)], avifgpu.planes_from_tensors(im.planes))
                 finally:
                     assert group.launch_count() == 0
@@ -446,9 +332,9 @@ def test_device_calls_refuse_bad_layouts(ctx, fault, status):
         desc.dest_layout = NVMSB
     else:
         desc.dest_layout = 4
-    im = EncImage(NV12, 64, 8, "bad_layout")
+    im = image(NV12, 64, 8, "bad_layout")
     before = ctx.launch_count()
-    for call in (lambda: im.direct(ctx, desc), lambda: run_batch(ctx, desc, [im]), lambda: Indirect(4).encode(ctx, desc)):
+    for call in (lambda: im.direct(ctx, desc=desc), lambda: run_batch(ctx, desc, [im]), lambda: Indirect(4).encode(ctx, desc)):
         with pytest.raises(avifgpu.AvifGpuError) as failure:
             call()
         assert failure.value.status == status
@@ -461,11 +347,12 @@ def test_device_calls_refuse_bad_layouts(ctx, fault, status):
 def test_api10_sized_description_encodes_planar(tables, desc):
     """A caller built against API version 10 passes the shorter struct; it means the planar layout, whatever follows it."""
     tables.prepare_encode(desc)
-    planar = planar_of(desc)
-    images = [EncImage(planar, 77, 9, "v10"), EncImage(planar, 136, 10, "v10b")]
+    planar = abi.EncodeDesc.from_buffer_copy(desc)
+    planar.dest_layout = abi.SOURCE_PLANAR
+    images = [image(planar, 77, 9, "v10"), image(planar, 136, 10, "v10b")]
     old = abi.EncodeDesc.from_buffer_copy(images[0].desc)
     old.struct_size = C.sizeof(abi.EncodeDesc) - 4
     old.dest_layout = NVMSB  # past the end of an API-10 struct: never read
-    images[0].direct(tables, old)
+    images[0].direct(tables, desc=old)
     run_batch(tables, old, images[1:])
     assert_layout_of_planar(tables, images)

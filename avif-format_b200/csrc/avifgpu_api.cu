@@ -104,7 +104,7 @@ struct avifgpu_context
     cudaStream_t streams[kPipelineStreams] = {};
     cudaEvent_t sliceDone[kPipelineStreams] = {};
     cudaEvent_t rowsConsumed[kPipelineStreams] = {}; // encode: the slot's H2D of caller rows has finished
-    cudaEvent_t callRowsConsumed[2] = {};            // the last H2D of an asynchronous encode call (calls alternate between the two)
+    cudaEvent_t callRowsConsumed[2] = {};            // every H2D of an asynchronous encode call has finished (calls alternate between the two)
     int64_t asyncEncodeCalls = 0;
     bool previousCallRowsPending = false;            // callRowsConsumed[(asyncEncodeCalls - 1) & 1] guards caller memory still on the wire
 
@@ -124,6 +124,7 @@ struct avifgpu_context
         bool busy = false;
         int64_t ticket = 0;
         std::vector<HostCopy> owed;
+        bool owesRows = false; // `owed` copies a decode's rows out of pinnedRows[slot]
     };
     SlotState slots[kPipelineStreams];
     int nextSlot = 0;
@@ -1446,6 +1447,7 @@ static int WaitSlot(avifgpu_context* ctx, int slot)
     if (status != AVIFGPU_OK)
     {
         state.owed.clear();
+        state.owesRows = false;
     }
     state.busy = false;
     return status;
@@ -1471,6 +1473,7 @@ static void PayOwed(avifgpu_context* ctx, int slot)
         CopyPool::Instance().Copy(batch, count); // all planes of the slice share the pool's threads
     }
     state.owed.clear();
+    state.owesRows = false;
 }
 
 static int RetireSlot(avifgpu_context* ctx, int slot)
@@ -1499,6 +1502,27 @@ static int RetireThrough(avifgpu_context* ctx, int64_t ticket)
     return result;
 }
 
+// Every host-pointer call that returns AVIFGPU_OK hands the rows of the previous asynchronous encode call back to the
+// caller (avifgpu.h).  A call takes that release before it queues its own copies and waits for those rows' H2Ds just
+// before it returns, so the link never idles at a call boundary.
+struct RowsRelease
+{
+    bool pending;
+    int event; // callRowsConsumed[event]
+};
+
+static RowsRelease TakeRowsRelease(avifgpu_context* ctx)
+{
+    const RowsRelease release{ ctx->previousCallRowsPending, static_cast<int>((ctx->asyncEncodeCalls - 1) & 1) };
+    ctx->previousCallRowsPending = false;
+    return release;
+}
+
+static int FinishRowsRelease(avifgpu_context* ctx, RowsRelease release)
+{
+    return release.pending ? ctx->Cuda(cudaEventSynchronize(ctx->callRowsConsumed[release.event]), "cudaEventSynchronize") : AVIFGPU_OK;
+}
+
 // A failure in the middle of a call: nothing of this context may still be writing into caller memory on return.
 static int AbandonCall(avifgpu_context* ctx, int status)
 {
@@ -1506,6 +1530,7 @@ static int AbandonCall(avifgpu_context* ctx, int status)
     {
         cudaStreamSynchronize(ctx->streams[i]);
         ctx->slots[i].owed.clear();
+        ctx->slots[i].owesRows = false;
         ctx->slots[i].busy = false;
     }
     cudaGetLastError();
@@ -1550,6 +1575,7 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
     DeviceGuard guard(ctx->device);
     if (nrows == 0 || desc->width == 0)
     {
+        if ((status = FinishRowsRelease(ctx, TakeRowsRelease(ctx))) != AVIFGPU_OK) return status;
         return wait ? RetireThrough(ctx, ticket) : AVIFGPU_OK;
     }
     PlaneGeometry geometry[AVIFGPU_MAX_PLANES];
@@ -1571,22 +1597,24 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
     const bool rowsPinned = IsPinned(host_rows);
     const int sliceRows = SliceRows(nrows, rowPayload);
 
-    // The rows handed to the PREVIOUS asynchronous call may be overwritten once this call returns.  Their last H2D is
-    // waited for at the END of this call, after this call's own copies are queued behind it, so the link never idles
-    // at a call boundary.
-    const bool waitForPreviousRows = ctx->previousCallRowsPending;
-    const int previousRowsEvent = static_cast<int>((ctx->asyncEncodeCalls - 1) & 1);
-    ctx->previousCallRowsPending = false;
+    const RowsRelease previousRows = TakeRowsRelease(ctx);
     bool recordedCallRows = false;
+    bool callSlots[kPipelineStreams] = {}; // the slots this call's H2Ds went through
 
     for (int begin = 0; begin < nrows; begin += sliceRows)
     {
         const int rows = std::min(sliceRows, nrows - begin);
         const int slot = ctx->nextSlot;
         cudaStream_t stream = ctx->streams[slot];
-        // The slot's previous slice: wait for the GPU, but pay its bounce copies only after this slice's H2D and kernel are
-        // queued -- the host then copies while the link and the SMs work (its D2H, which reuses the bounce buffers, comes last).
+        // The slot's previous slice: wait for the GPU, but pay an encode's plane copies only after this slice's H2D and
+        // kernel are queued -- the host then copies while the link and the SMs work (its D2H, which reuses the plane
+        // bounce buffers, comes last).  A decode's rows are paid first: this slice's rows land in (and may regrow) the
+        // same pinned buffer.
         if ((status = WaitSlot(ctx, slot)) != AVIFGPU_OK) return AbandonCall(ctx, status);
+        if (ctx->slots[slot].owesRows)
+        {
+            PayOwed(ctx, slot);
+        }
         ctx->nextSlot = (slot + 1) % kPipelineStreams;
 
         if ((status = ctx->EnsureDevice(ctx->deviceRows[slot], static_cast<size_t>(deviceRowStride) * rows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
@@ -1605,9 +1633,17 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
                                                   static_cast<size_t>(rows), cudaMemcpyHostToDevice, stream),
                                 "H2D rows")) != AVIFGPU_OK) return AbandonCall(ctx, status);
         if ((status = ctx->Cuda(cudaEventRecord(ctx->rowsConsumed[slot], stream), "cudaEventRecord")) != AVIFGPU_OK) return AbandonCall(ctx, status);
+        callSlots[slot] = true;
         if (!wait && rowsPinned && begin + sliceRows >= nrows)
         {
-            // the caller's own memory is on the wire until this H2D, the last of the call: the NEXT call waits for it before it returns
+            // The caller's own memory is on the wire until every H2D of the call has finished, and the H2Ds of different
+            // streams may finish out of order: the last slice's stream waits for the other slots' before it records the
+            // event the NEXT call waits for.
+            for (int s = 0; s < kPipelineStreams; ++s)
+            {
+                if (s != slot && callSlots[s] &&
+                    (status = ctx->Cuda(cudaStreamWaitEvent(stream, ctx->rowsConsumed[s], 0), "cudaStreamWaitEvent")) != AVIFGPU_OK) return AbandonCall(ctx, status);
+            }
             if ((status = ctx->Cuda(cudaEventRecord(ctx->callRowsConsumed[ctx->asyncEncodeCalls & 1], stream), "cudaEventRecord")) != AVIFGPU_OK) return AbandonCall(ctx, status);
             recordedCallRows = true;
         }
@@ -1669,10 +1705,7 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
         state.busy = true;
         state.ticket = ticket;
     }
-    if (waitForPreviousRows)
-    {
-        if ((status = ctx->Cuda(cudaEventSynchronize(ctx->callRowsConsumed[previousRowsEvent]), "cudaEventSynchronize")) != AVIFGPU_OK) return AbandonCall(ctx, status);
-    }
+    if ((status = FinishRowsRelease(ctx, previousRows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
     if (wait)
     {
         status = RetireThrough(ctx, ticket);
@@ -1727,6 +1760,7 @@ static int DecodeRowsHost(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
     DeviceGuard guard(ctx->device);
     if (nrows == 0 || desc->width == 0)
     {
+        if ((status = FinishRowsRelease(ctx, TakeRowsRelease(ctx))) != AVIFGPU_OK) return status;
         return wait ? RetireThrough(ctx, ticket) : AVIFGPU_OK;
     }
     PlaneGeometry geometry[AVIFGPU_MAX_PLANES];
@@ -1746,6 +1780,7 @@ static int DecodeRowsHost(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
     const int64_t deviceRowStride = (rowPayload + 255) & ~255ll;
     const int sliceRows = SliceRows(nrows, rowPayload);
     const bool rowsPinned = IsPinned(host_rows);
+    const RowsRelease previousRows = TakeRowsRelease(ctx);
 
     for (int begin = 0; begin < nrows; begin += sliceRows)
     {
@@ -1831,6 +1866,7 @@ static int DecodeRowsHost(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
             if ((status = ctx->EnsurePinned(ctx->pinnedRows[slot], static_cast<size_t>(rowPayload) * rows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
             uint8_t* bounce = static_cast<uint8_t*>(ctx->pinnedRows[slot].ptr);
             state.owed.push_back(avifgpu_context::HostCopy{ target, row_stride_bytes, bounce, rowPayload, rowPayload, rows });
+            state.owesRows = true;
             target = bounce;
             targetStride = rowPayload;
         }
@@ -1842,6 +1878,7 @@ static int DecodeRowsHost(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
         state.busy = true;
         state.ticket = ticket;
     }
+    if ((status = FinishRowsRelease(ctx, previousRows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
     if (wait)
     {
         status = RetireThrough(ctx, ticket);

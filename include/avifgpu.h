@@ -347,8 +347,11 @@ AVIFGPU_EXPORT int avifgpu_decode_rows(avifgpu_context* ctx, const avifgpu_decod
  * the GPU converts and copies this one.  Single-threaded contract like the rest of a context: calls on one context come
  * from one thread at a time.
  *   encode: on return the rows of THIS call may still be read by the copy engine when host_rows is page-locked memory
- *           (avifgpu_host_alloc); they may be overwritten once the NEXT call on this context has returned (two row
- *           buffers make a double-buffered shuttle) or avifgpu_wait() has.  Pageable rows are consumed before return.
+ *           (avifgpu_host_alloc).  They may be overwritten (two row buffers make a double-buffered shuttle) once one of
+ *           these has returned AVIFGPU_OK on this context: the next host-pointer call of either direction -- encode or
+ *           decode, synchronous or asynchronous, an empty row block included; avifgpu_wait() with a ticket covering
+ *           this call; avifgpu_synchronize().  A call refused with an error does not release them, and neither do the
+ *           device-pointer and batch calls.  Pageable rows are consumed before return.
  *           The destination planes are complete after avifgpu_wait(ticket).
  *   decode: the source planes must stay valid and the host rows are complete after avifgpu_wait(ticket).
  * out_ticket (may be NULL) identifies the call; tickets increase by one per host-pointer call on a context.

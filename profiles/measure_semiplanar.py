@@ -13,39 +13,14 @@ line with the card's name, power limit and maximum SM clock, read in the same ru
 
     python profiles/measure_semiplanar.py [--seconds 1.0] [--rounds 5] [--out semiplanar.json]
 """
-import argparse
-import json
-import os
-import subprocess
-import sys
+import harness
+import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "avif-format_b200", "python"))
-import torch  # noqa: E402
-
-import avifgpu  # noqa: E402
-from avifgpu import abi  # noqa: E402
+import avifgpu
+from avifgpu import abi
+from harness import median_us, padded, plane
 
 NV, NVMSB = abi.SOURCE_CHROMA_INTERLEAVED, abi.SOURCE_CHROMA_INTERLEAVED | abi.SOURCE_MSB_ALIGNED
-
-
-def card():
-    ident = {"name": torch.cuda.get_device_name(0)}
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", "0"],
-                             capture_output=True, text=True, timeout=10).stdout.strip().split(",")
-        ident["power_limit_w"], ident["sm_max_mhz"] = float(out[0]), float(out[1])
-    except Exception:
-        ident["power_limit_w"] = ident["sm_max_mhz"] = None
-    return ident
-
-
-def padded(n):
-    return (n + 63) // 64 * 64
-
-
-def plane(rows, samples, wide):
-    t = torch.empty((rows, padded(samples * (2 if wide else 1))), dtype=torch.uint8, device="cuda")
-    return t[:, :samples * (2 if wide else 1)]
 
 
 class Frame:
@@ -111,37 +86,6 @@ class Frame:
                     self.scratch[k].copy_(self.source[k])
 
 
-def timed(run, seconds):
-    """Microseconds per call of `run`, by CUDA events over at least `seconds` of back-to-back calls."""
-    run()
-    torch.cuda.synchronize()
-    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    calls = 1
-    while True:
-        start.record()
-        for _ in range(calls):
-            run()
-        end.record()
-        end.synchronize()
-        ms = start.elapsed_time(end)
-        if ms >= seconds * 1000.0:
-            return ms * 1000.0 / calls
-        calls = max(calls * 2, int(calls * seconds * 1100.0 / max(ms, 1e-3)))
-
-
-def measure(ways, seconds, rounds):
-    samples = {name: [] for name in ways}
-    for _ in range(rounds):
-        for name, run in ways.items():
-            samples[name].append(timed(run, seconds))
-    return {name: sorted(v)[len(v) // 2] for name, v in samples.items()}
-
-
-def same(a, b):
-    torch.cuda.synchronize()
-    return bool(torch.equal(a, b))
-
-
 def single(ctx, desc, w, h, seconds, rounds, generator):
     f = Frame(desc, w, h, generator)
     ctx.prepare_decode(f.desc)
@@ -159,8 +103,8 @@ def single(ctx, desc, w, h, seconds, rounds, generator):
     b = f.rows.clone()
     split_then_planar()
     c = f.rows.clone()
-    out = measure({"semi_planar": semi, "planar": planar, "deinterleave_then_planar": split_then_planar}, seconds, rounds)
-    out["identical"] = same(a, b) and same(a, c)
+    out = median_us({"semi_planar": semi, "planar": planar, "deinterleave_then_planar": split_then_planar}, seconds, rounds)
+    out["identical"] = torch.equal(a, b) and torch.equal(a, c)
     source_bytes = sum(p.numel() for p in f.source if p is not None)
     out["bytes_moved"] = source_bytes + f.rows.numel()
     out["semi_planar_gbs"] = out["bytes_moved"] / out["semi_planar"] / 1e3
@@ -194,38 +138,28 @@ def batches(ctx, desc, n, w, h, seconds, rounds, generator):
         run()
         torch.cuda.synchronize()
         outputs[name] = torch.cat([f.rows.reshape(-1) for f in frames]).clone()
-    out = {k: v / n for k, v in measure(ways, seconds, rounds).items()}  # per image
+    out = median_us(ways, seconds, rounds, n)
     first = next(iter(outputs.values()))
-    out["identical"] = all(same(first, o) for o in outputs.values())
+    out["identical"] = all(torch.equal(first, o) for o in outputs.values())
     return out
 
 
 def main():
-    parser = argparse.ArgumentParser()
-    parser.add_argument("--seconds", type=float, default=1.0)
-    parser.add_argument("--rounds", type=int, default=5)
-    parser.add_argument("--out")
-    args = parser.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("measure_semiplanar.py needs a CUDA device")
+    args = harness.arguments(rounds=5).parse_args()
+    harness.require_gpu()
     generator = torch.Generator(device="cuda")
     generator.manual_seed(20261016)
     pq = abi.Nclx(1, abi.PRIMARIES_BT2020, abi.TRANSFER_CHAR_PQ, abi.MATRIX_BT2020_NCL, 0)
     bt709 = abi.Nclx(1, abi.PRIMARIES_BT709, abi.TRANSFER_CHAR_SRGB, abi.MATRIX_BT709, 0)
     p010 = abi.DecodeDesc(0, 0, abi.COLORSPACE_YCBCR, abi.CHROMA_420, 10, abi.ALPHA_NONE, 32, pq, pq_peak_nits=1000, source_layout=NVMSB)
     nv12 = abi.DecodeDesc(0, 0, abi.COLORSPACE_YCBCR, abi.CHROMA_420, 8, abi.ALPHA_STRAIGHT, 8, bt709, source_layout=NV)
-    result = {"card": card(), "unit": "microseconds per image (device events, median of rounds)"}
+    result = {"card": harness.card(), "unit": "microseconds per image (device events, median of rounds)"}
     with avifgpu.Context(0) as ctx:
         result["p010_8k"] = single(ctx, p010, 7680, 4320, args.seconds, args.rounds, generator)
         result["nv12_8k"] = single(ctx, nv12, 7680, 4320, args.seconds, args.rounds, generator)
         result["nv12_b64"] = batches(ctx, nv12, 64, 512, 512, args.seconds, args.rounds, generator)
         result["nv12_b256"] = batches(ctx, nv12, 256, 512, 512, args.seconds, args.rounds, generator)
-    line = json.dumps(result)
-    print(line)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
+    harness.emit([result], args.out)
 
 
 if __name__ == "__main__":

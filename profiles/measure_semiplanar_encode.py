@@ -14,18 +14,12 @@ bit.  Prints one JSON line with the card's name, power limit and maximum SM cloc
 
     python profiles/measure_semiplanar_encode.py [--seconds 1.0] [--rounds 5] [--out semiplanar_encode.json]
 """
-import argparse
-import json
-import os
-import sys
+import harness
+import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "avif-format_b200", "python"))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import torch  # noqa: E402
-
-import avifgpu  # noqa: E402
-from avifgpu import abi  # noqa: E402
-from measure_semiplanar import card, measure, padded, plane, same  # noqa: E402
+import avifgpu
+from avifgpu import abi
+from harness import median_us, padded, plane
 
 NV, NVMSB = abi.SOURCE_CHROMA_INTERLEAVED, abi.SOURCE_CHROMA_INTERLEAVED | abi.SOURCE_MSB_ALIGNED
 
@@ -91,9 +85,9 @@ def single(ctx, desc, w, h, seconds, rounds, generator):
     semi()
     torch.cuda.synchronize()
     launches = ctx.launch_count() - before  # one call, before the timing
-    out = measure({"semi_planar": semi, "planar": planar, "planar_then_interleave": planar_then_interleave}, seconds, rounds)
+    out = median_us({"semi_planar": semi, "planar": planar, "planar_then_interleave": planar_then_interleave}, seconds, rounds)
     out["semi_planar_launches"] = launches
-    out["identical"] = same(f.outputs(f.semi), f.outputs(f.relaid))
+    out["identical"] = torch.equal(f.outputs(f.semi), f.outputs(f.relaid))
     out["table_valid"] = stats["valid"]
     out["bytes_moved"] = f.rows.numel() + sum(p.numel() for p in f.semi if p is not None)
     out["semi_planar_gbs"] = out["bytes_moved"] / out["semi_planar"] / 1e3
@@ -136,20 +130,15 @@ def batches(ctx, desc, n, w, h, seconds, rounds, generator):
         ways[semi_way]()
         ways[relaid_way]()
         torch.cuda.synchronize()
-        identical = identical and all(same(f.outputs(f.semi), f.outputs(f.relaid)) for f in frames)
-    out = {k: v / n for k, v in measure(ways, seconds, rounds).items()}  # per image
+        identical = identical and all(torch.equal(f.outputs(f.semi), f.outputs(f.relaid)) for f in frames)
+    out = median_us(ways, seconds, rounds, n)
     out["identical"] = identical
     return out
 
 
 def main():
-    parser = argparse.ArgumentParser()
-    parser.add_argument("--seconds", type=float, default=1.0)
-    parser.add_argument("--rounds", type=int, default=5)
-    parser.add_argument("--out")
-    args = parser.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("measure_semiplanar_encode.py needs a CUDA device")
+    args = harness.arguments(rounds=5).parse_args()
+    harness.require_gpu()
     generator = torch.Generator(device="cuda")
     generator.manual_seed(20261018)
     pq = abi.Nclx(1, abi.PRIMARIES_BT2020, abi.TRANSFER_CHAR_PQ, abi.MATRIX_BT2020_NCL, 1)
@@ -158,19 +147,14 @@ def main():
     p016 = abi.EncodeDesc(0, 0, 32, 3, abi.ALPHA_NONE, 12, abi.TRANSFER_PQ, 80, planar, abi.CHROMA_420, nclx=pq, dest_layout=NVMSB)
     p010a = abi.EncodeDesc(0, 0, 16, 4, abi.ALPHA_STRAIGHT, 10, abi.TRANSFER_CLIP, 80, planar, abi.CHROMA_420, nclx=pq, dest_layout=NVMSB)
     nv12 = abi.EncodeDesc(0, 0, 8, 3, abi.ALPHA_NONE, 8, abi.TRANSFER_CLIP, 80, planar, abi.CHROMA_420, nclx=bt709, dest_layout=NV)
-    result = {"card": card(), "unit": "microseconds per image (device events, median of rounds)"}
+    result = {"card": harness.card(), "unit": "microseconds per image (device events, median of rounds)"}
     with avifgpu.Context(0) as ctx:
         result["p016_4k"] = single(ctx, p016, 3840, 2160, args.seconds, args.rounds, generator)
         result["p016_8k"] = single(ctx, p016, 7680, 4320, args.seconds, args.rounds, generator)
         result["p010a_4k"] = single(ctx, p010a, 3840, 2160, args.seconds, args.rounds, generator)
         result["nv12_b64"] = batches(ctx, nv12, 64, 512, 512, args.seconds, args.rounds, generator)
         result["nv12_b256"] = batches(ctx, nv12, 256, 512, 512, args.seconds, args.rounds, generator)
-    line = json.dumps(result)
-    print(line)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
+    harness.emit([result], args.out)
 
 
 if __name__ == "__main__":

@@ -96,21 +96,12 @@ namespace
     // Two slots keep both copy engines busy; the third lets the host thread fill / drain a pinned bounce buffer
     // (pageable caller memory) while the other two are on the wire.
     constexpr int kPipelineStreams = 3;
-}
+    // A slot stages each plane k in its buffers k and the host rows in buffer kRowsBuffer.
+    constexpr int kRowsBuffer = AVIFGPU_MAX_PLANES;
+    constexpr int kSlotBuffers = AVIFGPU_MAX_PLANES + 1;
 
-struct avifgpu_context
-{
-    int device = -1;
-    cudaStream_t streams[kPipelineStreams] = {};
-    cudaEvent_t sliceDone[kPipelineStreams] = {};
-    cudaEvent_t rowsConsumed[kPipelineStreams] = {}; // encode: the slot's H2D of caller rows has finished
-    cudaEvent_t callRowsConsumed[2] = {};            // every H2D of an asynchronous encode call has finished (calls alternate between the two)
-    int64_t asyncEncodeCalls = 0;
-    bool previousCallRowsPending = false;            // callRowsConsumed[(asyncEncodeCalls - 1) & 1] guards caller memory still on the wire
-
-    // Work a slot still owes the caller once its stream has drained: copies from a pinned bounce buffer into pageable
-    // caller memory (libheif's planes on the encode side, pageable host rows on the decode side).
-    struct HostCopy
+    // `rows` rows of `payload` bytes from `source` to `target`.
+    struct RowCopy
     {
         uint8_t* target;
         int64_t targetStride;
@@ -119,31 +110,41 @@ struct avifgpu_context
         int64_t payload;
         int rows;
     };
-    struct SlotState
+}
+
+struct avifgpu_context
+{
+    int device = -1;
+    cudaEvent_t callRowsConsumed[2] = {};            // every H2D of an asynchronous encode call has finished (calls alternate between the two)
+    int64_t asyncEncodeCalls = 0;
+    bool previousCallRowsPending = false;            // callRowsConsumed[(asyncEncodeCalls - 1) & 1] guards caller memory still on the wire
+
+    struct Buffer
     {
+        void* ptr = nullptr;
+        size_t bytes = 0;
+    };
+    // One pipeline slot of the host-pointer entry points.  Its staging buffers are grow-only.
+    struct Slot
+    {
+        cudaStream_t stream = nullptr;
+        cudaEvent_t sliceDone = nullptr;
+        cudaEvent_t rowsConsumed = nullptr; // encode: the slot's H2D of caller rows has finished
         bool busy = false;
         int64_t ticket = 0;
-        std::vector<HostCopy> owed;
-        bool owesRows = false; // `owed` copies a decode's rows out of pinnedRows[slot]
+        Buffer device[kSlotBuffers];
+        Buffer pinned[kSlotBuffers]; // bounce buffers for pageable caller memory
+        // What the slot still owes the caller once its stream has drained: owed[b] copies pinned[b] into pageable caller
+        // memory (libheif's planes on the encode side, pageable host rows on the decode side); rows == 0 when nothing.
+        RowCopy owed[kSlotBuffers] = {};
     };
-    SlotState slots[kPipelineStreams];
+    Slot slots[kPipelineStreams];
     int nextSlot = 0;
     int64_t lastTicket = 0;       // ticket of the most recent host-pointer call
     std::string lastError;
     int64_t launches = 0;
     int smCount = 0;
 
-    // Device staging for the host-pointer entry points (grow-only).
-    struct Buffer
-    {
-        void* ptr = nullptr;
-        size_t bytes = 0;
-    };
-    Buffer deviceRows[kPipelineStreams];
-    Buffer devicePlanes[kPipelineStreams][AVIFGPU_MAX_PLANES];
-    // Pinned bounce buffers for pageable caller memory (grow-only).
-    Buffer pinnedRows[kPipelineStreams];
-    Buffer pinnedPlanes[kPipelineStreams][AVIFGPU_MAX_PLANES];
     Buffer transferScratch[2];
     std::vector<CurveTable*> curveTables; // exact step tables, built per (curve, param, depth): explicitly or once they pay off
     struct PendingTable
@@ -185,7 +186,7 @@ struct avifgpu_context
             {
                 return 0;
             }
-            premultiplyState[slot] = VerifyFastPremultiply((1u << d.image_bit_depth) - 1u, streams[0]) == 0 ? 1 : 0;
+            premultiplyState[slot] = VerifyFastPremultiply((1u << d.image_bit_depth) - 1u, slots[0].stream) == 0 ? 1 : 0;
             launches += 1;
         }
         return premultiplyState[slot];
@@ -202,7 +203,7 @@ struct avifgpu_context
             {
                 return 0;
             }
-            const long long disagreements = VerifyHlgDivisions(streams[0]);
+            const long long disagreements = VerifyHlgDivisions(slots[0].stream);
             hlgDivisionState = disagreements == 0 ? 1 : 0;
             launches += 1;
         }
@@ -220,7 +221,7 @@ struct avifgpu_context
             {
                 return 0;
             }
-            const long long disagreements = VerifyPqRatio(streams[0]);
+            const long long disagreements = VerifyPqRatio(slots[0].stream);
             pqRatioState = disagreements == 0 ? 1 : 0;
             launches += 1;
         }
@@ -258,7 +259,7 @@ struct avifgpu_context
         g.matrix = p.matrix;
         g.range = p.range;
         g.maxCode = p.maxCode;
-        g.state = VerifyGreenDivision(p, streams[0]) == 0 ? 1 : 0;
+        g.state = VerifyGreenDivision(p, slots[0].stream) == 0 ? 1 : 0;
         launches += 1;
         greenDivisions.push_back(g);
         return g.state;
@@ -291,8 +292,8 @@ struct avifgpu_context
             cudaGetLastError();
             return nullptr;
         }
-        if (BuildGray16Lut(lut.device, smpte428, (1u << d.image_bit_depth) - 1u, streams[0]) != cudaSuccess ||
-            cudaStreamSynchronize(streams[0]) != cudaSuccess)
+        if (BuildGray16Lut(lut.device, smpte428, (1u << d.image_bit_depth) - 1u, slots[0].stream) != cudaSuccess ||
+            cudaStreamSynchronize(slots[0].stream) != cudaSuccess)
         {
             cudaGetLastError();
             cudaFree(lut.device);
@@ -370,7 +371,7 @@ struct avifgpu_context
         {
             return nullptr;
         }
-        BuildCurveTable(curve, param, d.image_bit_depth, streams[0], t);
+        BuildCurveTable(curve, param, d.image_bit_depth, slots[0].stream, t);
         launches += t->stats.sweptInputs ? (t->stats.bandBitmapBytes ? 3 : 2) : 0; // sweep, (band bitmap,) verify
         curveTables.push_back(t);
         return t;
@@ -407,11 +408,11 @@ struct avifgpu_context
     int LaunchFailed(int status, const char* what, bool capturing = false)
     {
         const int code = TakeLaunchFailure();
-        for (cudaStream_t stream : streams)
+        for (const Slot& slot : slots)
         {
-            if (stream && !capturing)
+            if (slot.stream && !capturing)
             {
-                cudaStreamSynchronize(stream);
+                cudaStreamSynchronize(slot.stream);
             }
         }
         cudaGetLastError();
@@ -612,9 +613,10 @@ AVIFGPU_EXPORT int avifgpu_create(int device_ordinal, avifgpu_context** out_ctx)
     DeviceGuard guard(device_ordinal);
     for (int i = 0; i < kPipelineStreams; ++i)
     {
-        if (cudaStreamCreateWithFlags(&ctx->streams[i], cudaStreamNonBlocking) != cudaSuccess ||
-            cudaEventCreateWithFlags(&ctx->sliceDone[i], cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&ctx->rowsConsumed[i], cudaEventDisableTiming) != cudaSuccess ||
+        avifgpu_context::Slot& slot = ctx->slots[i];
+        if (cudaStreamCreateWithFlags(&slot.stream, cudaStreamNonBlocking) != cudaSuccess ||
+            cudaEventCreateWithFlags(&slot.sliceDone, cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&slot.rowsConsumed, cudaEventDisableTiming) != cudaSuccess ||
             (i < 2 && cudaEventCreateWithFlags(&ctx->callRowsConsumed[i], cudaEventDisableTiming) != cudaSuccess))
         {
             g_creationError = std::string("stream/event creation failed: ") + cudaGetErrorString(cudaGetLastError());
@@ -636,16 +638,15 @@ AVIFGPU_EXPORT void avifgpu_destroy(avifgpu_context* ctx)
     cudaDeviceSynchronize();
     for (int i = 0; i < kPipelineStreams; ++i)
     {
-        if (ctx->streams[i]) cudaStreamDestroy(ctx->streams[i]);
-        if (ctx->sliceDone[i]) cudaEventDestroy(ctx->sliceDone[i]);
-        if (ctx->rowsConsumed[i]) cudaEventDestroy(ctx->rowsConsumed[i]);
+        const avifgpu_context::Slot& slot = ctx->slots[i];
+        if (slot.stream) cudaStreamDestroy(slot.stream);
+        if (slot.sliceDone) cudaEventDestroy(slot.sliceDone);
+        if (slot.rowsConsumed) cudaEventDestroy(slot.rowsConsumed);
         if (i < 2 && ctx->callRowsConsumed[i]) cudaEventDestroy(ctx->callRowsConsumed[i]);
-        if (ctx->deviceRows[i].ptr) cudaFree(ctx->deviceRows[i].ptr);
-        if (ctx->pinnedRows[i].ptr) cudaFreeHost(ctx->pinnedRows[i].ptr);
-        for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
+        for (int b = 0; b < kSlotBuffers; ++b)
         {
-            if (ctx->devicePlanes[i][k].ptr) cudaFree(ctx->devicePlanes[i][k].ptr);
-            if (ctx->pinnedPlanes[i][k].ptr) cudaFreeHost(ctx->pinnedPlanes[i][k].ptr);
+            if (slot.device[b].ptr) cudaFree(slot.device[b].ptr);
+            if (slot.pinned[b].ptr) cudaFreeHost(slot.pinned[b].ptr);
         }
     }
     for (auto& b : ctx->transferScratch)
@@ -1255,9 +1256,12 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_indirect(avifgpu_context* ctx, const avi
 //
 // A call is cut into row-block slices; slice i uses pipeline slot i mod kPipelineStreams (a stream, device staging,
 // pinned bounce buffers).  Caller memory that is not page-locked is bounced through the slot's pinned buffers on BOTH
-// sides -- a copy to or from pageable memory would make the driver stage it synchronously and serialise the pipeline --
-// and the bounce -> pageable copies a slot still owes are made when the slot is retired (before it is reused, when a
-// call or a ticket is waited for).  Slots retire in issue order, so "everything up to ticket t" is a prefix.
+// sides -- a copy to or from pageable memory would make the driver stage it synchronously and serialise the pipeline.
+// The bounce -> pageable copies of a slot's last slice stay owed (its debts) until the slot's next slice or a retire
+// pays them.  Slots retire in issue order, so "everything up to ticket t" is a prefix.
+//
+// Both directions run a slice through the same steps: AcquireSlot, StageIn, the kernel launch, StageOut, CloseSlice.
+// Every pinned buffer those steps write into or regrow comes from TakePinned, which first pays the debts that read it.
 
 // Rows per pipeline slice: big enough to amortise launch + copy latency, small enough that the slots overlap.
 static int SliceRows(int nrows, int64_t bytesPerRow)
@@ -1288,16 +1292,6 @@ static void CopyRowsSerial(uint8_t* target, int64_t targetStride, const uint8_t*
 // rows that the threads -- and the caller -- pull from a common counter.
 namespace
 {
-    struct RowCopy
-    {
-        uint8_t* target;
-        int64_t targetStride;
-        const uint8_t* source;
-        int64_t sourceStride;
-        int64_t payload;
-        int rows;
-    };
-
     class CopyPool
     {
     public:
@@ -1429,61 +1423,39 @@ namespace
     };
 }
 
-static void CopyRows(uint8_t* target, int64_t targetStride, const uint8_t* source, int64_t sourceStride, int64_t payload, int rows)
-{
-    const RowCopy one{ target, targetStride, source, sourceStride, payload, rows };
-    CopyPool::Instance().Copy(&one, 1);
-}
+using Slot = avifgpu_context::Slot;
 
 // Waits for the slot's stream work (its device buffers are free again after this); what it owes the caller stays owed.
-static int WaitSlot(avifgpu_context* ctx, int slot)
+static int WaitSlot(avifgpu_context* ctx, Slot& slot)
 {
-    avifgpu_context::SlotState& state = ctx->slots[slot];
-    if (!state.busy)
+    if (!slot.busy)
     {
         return AVIFGPU_OK;
     }
-    const int status = ctx->Cuda(cudaEventSynchronize(ctx->sliceDone[slot]), "cudaEventSynchronize");
+    const int status = ctx->Cuda(cudaEventSynchronize(slot.sliceDone), "cudaEventSynchronize");
     if (status != AVIFGPU_OK)
     {
-        state.owed.clear();
-        state.owesRows = false;
+        for (RowCopy& c : slot.owed) c.rows = 0;
     }
-    state.busy = false;
+    slot.busy = false;
     return status;
 }
 
-// Pays what a waited-for slot owes the caller: the copies out of its pinned bounce buffers.
-static void PayOwed(avifgpu_context* ctx, int slot)
+// Pays, in one batch for the copy pool, what a waited-for slot owes out of the pinned buffers marked in `buffers` (out
+// of all of them when nullptr).  Separate batches would cost a wake-up and a wait each.
+static void PayDebts(Slot& slot, const bool* buffers = nullptr)
 {
-    avifgpu_context::SlotState& state = ctx->slots[slot];
-    if (!state.owed.empty())
+    RowCopy batch[kSlotBuffers];
+    int count = 0;
+    for (int b = 0; b < kSlotBuffers; ++b)
     {
-        RowCopy batch[AVIFGPU_MAX_PLANES + 1];
-        int count = 0;
-        for (const avifgpu_context::HostCopy& c : state.owed)
+        if (slot.owed[b].rows > 0 && (buffers == nullptr || buffers[b]))
         {
-            if (count == AVIFGPU_MAX_PLANES + 1)
-            {
-                CopyPool::Instance().Copy(batch, count);
-                count = 0;
-            }
-            batch[count++] = RowCopy{ c.target, c.targetStride, c.source, c.sourceStride, c.payload, c.rows };
+            batch[count++] = slot.owed[b];
+            slot.owed[b].rows = 0;
         }
-        CopyPool::Instance().Copy(batch, count); // all planes of the slice share the pool's threads
     }
-    state.owed.clear();
-    state.owesRows = false;
-}
-
-static int RetireSlot(avifgpu_context* ctx, int slot)
-{
-    const int status = WaitSlot(ctx, slot);
-    if (status == AVIFGPU_OK)
-    {
-        PayOwed(ctx, slot);
-    }
-    return status;
+    if (count > 0) CopyPool::Instance().Copy(batch, count); // the pool's threads start at the first copy
 }
 
 // Retires, oldest first, every slot issued by a call with ticket <= `ticket`.
@@ -1492,11 +1464,14 @@ static int RetireThrough(avifgpu_context* ctx, int64_t ticket)
     int result = AVIFGPU_OK;
     for (int i = 0; i < kPipelineStreams; ++i)
     {
-        const int slot = (ctx->nextSlot + i) % kPipelineStreams; // nextSlot is the oldest
-        if ((ctx->slots[slot].busy || !ctx->slots[slot].owed.empty()) && ctx->slots[slot].ticket <= ticket)
+        Slot& slot = ctx->slots[(ctx->nextSlot + i) % kPipelineStreams]; // nextSlot is the oldest
+        bool owes = false;
+        for (const RowCopy& c : slot.owed) owes = owes || c.rows > 0;
+        if ((slot.busy || owes) && slot.ticket <= ticket)
         {
-            const int status = RetireSlot(ctx, slot);
-            if (result == AVIFGPU_OK) result = status;
+            const int status = WaitSlot(ctx, slot);
+            if (status == AVIFGPU_OK) PayDebts(slot);
+            else if (result == AVIFGPU_OK) result = status;
         }
     }
     return result;
@@ -1504,36 +1479,186 @@ static int RetireThrough(avifgpu_context* ctx, int64_t ticket)
 
 // Every host-pointer call that returns AVIFGPU_OK hands the rows of the previous asynchronous encode call back to the
 // caller (avifgpu.h).  A call takes that release before it queues its own copies and waits for those rows' H2Ds just
-// before it returns, so the link never idles at a call boundary.
-struct RowsRelease
+// before it returns (FinishCall), so the link never idles at a call boundary.  Returns the callRowsConsumed event to
+// wait for, or -1.
+static int TakeRowsRelease(avifgpu_context* ctx)
 {
-    bool pending;
-    int event; // callRowsConsumed[event]
-};
-
-static RowsRelease TakeRowsRelease(avifgpu_context* ctx)
-{
-    const RowsRelease release{ ctx->previousCallRowsPending, static_cast<int>((ctx->asyncEncodeCalls - 1) & 1) };
+    const int event = ctx->previousCallRowsPending ? static_cast<int>((ctx->asyncEncodeCalls - 1) & 1) : -1;
     ctx->previousCallRowsPending = false;
-    return release;
-}
-
-static int FinishRowsRelease(avifgpu_context* ctx, RowsRelease release)
-{
-    return release.pending ? ctx->Cuda(cudaEventSynchronize(ctx->callRowsConsumed[release.event]), "cudaEventSynchronize") : AVIFGPU_OK;
+    return event;
 }
 
 // A failure in the middle of a call: nothing of this context may still be writing into caller memory on return.
 static int AbandonCall(avifgpu_context* ctx, int status)
 {
-    for (int i = 0; i < kPipelineStreams; ++i)
+    for (Slot& slot : ctx->slots)
     {
-        cudaStreamSynchronize(ctx->streams[i]);
-        ctx->slots[i].owed.clear();
-        ctx->slots[i].owesRows = false;
-        ctx->slots[i].busy = false;
+        cudaStreamSynchronize(slot.stream);
+        for (RowCopy& c : slot.owed) c.rows = 0;
+        slot.busy = false;
     }
     cudaGetLastError();
+    return status;
+}
+
+// The end of a call that has queued all its slices, or had none: release the previous asynchronous encode's rows, then
+// retire the call's slots if the call waits.
+static int FinishCall(avifgpu_context* ctx, int previousRows, int64_t ticket, bool wait)
+{
+    int status = previousRows < 0 ? AVIFGPU_OK : ctx->Cuda(cudaEventSynchronize(ctx->callRowsConsumed[previousRows]), "cudaEventSynchronize");
+    if (status == AVIFGPU_OK && wait)
+    {
+        status = RetireThrough(ctx, ticket);
+    }
+    return status == AVIFGPU_OK ? AVIFGPU_OK : AbandonCall(ctx, status);
+}
+
+// One host <-> device copy of a slice, between caller memory and the slot's buffers number `buffer`.
+struct SliceCopy
+{
+    int buffer;          // a plane index, or kRowsBuffer
+    uint8_t* host;       // the slice's first row in caller memory
+    int64_t hostStride;
+    bool hostPinned;     // false: the copy bounces through the slot's pinned buffer
+    int64_t payload;     // bytes per row
+    int64_t deviceStride;
+    int rows;
+};
+
+// Fills `windows` with the rows of each present whole-image plane that the slice of image rows [yFirst, yFirst + rows)
+// covers, and returns how many planes there are.
+static int PlaneWindows(const avifgpu_planes* planes, const PlaneGeometry* geometry, const bool* pinned, int yFirst, int rows, SliceCopy* windows)
+{
+    int count = 0;
+    for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
+    {
+        const PlaneGeometry& g = geometry[k];
+        if (g.present)
+        {
+            const int firstRow = yFirst >> g.ys;
+            const int64_t payload = static_cast<int64_t>(g.widthSamples) * g.bytesPerSample;
+            windows[count++] = SliceCopy{ k, static_cast<uint8_t*>(planes->data[k]) + static_cast<int64_t>(firstRow) * planes->stride[k], planes->stride[k],
+                                          pinned[k], payload, (payload + 255) & ~255ll, ((yFirst + rows - 1) >> g.ys) - firstRow + 1 };
+        }
+    }
+    return count;
+}
+
+static int EnsureDeviceStaging(avifgpu_context* ctx, Slot& slot, const SliceCopy* copies, int count)
+{
+    for (int i = 0; i < count; ++i)
+    {
+        const int status = ctx->EnsureDevice(slot.device[copies[i].buffer], static_cast<size_t>(copies[i].deviceStride) * copies[i].rows);
+        if (status != AVIFGPU_OK) return status;
+    }
+    return AVIFGPU_OK;
+}
+
+// Hands out, grown to fit, the slot's pinned buffers that the pageable sides of `copies` bounce through: the only way
+// to a pinned buffer that the host or the device is about to write.  It first pays, in one batch, the debts that read
+// those buffers, so no pinned buffer is written or regrown while the slot owes copies out of it.
+static int TakePinned(avifgpu_context* ctx, Slot& slot, const SliceCopy* copies, int count, uint8_t* pinned[kSlotBuffers])
+{
+    bool taken[kSlotBuffers] = {};
+    for (int i = 0; i < count; ++i)
+    {
+        taken[copies[i].buffer] = !copies[i].hostPinned;
+    }
+    PayDebts(slot, taken);
+    for (int i = 0; i < count; ++i)
+    {
+        const SliceCopy& c = copies[i];
+        if (!c.hostPinned)
+        {
+            const int status = ctx->EnsurePinned(slot.pinned[c.buffer], static_cast<size_t>(c.payload) * c.rows);
+            if (status != AVIFGPU_OK) return status;
+            pinned[c.buffer] = static_cast<uint8_t*>(slot.pinned[c.buffer].ptr);
+        }
+    }
+    return AVIFGPU_OK;
+}
+
+// Waits for the next slot in rotation and takes it for a slice; what the slot owes is paid by StageIn and StageOut.
+static int AcquireSlot(avifgpu_context* ctx, int* slot)
+{
+    *slot = ctx->nextSlot;
+    const int status = WaitSlot(ctx, ctx->slots[*slot]);
+    if (status == AVIFGPU_OK)
+    {
+        ctx->nextSlot = (*slot + 1) % kPipelineStreams;
+    }
+    return status;
+}
+
+// Queues a slice's host -> device copies on the slot's stream.  Pageable sources are bounced first, every one of the
+// slice in ONE batch for the copy pool (three batches for three planes cost three wake-ups and waits, ~0.5 ms per slice,
+// ahead of anything the GPU could do).
+static int StageIn(avifgpu_context* ctx, Slot& slot, const SliceCopy* copies, int count)
+{
+    uint8_t* pinned[kSlotBuffers] = {};
+    int status = EnsureDeviceStaging(ctx, slot, copies, count);
+    if (status != AVIFGPU_OK || (status = TakePinned(ctx, slot, copies, count, pinned)) != AVIFGPU_OK) return status;
+    RowCopy bounce[kSlotBuffers];
+    int bounced = 0;
+    for (int i = 0; i < count; ++i)
+    {
+        const SliceCopy& c = copies[i];
+        if (!c.hostPinned)
+        {
+            bounce[bounced++] = RowCopy{ pinned[c.buffer], c.payload, c.host, c.hostStride, c.payload, c.rows };
+        }
+    }
+    if (bounced > 0) CopyPool::Instance().Copy(bounce, bounced);
+    for (int i = 0; i < count; ++i)
+    {
+        const SliceCopy& c = copies[i];
+        const uint8_t* source = c.hostPinned ? c.host : pinned[c.buffer];
+        const int64_t sourceStride = c.hostPinned ? c.hostStride : c.payload;
+        if ((status = ctx->Cuda(cudaMemcpy2DAsync(slot.device[c.buffer].ptr, static_cast<size_t>(c.deviceStride), source,
+                                                  static_cast<size_t>(sourceStride), static_cast<size_t>(c.payload),
+                                                  static_cast<size_t>(c.rows), cudaMemcpyHostToDevice, slot.stream),
+                                c.buffer == kRowsBuffer ? "H2D rows" : "H2D plane")) != AVIFGPU_OK) return status;
+    }
+    return AVIFGPU_OK;
+}
+
+// Queues a slice's device -> host copies on the slot's stream, once everything the slot still owes is paid (in one
+// batch): paid here, after the slice's H2Ds and kernel are queued, the host copies while the link and the SMs work.  A
+// pageable target gets its rows in the slot's pinned buffer, and the copy across becomes a debt of the slot.
+static int StageOut(avifgpu_context* ctx, Slot& slot, const SliceCopy* copies, int count)
+{
+    PayDebts(slot);
+    uint8_t* pinned[kSlotBuffers] = {};
+    int status = TakePinned(ctx, slot, copies, count, pinned);
+    if (status != AVIFGPU_OK) return status;
+    for (int i = 0; i < count; ++i)
+    {
+        const SliceCopy& c = copies[i];
+        uint8_t* target = c.host;
+        int64_t targetStride = c.hostStride;
+        if (!c.hostPinned)
+        {
+            slot.owed[c.buffer] = RowCopy{ c.host, c.hostStride, pinned[c.buffer], c.payload, c.payload, c.rows };
+            target = pinned[c.buffer];
+            targetStride = c.payload;
+        }
+        if ((status = ctx->Cuda(cudaMemcpy2DAsync(target, static_cast<size_t>(targetStride), slot.device[c.buffer].ptr,
+                                                  static_cast<size_t>(c.deviceStride), static_cast<size_t>(c.payload),
+                                                  static_cast<size_t>(c.rows), cudaMemcpyDeviceToHost, slot.stream),
+                                c.buffer == kRowsBuffer ? "D2H rows" : "D2H plane")) != AVIFGPU_OK) return status;
+    }
+    return AVIFGPU_OK;
+}
+
+// Marks the end of the slice queued on the slot's stream; the slot belongs to the call with `ticket` until retired.
+static int CloseSlice(avifgpu_context* ctx, Slot& slot, int64_t ticket)
+{
+    const int status = ctx->Cuda(cudaEventRecord(slot.sliceDone, slot.stream), "cudaEventRecord");
+    if (status == AVIFGPU_OK)
+    {
+        slot.busy = true;
+        slot.ticket = ticket;
+    }
     return status;
 }
 
@@ -1575,8 +1700,7 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
     DeviceGuard guard(ctx->device);
     if (nrows == 0 || desc->width == 0)
     {
-        if ((status = FinishRowsRelease(ctx, TakeRowsRelease(ctx))) != AVIFGPU_OK) return status;
-        return wait ? RetireThrough(ctx, ticket) : AVIFGPU_OK;
+        return FinishCall(ctx, TakeRowsRelease(ctx), ticket, wait);
     }
     PlaneGeometry geometry[AVIFGPU_MAX_PLANES];
     bool planePinned[AVIFGPU_MAX_PLANES] = {};
@@ -1596,44 +1720,24 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
     const int64_t deviceRowStride = (rowPayload + 255) & ~255ll;
     const bool rowsPinned = IsPinned(host_rows);
     const int sliceRows = SliceRows(nrows, rowPayload);
+    uint8_t* rowsIn = static_cast<uint8_t*>(const_cast<void*>(host_rows)); // only ever read
 
-    const RowsRelease previousRows = TakeRowsRelease(ctx);
+    const int previousRows = TakeRowsRelease(ctx);
     bool recordedCallRows = false;
     bool callSlots[kPipelineStreams] = {}; // the slots this call's H2Ds went through
 
     for (int begin = 0; begin < nrows; begin += sliceRows)
     {
         const int rows = std::min(sliceRows, nrows - begin);
-        const int slot = ctx->nextSlot;
-        cudaStream_t stream = ctx->streams[slot];
-        // The slot's previous slice: wait for the GPU, but pay an encode's plane copies only after this slice's H2D and
-        // kernel are queued -- the host then copies while the link and the SMs work (its D2H, which reuses the plane
-        // bounce buffers, comes last).  A decode's rows are paid first: this slice's rows land in (and may regrow) the
-        // same pinned buffer.
-        if ((status = WaitSlot(ctx, slot)) != AVIFGPU_OK) return AbandonCall(ctx, status);
-        if (ctx->slots[slot].owesRows)
-        {
-            PayOwed(ctx, slot);
-        }
-        ctx->nextSlot = (slot + 1) % kPipelineStreams;
-
-        if ((status = ctx->EnsureDevice(ctx->deviceRows[slot], static_cast<size_t>(deviceRowStride) * rows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
-        const uint8_t* source = static_cast<const uint8_t*>(host_rows) + static_cast<int64_t>(begin) * row_stride_bytes;
-        int64_t sourceStride = row_stride_bytes;
-        if (!rowsPinned)
-        {
-            if ((status = ctx->EnsurePinned(ctx->pinnedRows[slot], static_cast<size_t>(rowPayload) * rows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
-            uint8_t* bounce = static_cast<uint8_t*>(ctx->pinnedRows[slot].ptr);
-            CopyRows(bounce, rowPayload, source, row_stride_bytes, rowPayload, rows);
-            source = bounce;
-            sourceStride = rowPayload;
-        }
-        if ((status = ctx->Cuda(cudaMemcpy2DAsync(ctx->deviceRows[slot].ptr, static_cast<size_t>(deviceRowStride), source,
-                                                  static_cast<size_t>(sourceStride), static_cast<size_t>(rowPayload),
-                                                  static_cast<size_t>(rows), cudaMemcpyHostToDevice, stream),
-                                "H2D rows")) != AVIFGPU_OK) return AbandonCall(ctx, status);
-        if ((status = ctx->Cuda(cudaEventRecord(ctx->rowsConsumed[slot], stream), "cudaEventRecord")) != AVIFGPU_OK) return AbandonCall(ctx, status);
-        callSlots[slot] = true;
+        int index;
+        if ((status = AcquireSlot(ctx, &index)) != AVIFGPU_OK) return AbandonCall(ctx, status);
+        Slot& slot = ctx->slots[index];
+        const SliceCopy in{ kRowsBuffer, rowsIn + static_cast<int64_t>(begin) * row_stride_bytes, row_stride_bytes, rowsPinned, rowPayload, deviceRowStride, rows };
+        SliceCopy out[AVIFGPU_MAX_PLANES];
+        const int planes = PlaneWindows(dst, geometry, planePinned, y0 + begin, rows, out);
+        if ((status = StageIn(ctx, slot, &in, 1)) != AVIFGPU_OK ||
+            (status = ctx->Cuda(cudaEventRecord(slot.rowsConsumed, slot.stream), "cudaEventRecord")) != AVIFGPU_OK) return AbandonCall(ctx, status);
+        callSlots[index] = true;
         if (!wait && rowsPinned && begin + sliceRows >= nrows)
         {
             // The caller's own memory is on the wire until every H2D of the call has finished, and the H2Ds of different
@@ -1641,82 +1745,39 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
             // event the NEXT call waits for.
             for (int s = 0; s < kPipelineStreams; ++s)
             {
-                if (s != slot && callSlots[s] &&
-                    (status = ctx->Cuda(cudaStreamWaitEvent(stream, ctx->rowsConsumed[s], 0), "cudaStreamWaitEvent")) != AVIFGPU_OK) return AbandonCall(ctx, status);
+                if (s != index && callSlots[s] &&
+                    (status = ctx->Cuda(cudaStreamWaitEvent(slot.stream, ctx->slots[s].rowsConsumed, 0), "cudaStreamWaitEvent")) != AVIFGPU_OK) return AbandonCall(ctx, status);
             }
-            if ((status = ctx->Cuda(cudaEventRecord(ctx->callRowsConsumed[ctx->asyncEncodeCalls & 1], stream), "cudaEventRecord")) != AVIFGPU_OK) return AbandonCall(ctx, status);
+            if ((status = ctx->Cuda(cudaEventRecord(ctx->callRowsConsumed[ctx->asyncEncodeCalls & 1], slot.stream), "cudaEventRecord")) != AVIFGPU_OK) return AbandonCall(ctx, status);
             recordedCallRows = true;
         }
 
+        if ((status = EnsureDeviceStaging(ctx, slot, out, planes)) != AVIFGPU_OK) return AbandonCall(ctx, status);
         EncodeParams p = base;
-        p.rows = ctx->deviceRows[slot].ptr;
+        p.rows = slot.device[kRowsBuffer].ptr;
         p.rowStride = deviceRowStride;
         p.rowCount = rows;
-        int64_t planeStride[AVIFGPU_MAX_PLANES] = {};
-        int planeRows[AVIFGPU_MAX_PLANES] = {};
-        int64_t planePayload[AVIFGPU_MAX_PLANES] = {};
-        for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
+        for (int i = 0; i < planes; ++i)
         {
-            const PlaneGeometry& g = geometry[k];
-            if (!g.present)
-            {
-                continue;
-            }
-            planePayload[k] = static_cast<int64_t>(g.widthSamples) * g.bytesPerSample;
-            planeStride[k] = (planePayload[k] + 255) & ~255ll;
-            planeRows[k] = (rows + g.ys) >> g.ys;
-            if ((status = ctx->EnsureDevice(ctx->devicePlanes[slot][k], static_cast<size_t>(planeStride[k]) * planeRows[k])) != AVIFGPU_OK) return AbandonCall(ctx, status);
-            p.plane[k] = ctx->devicePlanes[slot][k].ptr;
-            p.planeStride[k] = planeStride[k];
+            p.plane[out[i].buffer] = slot.device[out[i].buffer].ptr;
+            p.planeStride[out[i].buffer] = out[i].deviceStride;
         }
-        const int launched = LaunchEncode(p, desc->host_depth, stream);
+        const int launched = LaunchEncode(p, desc->host_depth, slot.stream);
         if (launched < 0)
         {
             return AbandonCall(ctx, ctx->LaunchFailed(launched, "encode kernel launch"));
         }
         ctx->launches += launched;
 
-        PayOwed(ctx, slot); // the previous slice's planes leave the bounce buffers now
-        avifgpu_context::SlotState& state = ctx->slots[slot];
-        for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
-        {
-            const PlaneGeometry& g = geometry[k];
-            if (!g.present)
-            {
-                continue;
-            }
-            uint8_t* target = static_cast<uint8_t*>(dst->data[k]) + static_cast<int64_t>((y0 + begin) >> g.ys) * dst->stride[k];
-            int64_t targetStride = dst->stride[k];
-            if (!planePinned[k])
-            {
-                // pageable plane (libheif's): land in pinned memory now, copy across when the slot retires
-                if ((status = ctx->EnsurePinned(ctx->pinnedPlanes[slot][k], static_cast<size_t>(planePayload[k]) * planeRows[k])) != AVIFGPU_OK) return AbandonCall(ctx, status);
-                uint8_t* bounce = static_cast<uint8_t*>(ctx->pinnedPlanes[slot][k].ptr);
-                state.owed.push_back(avifgpu_context::HostCopy{ target, dst->stride[k], bounce, planePayload[k], planePayload[k], planeRows[k] });
-                target = bounce;
-                targetStride = planePayload[k];
-            }
-            if ((status = ctx->Cuda(cudaMemcpy2DAsync(target, static_cast<size_t>(targetStride), p.plane[k],
-                                                      static_cast<size_t>(planeStride[k]), static_cast<size_t>(planePayload[k]),
-                                                      static_cast<size_t>(planeRows[k]), cudaMemcpyDeviceToHost, stream),
-                                    "D2H plane")) != AVIFGPU_OK) return AbandonCall(ctx, status);
-        }
-        if ((status = ctx->Cuda(cudaEventRecord(ctx->sliceDone[slot], stream), "cudaEventRecord")) != AVIFGPU_OK) return AbandonCall(ctx, status);
-        state.busy = true;
-        state.ticket = ticket;
+        if ((status = StageOut(ctx, slot, out, planes)) != AVIFGPU_OK || (status = CloseSlice(ctx, slot, ticket)) != AVIFGPU_OK) return AbandonCall(ctx, status);
     }
-    if ((status = FinishRowsRelease(ctx, previousRows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
-    if (wait)
-    {
-        status = RetireThrough(ctx, ticket);
-        return status == AVIFGPU_OK ? AVIFGPU_OK : AbandonCall(ctx, status);
-    }
-    if (recordedCallRows)
+    status = FinishCall(ctx, previousRows, ticket, wait);
+    if (status == AVIFGPU_OK && !wait && recordedCallRows)
     {
         ctx->asyncEncodeCalls += 1;
         ctx->previousCallRowsPending = true;
     }
-    return AVIFGPU_OK;
+    return status;
 }
 
 static int DecodeRowsHost(avifgpu_context* ctx, const avifgpu_decode_desc* desc, const avifgpu_planes* src, int32_t y0, int32_t nrows,
@@ -1760,8 +1821,7 @@ static int DecodeRowsHost(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
     DeviceGuard guard(ctx->device);
     if (nrows == 0 || desc->width == 0)
     {
-        if ((status = FinishRowsRelease(ctx, TakeRowsRelease(ctx))) != AVIFGPU_OK) return status;
-        return wait ? RetireThrough(ctx, ticket) : AVIFGPU_OK;
+        return FinishCall(ctx, TakeRowsRelease(ctx), ticket, wait);
     }
     PlaneGeometry geometry[AVIFGPU_MAX_PLANES];
     bool planePinned[AVIFGPU_MAX_PLANES] = {};
@@ -1780,111 +1840,41 @@ static int DecodeRowsHost(avifgpu_context* ctx, const avifgpu_decode_desc* desc,
     const int64_t deviceRowStride = (rowPayload + 255) & ~255ll;
     const int sliceRows = SliceRows(nrows, rowPayload);
     const bool rowsPinned = IsPinned(host_rows);
-    const RowsRelease previousRows = TakeRowsRelease(ctx);
+    const int previousRows = TakeRowsRelease(ctx);
 
     for (int begin = 0; begin < nrows; begin += sliceRows)
     {
         const int rows = std::min(sliceRows, nrows - begin);
-        const int slot = ctx->nextSlot;
-        cudaStream_t stream = ctx->streams[slot];
-        if ((status = RetireSlot(ctx, slot)) != AVIFGPU_OK) return AbandonCall(ctx, status);
-        ctx->nextSlot = (slot + 1) % kPipelineStreams;
-
+        int index;
+        if ((status = AcquireSlot(ctx, &index)) != AVIFGPU_OK) return AbandonCall(ctx, status);
+        Slot& slot = ctx->slots[index];
         const int yFirst = y0 + begin;
+        SliceCopy in[AVIFGPU_MAX_PLANES];
+        const int planes = PlaneWindows(src, geometry, planePinned, yFirst, rows, in);
+        const SliceCopy out{ kRowsBuffer, static_cast<uint8_t*>(host_rows) + static_cast<int64_t>(begin) * row_stride_bytes, row_stride_bytes, rowsPinned, rowPayload, deviceRowStride, rows };
+        if ((status = StageIn(ctx, slot, in, planes)) != AVIFGPU_OK ||
+            (status = EnsureDeviceStaging(ctx, slot, &out, 1)) != AVIFGPU_OK) return AbandonCall(ctx, status);
         DecodeParams p = base;
         p.rowCount = rows;
         p.yPhase = yFirst & p.ys;
         p.smCount = ctx->smCount;
-        // pageable planes (libheif's) go through the slot's pinned buffers: every plane of the slice in ONE batch for the copy
-        // pool (three separate batches cost three wake-ups and waits per slice, ~0.5 ms, ahead of anything the GPU could do)
-        struct PlaneStage
+        for (int i = 0; i < planes; ++i)
         {
-            const uint8_t* source;
-            int64_t sourceStride, payload, stride;
-            int planeRows;
-        } stage[AVIFGPU_MAX_PLANES] = {};
-        RowCopy bounceBatch[AVIFGPU_MAX_PLANES];
-        int bounceCount = 0;
-        for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
-        {
-            const PlaneGeometry& g = geometry[k];
-            if (!g.present)
-            {
-                continue;
-            }
-            const int firstRow = yFirst >> g.ys;
-            const int lastRow = (yFirst + rows - 1) >> g.ys;
-            PlaneStage& st = stage[k];
-            st.planeRows = lastRow - firstRow + 1;
-            st.payload = static_cast<int64_t>(g.widthSamples) * g.bytesPerSample;
-            st.stride = (st.payload + 255) & ~255ll;
-            if ((status = ctx->EnsureDevice(ctx->devicePlanes[slot][k], static_cast<size_t>(st.stride) * st.planeRows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
-            st.source = static_cast<const uint8_t*>(src->data[k]) + static_cast<int64_t>(firstRow) * src->stride[k];
-            st.sourceStride = src->stride[k];
-            if (!planePinned[k])
-            {
-                if ((status = ctx->EnsurePinned(ctx->pinnedPlanes[slot][k], static_cast<size_t>(st.payload) * st.planeRows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
-                uint8_t* bounce = static_cast<uint8_t*>(ctx->pinnedPlanes[slot][k].ptr);
-                bounceBatch[bounceCount++] = RowCopy{ bounce, st.payload, st.source, st.sourceStride, st.payload, st.planeRows };
-                st.source = bounce;
-                st.sourceStride = st.payload;
-            }
+            p.plane[in[i].buffer] = slot.device[in[i].buffer].ptr;
+            p.planeStride[in[i].buffer] = in[i].deviceStride;
         }
-        if (bounceCount > 0)
-        {
-            CopyPool::Instance().Copy(bounceBatch, bounceCount);
-        }
-        for (int k = 0; k < AVIFGPU_MAX_PLANES; ++k)
-        {
-            if (!geometry[k].present)
-            {
-                continue;
-            }
-            const PlaneStage& st = stage[k];
-            if ((status = ctx->Cuda(cudaMemcpy2DAsync(ctx->devicePlanes[slot][k].ptr, static_cast<size_t>(st.stride), st.source,
-                                                      static_cast<size_t>(st.sourceStride), static_cast<size_t>(st.payload),
-                                                      static_cast<size_t>(st.planeRows), cudaMemcpyHostToDevice, stream),
-                                    "H2D plane")) != AVIFGPU_OK) return AbandonCall(ctx, status);
-            p.plane[k] = ctx->devicePlanes[slot][k].ptr;
-            p.planeStride[k] = st.stride;
-        }
-        if ((status = ctx->EnsureDevice(ctx->deviceRows[slot], static_cast<size_t>(deviceRowStride) * rows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
-        p.rows = ctx->deviceRows[slot].ptr;
+        p.rows = slot.device[kRowsBuffer].ptr;
         p.rowStride = deviceRowStride;
-        const int launched = LaunchDecode(p, stream);
+        const int launched = LaunchDecode(p, slot.stream);
         if (launched < 0)
         {
             return AbandonCall(ctx, ctx->LaunchFailed(launched, "decode kernel launch"));
         }
         ctx->launches += launched;
 
-        avifgpu_context::SlotState& state = ctx->slots[slot];
-        uint8_t* target = static_cast<uint8_t*>(host_rows) + static_cast<int64_t>(begin) * row_stride_bytes;
-        int64_t targetStride = row_stride_bytes;
-        if (!rowsPinned)
-        {
-            if ((status = ctx->EnsurePinned(ctx->pinnedRows[slot], static_cast<size_t>(rowPayload) * rows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
-            uint8_t* bounce = static_cast<uint8_t*>(ctx->pinnedRows[slot].ptr);
-            state.owed.push_back(avifgpu_context::HostCopy{ target, row_stride_bytes, bounce, rowPayload, rowPayload, rows });
-            state.owesRows = true;
-            target = bounce;
-            targetStride = rowPayload;
-        }
-        if ((status = ctx->Cuda(cudaMemcpy2DAsync(target, static_cast<size_t>(targetStride), ctx->deviceRows[slot].ptr,
-                                                  static_cast<size_t>(deviceRowStride), static_cast<size_t>(rowPayload),
-                                                  static_cast<size_t>(rows), cudaMemcpyDeviceToHost, stream),
-                                "D2H rows")) != AVIFGPU_OK) return AbandonCall(ctx, status);
-        if ((status = ctx->Cuda(cudaEventRecord(ctx->sliceDone[slot], stream), "cudaEventRecord")) != AVIFGPU_OK) return AbandonCall(ctx, status);
-        state.busy = true;
-        state.ticket = ticket;
+        if ((status = StageOut(ctx, slot, &out, 1)) != AVIFGPU_OK || (status = CloseSlice(ctx, slot, ticket)) != AVIFGPU_OK) return AbandonCall(ctx, status);
     }
-    if ((status = FinishRowsRelease(ctx, previousRows)) != AVIFGPU_OK) return AbandonCall(ctx, status);
-    if (wait)
-    {
-        status = RetireThrough(ctx, ticket);
-        return status == AVIFGPU_OK ? AVIFGPU_OK : AbandonCall(ctx, status);
-    }
-    return AVIFGPU_OK;
+    return FinishCall(ctx, previousRows, ticket, wait);
 }
 
 extern "C" {
@@ -2238,7 +2228,7 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_device(avifgpu_shard_group* group
         }
         avifgpu_context* ctx = group->members[r];
         const int status = avifgpu_encode_rows_device(ctx, desc, device_rows[r], row_stride_bytes[r], blockY0[r], blockRows[r], owner_planes,
-                                                      ctx->streams[0]);
+                                                      ctx->slots[0].stream);
         if (status != AVIFGPU_OK)
         {
             return group->Fail(status, "member " + std::to_string(r) + ": " + ctx->lastError);
@@ -2350,7 +2340,7 @@ AVIFGPU_EXPORT int avifgpu_transfer_f32(avifgpu_context* ctx, int32_t function, 
     const size_t bytes = n * sizeof(float);
     if ((status = ctx->EnsureDevice(ctx->transferScratch[0], bytes)) != AVIFGPU_OK) return status;
     if ((status = ctx->EnsureDevice(ctx->transferScratch[1], bytes)) != AVIFGPU_OK) return status;
-    cudaStream_t stream = ctx->streams[0];
+    cudaStream_t stream = ctx->slots[0].stream;
     if ((status = ctx->Cuda(cudaMemcpyAsync(ctx->transferScratch[0].ptr, in, bytes, cudaMemcpyHostToDevice, stream), "H2D")) != AVIFGPU_OK) return status;
     const int launched = LaunchTransfer(function, param, static_cast<const float*>(ctx->transferScratch[0].ptr),
                                         static_cast<float*>(ctx->transferScratch[1].ptr), n, stream);
@@ -2388,7 +2378,7 @@ AVIFGPU_EXPORT int avifgpu_hlg_ootf_f32(avifgpu_context* ctx, int32_t inverse, i
     const size_t bytes = pixels * 3 * sizeof(float);
     if ((status = ctx->EnsureDevice(ctx->transferScratch[0], bytes)) != AVIFGPU_OK) return status;
     if ((status = ctx->EnsureDevice(ctx->transferScratch[1], bytes)) != AVIFGPU_OK) return status;
-    cudaStream_t stream = ctx->streams[0];
+    cudaStream_t stream = ctx->slots[0].stream;
     if ((status = ctx->Cuda(cudaMemcpyAsync(ctx->transferScratch[0].ptr, rgb_in, bytes, cudaMemcpyHostToDevice, stream), "H2D")) != AVIFGPU_OK) return status;
     const int launched = LaunchHlgOotf(inverse != 0, luma, display_gamma, nominal_peak_nits, static_cast<const float*>(ctx->transferScratch[0].ptr),
                                        static_cast<float*>(ctx->transferScratch[1].ptr), pixels, stream);

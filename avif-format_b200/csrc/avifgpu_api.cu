@@ -43,25 +43,29 @@ static int TakeLaunchFailure()
     return code;
 }
 
-int LaunchEncode(const EncodeParams& params, int hostDepth, void* stream)
+int LaunchEncode(const EncodeParams& params, int hostDepth, void* stream, const LightSink* light)
 {
-    const EncodeFamily family = EncodeFamilyOf(params, hostDepth);
+    EncodeFamily family = EncodeFamilyOf(params, hostDepth);
+    if (light != nullptr && (family == EncodeFamily::RgbF32Interleaved || family == EncodeFamily::RgbF32Flat) && !FlatCompactFits(*params.curveTable))
+    {
+        family = EncodeFamily::Generic; // the light-level flat kernels have the compact table only, which every PQ table built so far has
+    }
     const Interior inner = EncodeBlockInterior(family, params, hostDepth);
     if (inner.width == 0)
     {
-        return LaunchEncodeGeneric(params, hostDepth, stream);
+        return LaunchEncodeGeneric(params, hostDepth, stream, light);
     }
     cudaError_t e;
     switch (family)
     {
-    case EncodeFamily::RgbF32Interleaved: e = LaunchEncodeRgbF32Interleaved(params, inner, stream); break;
+    case EncodeFamily::RgbF32Interleaved: e = LaunchEncodeRgbF32Interleaved(params, inner, stream, light); break;
     case EncodeFamily::Gray16Lut: e = LaunchEncodeGray16Lut(params, inner, stream); break;
     case EncodeFamily::GrayInt: e = LaunchEncodeGrayInt(params, hostDepth, inner, stream); break;
     case EncodeFamily::RgbInt: e = LaunchEncodeRgbInt(params, hostDepth, inner, stream); break;
-    case EncodeFamily::GrayF32: e = LaunchEncodeGrayF32(params, inner, stream); break;
-    default: e = LaunchEncodeRgbF32Planar(family, params, inner, stream); break; // RgbF32Flat, RgbaF32Flat, RgbF32Clip
+    case EncodeFamily::GrayF32: e = LaunchEncodeGrayF32(params, inner, stream, light); break;
+    default: e = LaunchEncodeRgbF32Planar(family, params, inner, stream, light); break; // RgbF32Flat, RgbaF32Flat, RgbF32Clip
     }
-    return CompleteEncode(e, params, hostDepth, inner.width, inner.rows, stream);
+    return CompleteEncode(e, params, hostDepth, inner.width, inner.rows, stream, light);
 }
 
 int LaunchDecode(const DecodeParams& params, void* stream)
@@ -161,6 +165,7 @@ struct avifgpu_context
         uint16_t* device = nullptr;
     };
     std::vector<Gray16Lut> gray16Luts;
+    uint32_t* lightLevels[3] = {}; // level(k) of every code (light_level.cuh) at image depth 8 / 10 / 12, made with the depth's first PQ step table
     int premultiplyState[3] = { -1, -1, -1 }; // image depth 8 / 10 / 12: -1 not checked yet, 0 keep the reference sequence, 1 fast form verified
     // The first-use helpers below take `capturing`: the call is being recorded into a CUDA graph, where nothing but kernel
     // launches on the caller's stream may happen.  What is not prepared yet then answers "not verified" / nullptr for
@@ -374,7 +379,44 @@ struct avifgpu_context
         BuildCurveTable(curve, param, d.image_bit_depth, slots[0].stream, t);
         launches += t->stats.sweptInputs ? (t->stats.bandBitmapBytes ? 3 : 2) : 0; // sweep, (band bitmap,) verify
         curveTables.push_back(t);
+        if (curve == kCurveLinearToPQ)
+        {
+            BuildLightLevels(d.image_bit_depth); // the light-level call's tuned kernels run wherever a PQ step table is
+        }
         return t;
+    }
+
+    // The level table of an image depth (host arithmetic, one copy), once; a failure leaves it absent, and the light-level
+    // call then takes the generic kernel.
+    void BuildLightLevels(int depth)
+    {
+        uint32_t*& levels = lightLevels[depth == 8 ? 0 : depth == 10 ? 1 : 2];
+        if (levels != nullptr)
+        {
+            return;
+        }
+        std::vector<uint32_t> host(static_cast<size_t>(1) << depth);
+        const avifmath::LibmTables tables = avifmath::HostLibmTables();
+        const float maxCodeFloat = static_cast<float>(host.size() - 1);
+        for (size_t k = 0; k < host.size(); ++k)
+        {
+            host[k] = LightLevelOf(static_cast<uint32_t>(k), maxCodeFloat, tables);
+        }
+        uint32_t* device = nullptr;
+        const size_t bytes = host.size() * sizeof(uint32_t);
+        if (cudaMalloc(&device, bytes) != cudaSuccess)
+        {
+            cudaGetLastError();
+            return;
+        }
+        if (cudaMemcpyAsync(device, host.data(), bytes, cudaMemcpyHostToDevice, slots[0].stream) != cudaSuccess ||
+            cudaStreamSynchronize(slots[0].stream) != cudaSuccess)
+        {
+            cudaGetLastError();
+            cudaFree(device);
+            return;
+        }
+        levels = device;
     }
 
     // The first-use state an encode call reads: step table, Gray16 LUT, premultiply check.
@@ -662,6 +704,10 @@ AVIFGPU_EXPORT void avifgpu_destroy(avifgpu_context* ctx)
     {
         cudaFree(l.device);
     }
+    for (uint32_t* levels : ctx->lightLevels)
+    {
+        if (levels) cudaFree(levels);
+    }
     delete ctx;
 }
 
@@ -797,22 +843,11 @@ AVIFGPU_EXPORT int avifgpu_build_yuv_tables(const avifgpu_nclx* nclx, int32_t bi
 
 // ---- device-pointer entry points -------------------------------------------------------------------------------
 
-AVIFGPU_EXPORT int avifgpu_encode_rows_device(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const void* device_rows,
-                                              int64_t row_stride_bytes, int32_t y0, int32_t nrows,
-                                              const avifgpu_planes* device_dst, void* cuda_stream)
+// The device-pointer encode; `acc` != nullptr: the light-level call, whose description the caller has checked.
+static int EncodeRowsDevice(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const void* device_rows, int64_t row_stride_bytes, int32_t y0,
+                            int32_t nrows, const avifgpu_planes* device_dst, avifgpu_light_level* acc, void* cuda_stream)
 {
-    if (ctx == nullptr)
-    {
-        return AVIFGPU_ERR_BAD_PARAM;
-    }
-    avifgpu_encode_desc full;
-    desc = WidenEncodeDesc(desc, &full);
-    std::string error;
-    int status = ValidateEncodeDesc(desc, &error);
-    if (status != AVIFGPU_OK)
-    {
-        return ctx->Fail(status, error);
-    }
+    int status;
     if (device_dst == nullptr || (device_rows == nullptr && nrows > 0 && desc->width > 0))
     {
         return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL buffer");
@@ -853,12 +888,91 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_device(avifgpu_context* ctx, const avifgp
     }
     p.smCount = ctx->smCount;
     ctx->FirstUseEncode(*desc, static_cast<int64_t>(desc->width) * nrows, capturing, &p);
-    const int launched = LaunchEncode(p, desc->host_depth, cuda_stream);
+    const LightSink light = { acc, ctx->lightLevels[desc->image_bit_depth == 8 ? 0 : desc->image_bit_depth == 10 ? 1 : 2] };
+    if (acc != nullptr && light.levels == nullptr)
+    {
+        p.curveTable = nullptr; // no level table (not built yet, or its allocation failed): the generic kernel evaluates the levels
+    }
+    const int launched = LaunchEncode(p, desc->host_depth, cuda_stream, acc != nullptr ? &light : nullptr);
     if (launched < 0)
     {
         return ctx->LaunchFailed(launched, "encode kernel launch", capturing);
     }
     ctx->launches += launched;
+    return AVIFGPU_OK;
+}
+
+AVIFGPU_EXPORT int avifgpu_encode_rows_device(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const void* device_rows,
+                                              int64_t row_stride_bytes, int32_t y0, int32_t nrows,
+                                              const avifgpu_planes* device_dst, void* cuda_stream)
+{
+    if (ctx == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
+    std::string error;
+    const int status = ValidateEncodeDesc(desc, &error);
+    if (status != AVIFGPU_OK)
+    {
+        return ctx->Fail(status, error);
+    }
+    return EncodeRowsDevice(ctx, desc, device_rows, row_stride_bytes, y0, nrows, device_dst, nullptr, cuda_stream);
+}
+
+AVIFGPU_EXPORT int avifgpu_encode_rows_device_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const void* device_rows,
+                                                          int64_t row_stride_bytes, int32_t y0, int32_t nrows,
+                                                          const avifgpu_planes* device_dst, avifgpu_light_level* device_acc,
+                                                          void* cuda_stream)
+{
+    if (ctx == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    avifgpu_encode_desc full;
+    desc = WidenEncodeDesc(desc, &full);
+    std::string error;
+    const int status = ValidateEncodeDesc(desc, &error);
+    if (status != AVIFGPU_OK)
+    {
+        return ctx->Fail(status, error);
+    }
+    if (desc->host_depth != 32 || desc->transfer != AVIFGPU_TRANSFER_PQ)
+    {
+        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "the content light level is measured on float-host PQ encodes only");
+    }
+    if (device_acc == nullptr)
+    {
+        return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL light-level accumulator");
+    }
+    return EncodeRowsDevice(ctx, desc, device_rows, row_stride_bytes, y0, nrows, device_dst, device_acc, cuda_stream);
+}
+
+AVIFGPU_EXPORT int avifgpu_content_light_level(const avifgpu_light_level* acc, int32_t image_bit_depth, uint16_t* out_max_cll,
+                                               uint16_t* out_max_fall)
+{
+    if (acc == nullptr || out_max_cll == nullptr || out_max_fall == nullptr ||
+        (image_bit_depth != 8 && image_bit_depth != 10 && image_bit_depth != 12))
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    const uint32_t maxCode = (1u << image_bit_depth) - 1u;
+    using Wide = unsigned __int128;
+    const Wide unit = static_cast<Wide>(acc->pixels) << 22; // 2^22 x pixels: the level sum of that many pixels at 10000 cd/m2
+    if (acc->max_code > maxCode || static_cast<Wide>(acc->level_sum) > unit)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    if (acc->pixels == 0)
+    {
+        *out_max_cll = 0;
+        *out_max_fall = 0;
+        return AVIFGPU_OK;
+    }
+    const uint64_t peak = LightLevelOf(acc->max_code, static_cast<float>(maxCode), avifmath::HostLibmTables());
+    *out_max_cll = static_cast<uint16_t>((10000u * peak + (1u << 22) - 1u) >> 22);
+    *out_max_fall = static_cast<uint16_t>((static_cast<Wide>(acc->level_sum) * 10000u + unit - 1u) / unit);
     return AVIFGPU_OK;
 }
 

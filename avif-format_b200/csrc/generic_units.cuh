@@ -168,6 +168,14 @@ __device__ __forceinline__ void HostPixelToCodes(const EncodeParams& p, const Ho
     }
 }
 
+// A pixel's codes (HostPixelToCodes) into the light-level kernels' tally: the level from the context's table, or evaluated
+// here when the call runs before the table exists.
+__device__ __forceinline__ void TallyPixel(LightTally& tally, const uint32_t* levels, const EncodeParams& p, const uint32_t codes[4], const LibmTables& t)
+{
+    const uint32_t k = p.channels <= 2 ? codes[0] : max(max(codes[0], codes[1]), codes[2]);
+    TallyCode(tally, k, levels != nullptr ? __ldg(levels + k) : LightLevelOf(k, p.maxCodeFloat, t));
+}
+
 __device__ __forceinline__ void StoreCode(void* plane, int64_t stride, int y, int index, bool wide, uint32_t code)
 {
     uint8_t* row = static_cast<uint8_t*>(plane) + static_cast<int64_t>(y) * stride;
@@ -182,9 +190,11 @@ __device__ __forceinline__ void StoreCode(void* plane, int64_t stride, int y, in
 }
 
 // Planar YCbCr layout, one thread per chroma site (1x1, 2x1 or 2x2 pixels): the thread's site of CTA-sized chunk
-// `chunk` of the block, whose sites are numbered row by row in chunks of blockDim.x (== `threads`).
-template <typename HostT, int threads>
-__device__ __forceinline__ void EncodePlanarSite(const EncodeParams& p, const LibmTables& t, unsigned chunk)
+// `chunk` of the block, whose sites are numbered row by row in chunks of blockDim.x (== `threads`).  LIGHT = 1: each pixel
+// converted also goes into `*tally`, its level read from `levels` (or evaluated when that is null).
+template <typename HostT, int threads, int LIGHT = 0>
+__device__ __forceinline__ void EncodePlanarSite(const EncodeParams& p, const LibmTables& t, unsigned chunk, LightTally* tally = nullptr,
+                                                 const uint32_t* levels = nullptr)
 {
     const int chunks = (((p.width + p.xs) >> p.xs) + threads - 1) / threads;
     const int cx = static_cast<int>(chunk % chunks) * threads + threadIdx.x;
@@ -221,6 +231,10 @@ __device__ __forceinline__ void EncodePlanarSite(const EncodeParams& p, const Li
                               static_cast<int64_t>(x) * p.channels;
             uint32_t codes[4] = { 0, 0, 0, 0 };
             HostPixelToCodes<HostT>(p, px, codes, t);
+            if constexpr (LIGHT != 0)
+            {
+                TallyPixel(*tally, levels, p, codes, t);
+            }
             float yf;
             ForwardPixel(p.matrix, codes[0], codes[1], codes[2], yf, cb[dy][dx], cr[dy][dx]);
             have[dy][dx] = true;

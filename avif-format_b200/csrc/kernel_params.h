@@ -17,6 +17,7 @@
 
 #include "../../include/avifgpu.h"
 #include "curve_tables.h"
+#include "light_level.cuh"
 #include "pixel_math.cuh"
 
 // The routing and window arithmetic below is plain C++ that the plan kernel of the device-described batch
@@ -661,21 +662,24 @@ int ReportLaunchFailure(int cudaErrorCode);
 // LaunchEncode / LaunchDecode (avifgpu_api.cu) route a direct call (EncodeFamilyOf / DecodeFamilyOf, then the block half),
 // launch the family's kernel on the interior and complete the block.  They only enqueue work on `stream` and return the
 // number of kernels launched (>= 1; 0 for an empty block) or a negative avifgpu_status.
-int LaunchEncode(const EncodeParams& params, int hostDepth, void* stream);
+// `light` (the light-level call, light_level.cuh): the same route through the LIGHT instantiations, which add the block's
+// content light level into light->acc.
+int LaunchEncode(const EncodeParams& params, int hostDepth, void* stream, const LightSink* light = nullptr);
 int LaunchDecode(const DecodeParams& params, void* stream);
-int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* stream);
+int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* stream, const LightSink* light = nullptr);
 int LaunchDecodeGeneric(const DecodeParams& params, void* stream);
 int LaunchTransfer(int function, float param, const float* in, float* out, size_t count, void* stream);
 int LaunchHlgOotf(int inverse, const float luma[3], float displayGamma, float peak, const float* in, float* out, size_t pixels, void* stream);
 
 // The tuned launchers (kernels_fast*.cu): each fills its kernel's parameters for the interior `inner` of the block `p`
 // that the route gave its family, enqueues the kernel and returns the launch's status.
-cudaError_t LaunchEncodeRgbF32Interleaved(const EncodeParams& p, Interior inner, void* stream);
-cudaError_t LaunchEncodeRgbF32Planar(EncodeFamily family, const EncodeParams& p, Interior inner, void* stream); // RgbF32Flat, RgbaF32Flat, RgbF32Clip
+cudaError_t LaunchEncodeRgbF32Interleaved(const EncodeParams& p, Interior inner, void* stream, const LightSink* light = nullptr);
+cudaError_t LaunchEncodeRgbF32Planar(EncodeFamily family, const EncodeParams& p, Interior inner, void* stream,
+                                     const LightSink* light = nullptr); // RgbF32Flat, RgbaF32Flat, RgbF32Clip
 cudaError_t LaunchEncodeGray16Lut(const EncodeParams& p, Interior inner, void* stream);
 cudaError_t LaunchEncodeGrayInt(const EncodeParams& p, int hostDepth, Interior inner, void* stream);
 cudaError_t LaunchEncodeRgbInt(const EncodeParams& p, int hostDepth, Interior inner, void* stream);
-cudaError_t LaunchEncodeGrayF32(const EncodeParams& p, Interior inner, void* stream);
+cudaError_t LaunchEncodeGrayF32(const EncodeParams& p, Interior inner, void* stream, const LightSink* light = nullptr);
 cudaError_t LaunchDecodeYccF32(const DecodeParams& p, Interior inner, void* stream);
 cudaError_t LaunchDecodeYccInt(const DecodeParams& p, Interior inner, void* stream);
 cudaError_t LaunchDecodeStream(const DecodeParams& p, Interior inner, void* stream); // MonoInt, PlanarRgbInt
@@ -685,7 +689,8 @@ cudaError_t LaunchDecodeTable(const DecodeParams& p, Interior inner, void* strea
 // `tuned` is its launch status.  On success the generic kernel converts the right strip [coveredWidth, width) x
 // [0, rowCount), then the bottom strip [0, coveredWidth) x [coveredRows, rowCount); an empty strip launches nothing.
 // Returns 1 + the strip launches, or a negative status.
-int CompleteEncode(cudaError_t tuned, const EncodeParams& p, int hostDepth, int coveredWidth, int coveredRows, void* stream);
+int CompleteEncode(cudaError_t tuned, const EncodeParams& p, int hostDepth, int coveredWidth, int coveredRows, void* stream,
+                   const LightSink* light = nullptr);
 int CompleteDecode(cudaError_t tuned, const DecodeParams& p, int coveredWidth, int coveredRows, void* stream);
 
 // The launches of one planned chunk (PlanEncodeBatch / PlanDecodeBatch, batch_plan.h; kernels_batch.cu); `shared` is the

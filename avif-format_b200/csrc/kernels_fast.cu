@@ -141,7 +141,7 @@ cudaError_t LaunchClipKernel(const FastEncodeParams& fp, int smCount, cudaStream
 
 } // namespace
 
-cudaError_t LaunchEncodeRgbF32Interleaved(const EncodeParams& p, Interior inner, void* streamHandle)
+cudaError_t LaunchEncodeRgbF32Interleaved(const EncodeParams& p, Interior inner, void* streamHandle, const LightSink* light)
 {
     // The reference's own layout: interleaved RGB codes (WriteHeifImage.cpp:1098-1130), same kernel without the matrix.
     FastEncodeParams fp{};
@@ -156,10 +156,10 @@ cudaError_t LaunchEncodeRgbF32Interleaved(const EncodeParams& p, Interior inner,
     fp.maxCode = static_cast<int32_t>(p.maxCode);
     fp.table = *p.curveTable;
     const int curve = p.transfer == AVIFGPU_TRANSFER_PQ ? kCurveLinearToPQ : kCurveLinearToSMPTE428;
-    return LaunchFastEncodeFlatInterleaved(fp, curve, SmCountOrDefault(p.smCount), static_cast<cudaStream_t>(streamHandle));
+    return LaunchFastEncodeFlatInterleaved(fp, curve, SmCountOrDefault(p.smCount), static_cast<cudaStream_t>(streamHandle), light);
 }
 
-cudaError_t LaunchEncodeRgbF32Planar(EncodeFamily family, const EncodeParams& p, Interior inner, void* streamHandle)
+cudaError_t LaunchEncodeRgbF32Planar(EncodeFamily family, const EncodeParams& p, Interior inner, void* streamHandle, const LightSink* light)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
     const int curve = p.transfer == AVIFGPU_TRANSFER_PQ ? kCurveLinearToPQ : p.transfer == AVIFGPU_TRANSFER_SMPTE428 ? kCurveLinearToSMPTE428 : kCurveClip;
@@ -191,8 +191,8 @@ cudaError_t LaunchEncodeRgbF32Planar(EncodeFamily family, const EncodeParams& p,
         fp.planeA = static_cast<uint8_t*>(p.plane[3]);
         fp.strideA = p.planeStride[3];
         fp.premultiply = p.premultiply;
-        return LaunchFastEncodeRgba(fp, curve, p.xs, p.ys, p.destLayout, smCount, stream);
-    case EncodeFamily::RgbF32Flat: return LaunchFastEncodeFlat(fp, curve, p.xs, p.ys, p.destLayout, smCount, stream);
+        return LaunchFastEncodeRgba(fp, curve, p.xs, p.ys, p.destLayout, smCount, stream, light);
+    case EncodeFamily::RgbF32Flat: return LaunchFastEncodeFlat(fp, curve, p.xs, p.ys, p.destLayout, smCount, stream, light);
     default:
         return WithChroma(p.xs, p.ys, [&](auto xs, auto ys) {
             return WithLayout(p.destLayout, [&](auto dest) { return LaunchClipKernel<xs(), ys(), dest()>(fp, smCount, stream); });

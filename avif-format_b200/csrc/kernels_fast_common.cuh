@@ -234,11 +234,11 @@ __device__ __forceinline__ void StoreTile(const FastEncodeParams& p, const float
 } // namespace fastenc
 
 // kernels_fast_rgba.cu; `dest` is the description's avifgpu_source_layout bits (EncodeParams::destLayout)
-cudaError_t LaunchFastEncodeRgba(const fastenc::FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream);
+cudaError_t LaunchFastEncodeRgba(const fastenc::FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream, const LightSink* light);
 
 // kernels_fast_flat.cu
-cudaError_t LaunchFastEncodeFlat(const fastenc::FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream);
-cudaError_t LaunchFastEncodeFlatInterleaved(const fastenc::FastEncodeParams& fp, int curve, int smCount, cudaStream_t stream);
+cudaError_t LaunchFastEncodeFlat(const fastenc::FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream, const LightSink* light);
+cudaError_t LaunchFastEncodeFlatInterleaved(const fastenc::FastEncodeParams& fp, int curve, int smCount, cudaStream_t stream, const LightSink* light);
 
 } // namespace avifgpu
 

@@ -74,8 +74,9 @@ constexpr int kTableCompact14 = 3;
 // DEST: the avifgpu_source_layout bits of the YCbCr planes written (StoreTile); with interleaved chroma the lane's chroma
 // pointer walks plane 1 in steps of twice the bytes.  The body of EncodeRgbF32FlatKernel (DEST 0) and of
 // EncodeDestRgbF32FlatKernel (the other layouts).
-template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED, int DEST>
-__device__ __forceinline__ void EncodeRgbF32FlatBody(const FastEncodeParams& p, const FlatSchedule& schedule)
+// LIGHT = 1: also the content light level of the tile's codes (light_level.cuh), the body of EncodeLightRgbF32FlatKernel.
+template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED, int DEST, int LIGHT = 0>
+__device__ __forceinline__ void EncodeRgbF32FlatBody(const FastEncodeParams& p, const FlatSchedule& schedule, const LightSink& light = {})
 {
     constexpr bool kCompact = TABLE != kTableTwoLevel;
     constexpr int kCompactShift = TABLE == kTableCompact14 ? 14 : 0;
@@ -176,6 +177,7 @@ __device__ __forceinline__ void EncodeRgbF32FlatBody(const FastEncodeParams& p, 
     const uint32_t compactCodeMask = p.table.compactCodeMask;
     const uint32_t compactMagic = p.table.compactMagic;
     uint32_t parity = 0;
+    LightTally tally{ 0u, 0ull };
 
 #pragma unroll 1
     for (int item = firstItem; item < schedule.items; item += warpCount)
@@ -314,6 +316,19 @@ __device__ __forceinline__ void EncodeRgbF32FlatBody(const FastEncodeParams& p, 
             }
         }
 
+        if (LIGHT && laneActive)
+        {
+#pragma unroll
+            for (int pixel = 0; pixel < 8; ++pixel)
+            {
+                if (pixel < 4 || secondRow)
+                {
+                    const uint32_t k = __float2uint_rz(fmaxf(fmaxf(codeF[3 * pixel], codeF[3 * pixel + 1]), codeF[3 * pixel + 2]));
+                    TallyCode(tally, k, __ldg(light.levels + k));
+                }
+            }
+        }
+
         if (laneActive)
         {
             if (INTERLEAVED)
@@ -345,6 +360,10 @@ __device__ __forceinline__ void EncodeRgbF32FlatBody(const FastEncodeParams& p, 
         crPointer += kChromaRowsPerTile * p.strideCr;
     }
     }
+    if (LIGHT)
+    {
+        FlushLightTally(tally, LaunchPixelsForFirstWarp(static_cast<uint64_t>(p.width) * p.rowCount), light.acc);
+    }
 }
 
 template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED>
@@ -360,10 +379,21 @@ __global__ void __launch_bounds__(kFlatThreads, 1) EncodeDestRgbF32FlatKernel(co
     EncodeRgbF32FlatBody<CURVE, XS, YS, TABLE, 0, DEST>(p, schedule);
 }
 
+// The same with the content light level (every layout; PQ only).
 template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED, int DEST>
+__global__ void __launch_bounds__(kFlatThreads, 1) EncodeLightRgbF32FlatKernel(const FastEncodeParams p, const FlatSchedule schedule, const LightSink light)
+{
+    EncodeRgbF32FlatBody<CURVE, XS, YS, TABLE, INTERLEAVED, DEST, 1>(p, schedule, light);
+}
+
+template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED, int DEST, int LIGHT>
 constexpr auto FlatKernelFor()
 {
-    if constexpr (DEST == AVIFGPU_SOURCE_PLANAR)
+    if constexpr (LIGHT)
+    {
+        return EncodeLightRgbF32FlatKernel<CURVE, XS, YS, TABLE, INTERLEAVED, DEST>;
+    }
+    else if constexpr (DEST == AVIFGPU_SOURCE_PLANAR)
     {
         return EncodeRgbF32FlatKernel<CURVE, XS, YS, TABLE, INTERLEAVED>;
     }
@@ -373,13 +403,13 @@ constexpr auto FlatKernelFor()
     }
 }
 
-template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED = 0, int DEST = AVIFGPU_SOURCE_PLANAR>
-cudaError_t LaunchFlatKernel(const FastEncodeParams& fp, int smCount, cudaStream_t stream)
+template <int CURVE, int XS, int YS, int TABLE, int INTERLEAVED = 0, int DEST = AVIFGPU_SOURCE_PLANAR, int LIGHT = 0>
+cudaError_t LaunchFlatKernel(const FastEncodeParams& fp, int smCount, cudaStream_t stream, const LightSink* light = nullptr)
 {
     const size_t shared = static_cast<size_t>(FlatFixedBytes()) + FlatTableBytes(fp.table, TABLE == kTableTwoLevel);
     static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
     {
-        const cudaError_t e = AllowDynamicShared(FlatKernelFor<CURVE, XS, YS, TABLE, INTERLEAVED, DEST>(), kSharedLimit, configuredDevices);
+        const cudaError_t e = AllowDynamicShared(FlatKernelFor<CURVE, XS, YS, TABLE, INTERLEAVED, DEST, LIGHT>(), kSharedLimit, configuredDevices);
         if (e != cudaSuccess)
         {
             return e;
@@ -407,23 +437,39 @@ cudaError_t LaunchFlatKernel(const FastEncodeParams& fp, int smCount, cudaStream
     schedule.longSegments = schedule.tileRows % schedule.segments;
     schedule.lastColumnBytes = (fp.width - (schedule.tilesX - 1) * kTilePixels) * 12;
     schedule.unpairedTileRow = (fp.rowCount & 1) ? fp.rowCount / 2 : -1;
-    FlatKernelFor<CURVE, XS, YS, TABLE, INTERLEAVED, DEST>()<<<static_cast<unsigned>(blocks), kFlatThreads, shared, stream>>>(fp, schedule);
+    if constexpr (LIGHT)
+    {
+        FlatKernelFor<CURVE, XS, YS, TABLE, INTERLEAVED, DEST, LIGHT>()<<<static_cast<unsigned>(blocks), kFlatThreads, shared, stream>>>(fp, schedule, *light);
+    }
+    else
+    {
+        FlatKernelFor<CURVE, XS, YS, TABLE, INTERLEAVED, DEST, LIGHT>()<<<static_cast<unsigned>(blocks), kFlatThreads, shared, stream>>>(fp, schedule);
+    }
     return cudaGetLastError();
 }
 
 } // namespace
 
 // The reference's interleaved RGB layout through the same kernel (fp.planeY / strideY = the interleaved buffer).
-cudaError_t LaunchFastEncodeFlatInterleaved(const FastEncodeParams& fp, int curve, int smCount, cudaStream_t stream)
+cudaError_t LaunchFastEncodeFlatInterleaved(const FastEncodeParams& fp, int curve, int smCount, cudaStream_t stream, const LightSink* light)
 {
     if (FlatCompactFits(fp.table))
     {
+        if (curve == kCurveLinearToPQ && light != nullptr)
+        {
+            return fp.table.flatShift == 14 ? LaunchFlatKernel<kCurveLinearToPQ, 0, 0, kTableCompact14, 1, AVIFGPU_SOURCE_PLANAR, 1>(fp, smCount, stream, light)
+                                            : LaunchFlatKernel<kCurveLinearToPQ, 0, 0, kTableCompact, 1, AVIFGPU_SOURCE_PLANAR, 1>(fp, smCount, stream, light);
+        }
         if (curve == kCurveLinearToPQ)
         {
             return fp.table.flatShift == 14 ? LaunchFlatKernel<kCurveLinearToPQ, 0, 0, kTableCompact14, 1>(fp, smCount, stream)
                                             : LaunchFlatKernel<kCurveLinearToPQ, 0, 0, kTableCompact, 1>(fp, smCount, stream);
         }
         return LaunchFlatKernel<kCurveLinearToSMPTE428, 0, 0, kTableCompact, 1>(fp, smCount, stream);
+    }
+    if (light != nullptr)
+    {
+        return cudaErrorInvalidValue; // LaunchEncode sends a light-level call without the compact table to the generic kernel
     }
     if (curve == kCurveLinearToPQ) return LaunchFlatKernel<kCurveLinearToPQ, 0, 0, kTableTwoLevel, 1>(fp, smCount, stream);
     return LaunchFlatKernel<kCurveLinearToSMPTE428, 0, 0, kTableTwoLevel, 1>(fp, smCount, stream);
@@ -434,11 +480,21 @@ cudaError_t LaunchFastEncodeFlatInterleaved(const FastEncodeParams& fp, int curv
 // pairs the tables built for 10/12-bit encodes reach (DESIGN.md 4.2): PQ with the compact table (kTableCompact14 for
 // flatShift 14, as at 12 bits, kTableCompact for any other shift), SMPTE 428 with the compact table (10 bits) or the
 // two-level one (12 bits, the only form built there).  A PQ table without its compact form has not been built for any
-// configuration so far; EncodeFamilyOf leaves such a description with another layout to the generic kernel.
-cudaError_t LaunchFastEncodeFlat(const FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream)
+// configuration so far; EncodeFamilyOf leaves such a description with another layout to the generic kernel, and LaunchEncode
+// a light-level call (`light` set: the LIGHT = 1 instantiations, PQ with the compact table only) in any layout.
+cudaError_t LaunchFastEncodeFlat(const FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream, const LightSink* light)
 {
     return WithChroma(xs, ys, [&](auto XS, auto YS) {
         return WithLayout(dest, [&](auto DEST) {
+            if (light != nullptr)
+            {
+                if (curve != kCurveLinearToPQ || !FlatCompactFits(fp.table))
+                {
+                    return cudaErrorInvalidValue; // LaunchEncode said no: the launcher does not get here
+                }
+                return fp.table.flatShift == 14 ? LaunchFlatKernel<kCurveLinearToPQ, XS(), YS(), kTableCompact14, 0, DEST(), 1>(fp, smCount, stream, light)
+                                                : LaunchFlatKernel<kCurveLinearToPQ, XS(), YS(), kTableCompact, 0, DEST(), 1>(fp, smCount, stream, light);
+            }
             if (FlatCompactFits(fp.table))
             {
                 if (curve == kCurveLinearToPQ)

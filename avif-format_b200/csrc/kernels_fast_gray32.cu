@@ -40,9 +40,10 @@ struct Gray32Params
     CurveTableView table;
 };
 
-// CHANNELS 1 (Gray) or 2 (Gray + alpha); PQ = 1: LinearToPQ through the compact table, 0: clip.
-template <int CHANNELS, int PQ>
-__global__ void __launch_bounds__(PQ ? kGrayTableThreads : kGrayClipThreads) EncodeGrayF32Kernel(const Gray32Params p)
+// CHANNELS 1 (Gray) or 2 (Gray + alpha); PQ = 1: LinearToPQ through the compact table, 0: clip.  LIGHT = 1 (PQ only): also
+// the content light level of the Y codes (light_level.cuh).
+template <int CHANNELS, int PQ, int LIGHT>
+__device__ __forceinline__ void EncodeGrayF32Body(const Gray32Params& p, const LightSink& light = {})
 {
     extern __shared__ __align__(16) uint8_t sharedBytes[];
     uint64_t* libmStorage = reinterpret_cast<uint64_t*>(sharedBytes);
@@ -65,6 +66,7 @@ __global__ void __launch_bounds__(PQ ? kGrayTableThreads : kGrayClipThreads) Enc
     const int32_t span = static_cast<int32_t>(p.table.flatHigh - p.table.flatLow);
     const uint32_t topShift = 32u - shift;
 
+    LightTally tally{ 0u, 0ull };
     GroupWalk walk(static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x, static_cast<long long>(gridDim.x) * blockDim.x, p.groupsPerRow, p.rowCount);
     while (walk.Inside(p.rowCount))
     {
@@ -210,6 +212,14 @@ __global__ void __launch_bounds__(PQ ? kGrayTableThreads : kGrayClipThreads) Enc
             {
                 continue;
             }
+            if (LIGHT)
+            {
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                {
+                    TallyCode(tally, yCode[4 * u + i], __ldg(light.levels + yCode[4 * u + i]));
+                }
+            }
             __stcs(reinterpret_cast<uint2*>(p.planeY + planeOffsetY[u]),
                    make_uint2(yCode[4 * u] | (yCode[4 * u + 1] << 16), yCode[4 * u + 2] | (yCode[4 * u + 3] << 16)));
             if (CHANNELS == 2)
@@ -219,14 +229,44 @@ __global__ void __launch_bounds__(PQ ? kGrayTableThreads : kGrayClipThreads) Enc
             }
         }
     }
+    if (LIGHT)
+    {
+        FlushLightTally(tally, LaunchPixelsForFirstWarp(static_cast<uint64_t>(p.groupsPerRow) * 4 * p.rowCount), light.acc);
+    }
 }
 
 template <int CHANNELS, int PQ>
-cudaError_t LaunchGray32(const Gray32Params& gp, size_t shared, int smCount, cudaStream_t stream)
+__global__ void __launch_bounds__(PQ ? kGrayTableThreads : kGrayClipThreads) EncodeGrayF32Kernel(const Gray32Params p)
+{
+    EncodeGrayF32Body<CHANNELS, PQ, 0>(p);
+}
+
+// The same through the PQ table, with the content light level.
+template <int CHANNELS>
+__global__ void __launch_bounds__(kGrayTableThreads) EncodeLightGrayF32Kernel(const Gray32Params p, const LightSink light)
+{
+    EncodeGrayF32Body<CHANNELS, 1, 1>(p, light);
+}
+
+template <int CHANNELS, int PQ, int LIGHT>
+constexpr auto GrayKernelFor()
+{
+    if constexpr (LIGHT)
+    {
+        return EncodeLightGrayF32Kernel<CHANNELS>;
+    }
+    else
+    {
+        return EncodeGrayF32Kernel<CHANNELS, PQ>;
+    }
+}
+
+template <int CHANNELS, int PQ, int LIGHT = 0>
+cudaError_t LaunchGray32(const Gray32Params& gp, size_t shared, int smCount, cudaStream_t stream, const LightSink* light = nullptr)
 {
     static std::atomic<uint64_t> configuredDevices{ 0 };
     {
-        const cudaError_t e = AllowDynamicShared(EncodeGrayF32Kernel<CHANNELS, PQ>, kGrayF32SharedLimit, configuredDevices);
+        const cudaError_t e = AllowDynamicShared(GrayKernelFor<CHANNELS, PQ, LIGHT>(), kGrayF32SharedLimit, configuredDevices);
         if (e != cudaSuccess)
         {
             return e;
@@ -235,13 +275,20 @@ cudaError_t LaunchGray32(const Gray32Params& gp, size_t shared, int smCount, cud
     constexpr int kThreads = PQ ? kGrayTableThreads : kGrayClipThreads;
     const long long groups = static_cast<long long>(gp.groupsPerRow) * gp.rowCount;
     const long long cap = PQ ? static_cast<long long>(smCount) : static_cast<long long>(smCount) * 8; // a table per CTA: one long-lived CTA per SM
-    EncodeGrayF32Kernel<CHANNELS, PQ><<<GridFor((groups + kThreads - 1) / kThreads, cap), kThreads, shared, stream>>>(gp);
+    if constexpr (LIGHT)
+    {
+        GrayKernelFor<CHANNELS, PQ, LIGHT>()<<<GridFor((groups + kThreads - 1) / kThreads, cap), kThreads, shared, stream>>>(gp, *light);
+    }
+    else
+    {
+        GrayKernelFor<CHANNELS, PQ, LIGHT>()<<<GridFor((groups + kThreads - 1) / kThreads, cap), kThreads, shared, stream>>>(gp);
+    }
     return cudaGetLastError();
 }
 
 } // namespace
 
-cudaError_t LaunchEncodeGrayF32(const EncodeParams& p, Interior inner, void* streamHandle)
+cudaError_t LaunchEncodeGrayF32(const EncodeParams& p, Interior inner, void* streamHandle, const LightSink* light)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
     const bool pq = p.transfer == AVIFGPU_TRANSFER_PQ;
@@ -265,6 +312,11 @@ cudaError_t LaunchEncodeGrayF32(const EncodeParams& p, Interior inner, void* str
         shared += gp.table.compactImageBytes;
     }
     const int smCount = SmCountOrDefault(p.smCount);
+    if (light != nullptr)
+    {
+        if (!pq) return cudaErrorInvalidValue; // the light-level call takes PQ descriptions only
+        return p.channels == 2 ? LaunchGray32<2, 1, 1>(gp, shared, smCount, stream, light) : LaunchGray32<1, 1, 1>(gp, shared, smCount, stream, light);
+    }
     if (p.channels == 2) return pq ? LaunchGray32<2, 1>(gp, shared, smCount, stream) : LaunchGray32<2, 0>(gp, shared, smCount, stream);
     return pq ? LaunchGray32<1, 1>(gp, shared, smCount, stream) : LaunchGray32<1, 0>(gp, shared, smCount, stream);
 }

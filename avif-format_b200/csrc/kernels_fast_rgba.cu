@@ -26,9 +26,10 @@ constexpr int kRgbaThreads = kRgbaWarps * 32;
 
 // The compact table + first_k array in shared memory (kernels_fast_flat.cu has the commentary).  DEST: the
 // avifgpu_source_layout bits of the planes written (StoreTile; the alpha plane is shifted like the others).  The body of
-// EncodeRgbaF32FlatKernel (DEST 0) and of EncodeDestRgbaF32FlatKernel (the other layouts).
-template <int CURVE, int XS, int YS, int DEST>
-__device__ __forceinline__ void EncodeRgbaF32FlatBody(const FastEncodeParams& p)
+// EncodeRgbaF32FlatKernel (DEST 0) and of EncodeDestRgbaF32FlatKernel (the other layouts).  LIGHT = 1: also the content
+// light level of the colour codes (light_level.cuh), the body of EncodeLightRgbaF32FlatKernel.
+template <int CURVE, int XS, int YS, int DEST, int LIGHT = 0>
+__device__ __forceinline__ void EncodeRgbaF32FlatBody(const FastEncodeParams& p, const LightSink& light = {})
 {
     extern __shared__ __align__(16) uint8_t sharedBytes[];
     uint64_t* libmStorage = reinterpret_cast<uint64_t*>(sharedBytes);
@@ -65,6 +66,7 @@ __device__ __forceinline__ void EncodeRgbaF32FlatBody(const FastEncodeParams& p)
     const int stepX = warpCount - stepRows * tilesX;
     int tileRow = firstTile / tilesX;
     int tileX = firstTile - tileRow * tilesX;
+    LightTally tally{ 0u, 0ull };
 
     uint4 raw[8]; // pixel i of row r = raw[4 * r + i] = { R, G, B, A }
     auto loadTile = [&](int row, int column, bool valid)
@@ -195,6 +197,19 @@ __device__ __forceinline__ void EncodeRgbaF32FlatBody(const FastEncodeParams& p)
             }
         }
 
+        if (LIGHT && laneActive)
+        {
+#pragma unroll
+            for (int pixel = 0; pixel < 8; ++pixel)
+            {
+                if (pixel < 4 || secondRow)
+                {
+                    const uint32_t k = __float2uint_rz(fmaxf(fmaxf(codeF[3 * pixel], codeF[3 * pixel + 1]), codeF[3 * pixel + 2]));
+                    TallyCode(tally, k, __ldg(light.levels + k));
+                }
+            }
+        }
+
         if (laneActive)
         {
             const int64_t chromaRow = YS ? tileRow : y0;
@@ -213,6 +228,10 @@ __device__ __forceinline__ void EncodeRgbaF32FlatBody(const FastEncodeParams& p)
         tileRow = nextRow;
         tileX = nextX;
     }
+    if (LIGHT)
+    {
+        FlushLightTally(tally, LaunchPixelsForFirstWarp(static_cast<uint64_t>(p.width) * p.rowCount), light.acc);
+    }
 }
 
 template <int CURVE, int XS, int YS>
@@ -228,10 +247,21 @@ __global__ void __launch_bounds__(kRgbaThreads, 1) EncodeDestRgbaF32FlatKernel(c
     EncodeRgbaF32FlatBody<CURVE, XS, YS, DEST>(p);
 }
 
+// The same with the content light level (every layout; PQ only).
 template <int CURVE, int XS, int YS, int DEST>
+__global__ void __launch_bounds__(kRgbaThreads, 1) EncodeLightRgbaF32FlatKernel(const FastEncodeParams p, const LightSink light)
+{
+    EncodeRgbaF32FlatBody<CURVE, XS, YS, DEST, 1>(p, light);
+}
+
+template <int CURVE, int XS, int YS, int DEST, int LIGHT>
 constexpr auto RgbaKernelFor()
 {
-    if constexpr (DEST == AVIFGPU_SOURCE_PLANAR)
+    if constexpr (LIGHT)
+    {
+        return EncodeLightRgbaF32FlatKernel<CURVE, XS, YS, DEST>;
+    }
+    else if constexpr (DEST == AVIFGPU_SOURCE_PLANAR)
     {
         return EncodeRgbaF32FlatKernel<CURVE, XS, YS>;
     }
@@ -241,13 +271,13 @@ constexpr auto RgbaKernelFor()
     }
 }
 
-template <int CURVE, int XS, int YS, int DEST>
-cudaError_t LaunchRgbaKernel(const FastEncodeParams& fp, int smCount, cudaStream_t stream)
+template <int CURVE, int XS, int YS, int DEST, int LIGHT = 0>
+cudaError_t LaunchRgbaKernel(const FastEncodeParams& fp, int smCount, cudaStream_t stream, const LightSink* light = nullptr)
 {
     const size_t shared = static_cast<size_t>(RgbaFixedBytes()) + fp.table.compactImageBytes;
     static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
     {
-        const cudaError_t e = AllowDynamicShared(RgbaKernelFor<CURVE, XS, YS, DEST>(), kSharedLimit, configuredDevices);
+        const cudaError_t e = AllowDynamicShared(RgbaKernelFor<CURVE, XS, YS, DEST, LIGHT>(), kSharedLimit, configuredDevices);
         if (e != cudaSuccess)
         {
             return e;
@@ -263,16 +293,27 @@ cudaError_t LaunchRgbaKernel(const FastEncodeParams& fp, int smCount, cudaStream
     {
         blocks = smCount;
     }
-    RgbaKernelFor<CURVE, XS, YS, DEST>()<<<static_cast<unsigned>(blocks), kRgbaThreads, shared, stream>>>(fp);
+    if constexpr (LIGHT)
+    {
+        RgbaKernelFor<CURVE, XS, YS, DEST, LIGHT>()<<<static_cast<unsigned>(blocks), kRgbaThreads, shared, stream>>>(fp, *light);
+    }
+    else
+    {
+        RgbaKernelFor<CURVE, XS, YS, DEST, LIGHT>()<<<static_cast<unsigned>(blocks), kRgbaThreads, shared, stream>>>(fp);
+    }
     return cudaGetLastError();
 }
 
 } // namespace
 
-cudaError_t LaunchFastEncodeRgba(const FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream)
+cudaError_t LaunchFastEncodeRgba(const FastEncodeParams& fp, int curve, int xs, int ys, int dest, int smCount, cudaStream_t stream, const LightSink* light)
 {
     return WithChroma(xs, ys, [&](auto XS, auto YS) {
         return WithLayout(dest, [&](auto DEST) {
+            if (light != nullptr)
+            {
+                return curve == kCurveLinearToPQ ? LaunchRgbaKernel<kCurveLinearToPQ, XS(), YS(), DEST(), 1>(fp, smCount, stream, light) : cudaErrorInvalidValue;
+            }
             return curve == kCurveLinearToPQ ? LaunchRgbaKernel<kCurveLinearToPQ, XS(), YS(), DEST()>(fp, smCount, stream)
                                              : LaunchRgbaKernel<kCurveLinearToSMPTE428, XS(), YS(), DEST()>(fp, smCount, stream);
         });

@@ -70,6 +70,55 @@ __global__ void __launch_bounds__(kThreads) EncodePlanarKernel(const EncodeParam
 
     EncodePlanarSite<HostT, kThreads>(p, t, blockIdx.x);
 }
+
+// The light-level kernels (float hosts, PQ; light_level.cuh): the kernels above, every pixel's codes into the thread's tally,
+// one flush per warp.  No thread leaves early: the flush needs the whole warp.
+__global__ void __launch_bounds__(kThreads) EncodeReferenceLayoutLightKernel(const EncodeParams p, const LightSink light)
+{
+    __shared__ uint64_t libmStorage[96];
+    const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
+    __syncthreads();
+
+    LightTally tally{ 0u, 0ull };
+    const int chunks = (p.width + kThreads - 1) / kThreads;
+    const int x = static_cast<int>(blockIdx.x % chunks) * kThreads + threadIdx.x;
+    const int y = static_cast<int>(blockIdx.x / chunks);
+    if (x < p.width && y < p.rowCount)
+    {
+        const float* px = reinterpret_cast<const float*>(static_cast<const uint8_t*>(p.rows) + static_cast<int64_t>(y) * p.rowStride) +
+                          static_cast<int64_t>(x) * p.channels;
+        uint32_t codes[4] = { 0, 0, 0, 0 };
+        HostPixelToCodes<float>(p, px, codes, t);
+        TallyPixel(tally, light.levels, p, codes, t);
+        if (p.channels <= 2)
+        {
+            StoreCode(p.plane[0], p.planeStride[0], y, x, true, codes[0]);
+            if (p.hasAlpha)
+            {
+                StoreCode(p.plane[3], p.planeStride[3], y, x, true, codes[1]);
+            }
+        }
+        else
+        {
+            for (int i = 0; i < p.channels; ++i)
+            {
+                StoreCode(p.plane[0], p.planeStride[0], y, x * p.channels + i, true, codes[i]);
+            }
+        }
+    }
+    FlushLightTally(tally, LaunchPixelsForFirstWarp(static_cast<uint64_t>(p.width) * p.rowCount), light.acc);
+}
+
+__global__ void __launch_bounds__(kThreads) EncodePlanarLightKernel(const EncodeParams p, const LightSink light)
+{
+    __shared__ uint64_t libmStorage[96];
+    const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
+    __syncthreads();
+
+    LightTally tally{ 0u, 0ull };
+    EncodePlanarSite<float, kThreads, 1>(p, t, blockIdx.x, &tally, light.levels);
+    FlushLightTally(tally, LaunchPixelsForFirstWarp(static_cast<uint64_t>(p.width) * p.rowCount), light.acc);
+}
 // ---- decode ----------------------------------------------------------------------------------------------
 
 // PlaneT uint8_t pairs with HostT uint8_t; PlaneT uint16_t with HostT uint16_t or float.
@@ -116,7 +165,7 @@ __global__ void __launch_bounds__(kThreads) TransferKernel(int function, float p
 
 } // namespace
 
-int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* streamHandle)
+int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* streamHandle, const LightSink* light)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
     if (params.width <= 0 || params.rowCount <= 0)
@@ -136,12 +185,26 @@ int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* streamH
         const int sitesX = (p.width + p.xs) >> p.xs;
         const int sitesY = (p.rowCount + p.ys) >> p.ys;
         const unsigned grid = static_cast<unsigned>((sitesX + kThreads - 1) / kThreads) * static_cast<unsigned>(sitesY);
-        WithHostDepth(hostDepth, [&](auto, auto host) { EncodePlanarKernel<TypeOf<decltype(host)>><<<grid, kThreads, 0, stream>>>(p); });
+        if (light != nullptr)
+        {
+            EncodePlanarLightKernel<<<grid, kThreads, 0, stream>>>(p, *light); // float hosts only (avifgpu_encode_rows_device_light_level)
+        }
+        else
+        {
+            WithHostDepth(hostDepth, [&](auto, auto host) { EncodePlanarKernel<TypeOf<decltype(host)>><<<grid, kThreads, 0, stream>>>(p); });
+        }
     }
     else
     {
         const unsigned grid = static_cast<unsigned>((p.width + kThreads - 1) / kThreads) * static_cast<unsigned>(p.rowCount);
-        WithHostDepth(hostDepth, [&](auto, auto host) { EncodeReferenceLayoutKernel<TypeOf<decltype(host)>><<<grid, kThreads, 0, stream>>>(p); });
+        if (light != nullptr)
+        {
+            EncodeReferenceLayoutLightKernel<<<grid, kThreads, 0, stream>>>(p, *light);
+        }
+        else
+        {
+            WithHostDepth(hostDepth, [&](auto, auto host) { EncodeReferenceLayoutKernel<TypeOf<decltype(host)>><<<grid, kThreads, 0, stream>>>(p); });
+        }
     }
     const cudaError_t launchError = cudaGetLastError();
     return launchError == cudaSuccess ? 1 : ReportLaunchFailure(static_cast<int>(launchError));
@@ -161,18 +224,18 @@ int LaunchDecodeGeneric(const DecodeParams& p, void* streamHandle)
 }
 
 // The generic launchers return 0 for an empty strip.
-int CompleteEncode(cudaError_t tuned, const EncodeParams& p, int hostDepth, int coveredWidth, int coveredRows, void* stream)
+int CompleteEncode(cudaError_t tuned, const EncodeParams& p, int hostDepth, int coveredWidth, int coveredRows, void* stream, const LightSink* light)
 {
     if (tuned != cudaSuccess)
     {
         return ReportLaunchFailure(static_cast<int>(tuned));
     }
-    const int right = LaunchEncodeGeneric(EncodeWindow(p, hostDepth, coveredWidth, 0, p.width - coveredWidth, p.rowCount), hostDepth, stream);
+    const int right = LaunchEncodeGeneric(EncodeWindow(p, hostDepth, coveredWidth, 0, p.width - coveredWidth, p.rowCount), hostDepth, stream, light);
     if (right < 0)
     {
         return right;
     }
-    const int bottom = LaunchEncodeGeneric(EncodeWindow(p, hostDepth, 0, coveredRows, coveredWidth, p.rowCount - coveredRows), hostDepth, stream);
+    const int bottom = LaunchEncodeGeneric(EncodeWindow(p, hostDepth, 0, coveredRows, coveredWidth, p.rowCount - coveredRows), hostDepth, stream, light);
     return bottom < 0 ? bottom : 1 + right + bottom;
 }
 

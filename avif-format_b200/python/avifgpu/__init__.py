@@ -68,6 +68,10 @@ def library():
         [ctx_p, C.POINTER(abi.EncodeDesc), C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(abi.Planes), C.c_void_p])
     sig("avifgpu_decode_rows_device", C.c_int,
         [ctx_p, C.POINTER(abi.DecodeDesc), C.POINTER(abi.Planes), C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p])
+    sig("avifgpu_encode_rows_device_light_level", C.c_int,
+        [ctx_p, C.POINTER(abi.EncodeDesc), C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(abi.Planes), C.c_void_p, C.c_void_p])
+    sig("avifgpu_content_light_level", C.c_int,
+        [C.POINTER(abi.LightLevel), C.c_int32, C.POINTER(C.c_uint16), C.POINTER(C.c_uint16)])
     sig("avifgpu_encode_batch_device", C.c_int,
         [ctx_p, C.POINTER(abi.EncodeDesc), C.POINTER(abi.BatchImage), C.c_int32, C.c_void_p])
     sig("avifgpu_decode_batch_device", C.c_int,
@@ -141,7 +145,22 @@ EXPORTED_SYMBOLS = [
     "avifgpu_shard_group_peer_access", "avifgpu_shard_group_last_error", "avifgpu_shard_group_prepare_encode",
     "avifgpu_shard_group_synchronize", "avifgpu_shard_row_blocks", "avifgpu_encode_rows_sharded", "avifgpu_decode_rows_sharded",
     "avifgpu_encode_rows_sharded_device", "avifgpu_icc_to_rec2020_linear_matrix",
+    "avifgpu_encode_rows_device_light_level", "avifgpu_content_light_level",
 ]
+
+
+def content_light_level(acc, image_bit_depth):
+    """(MaxCLL, MaxFALL) in cd/m2 of an accumulator (abi.LightLevel, a dict with its fields, or the 24 bytes of the device
+    accumulator as any buffer) -- avifgpu_content_light_level, pure host arithmetic."""
+    if isinstance(acc, dict):
+        acc = abi.LightLevel(max_code=acc["max_code"], reserved=acc.get("reserved", 0), level_sum=acc["level_sum"], pixels=acc["pixels"])
+    elif not isinstance(acc, abi.LightLevel):
+        acc = abi.LightLevel.from_buffer_copy(bytes(memoryview(acc).cast("B")))
+    max_cll, max_fall = C.c_uint16(0), C.c_uint16(0)
+    status = library().avifgpu_content_light_level(C.byref(acc), image_bit_depth, C.byref(max_cll), C.byref(max_fall))
+    if status != 0:
+        raise AvifGpuError(status, "avifgpu_content_light_level")
+    return int(max_cll.value), int(max_fall.value)
 
 
 # ---- host-arithmetic helpers (usable without a device) -------------------------------------------------------
@@ -306,6 +325,13 @@ class Context:
         nrows = desc.height - y0 if nrows is None else nrows
         self._check(self.lib.avifgpu_encode_rows_device(self.handle, C.byref(desc), rows_ptr, row_stride, y0, nrows,
                                                         C.byref(planes_struct), stream))
+
+    def encode_device_light_level(self, desc, rows_ptr, row_stride, planes_struct, acc_ptr, y0=0, nrows=None, stream=0):
+        """avifgpu_encode_rows_device_light_level: encode_device, plus the content light level of the rows added into the
+        device accumulator at `acc_ptr` (24 bytes, zeroed by the caller; see abi.LightLevel)."""
+        nrows = desc.height - y0 if nrows is None else nrows
+        self._check(self.lib.avifgpu_encode_rows_device_light_level(self.handle, C.byref(desc), rows_ptr, row_stride, y0, nrows,
+                                                                    C.byref(planes_struct), acc_ptr, stream))
 
     def encode_batch_device(self, desc, images, stream=0):
         """avifgpu_encode_batch_device: `images` is a ctypes array of abi.BatchImage (see batch_images_from_tensors)."""

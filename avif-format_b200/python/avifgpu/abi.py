@@ -8,7 +8,7 @@ import ctypes as C
 
 import numpy as np
 
-API_VERSION = 11
+API_VERSION = 12
 
 # avifgpu_status
 OK = 0
@@ -193,6 +193,19 @@ class CurveStats(C.Structure):
 
     def as_dict(self):
         return {name: getattr(self, name) for name, _ in self._fields_}
+
+
+class LightLevel(C.Structure):
+    """avifgpu_light_level: the device accumulator of avifgpu_encode_rows_device_light_level (24 bytes)."""
+    _fields_ = [
+        ("max_code", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("level_sum", C.c_uint64),
+        ("pixels", C.c_uint64),
+    ]
+
+    def as_dict(self):
+        return {name: int(getattr(self, name)) for name, _ in self._fields_}
 
 
 # ---- geometry (mirrors avifgpu_*_plane_geometry / *_host_col_bytes) ---------------------------------------

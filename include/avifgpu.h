@@ -50,7 +50,7 @@ extern "C" {
 #define AVIFGPU_EXPORT __attribute__((visibility("default")))
 #endif
 
-#define AVIFGPU_API_VERSION 11
+#define AVIFGPU_API_VERSION 12
 
 typedef enum avifgpu_status
 {
@@ -399,6 +399,59 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_device(avifgpu_context* ctx, const avifgp
                                               const avifgpu_planes* device_src, int32_t y0, int32_t nrows,
                                               void* device_rows, int64_t row_stride_bytes,
                                               void* cuda_stream);
+
+/* ---- content light level of PQ encodes (since API version 12) ---------------------------------------------------- */
+
+/*
+ * The static HDR metadata every PQ stream or still carries -- the HEVC / AV1 content light level SEI or metadata OBU, the
+ * AVIF / HEIF `clli` property -- holds two values (CTA-861.3): MaxCLL, the brightest pixel, and MaxFALL, the frame-average
+ * light level, where a pixel's light level is max(R, G, B) in cd/m2.  The light-level encode measures them on the codes it
+ * writes, in the same pass.
+ *
+ * Definition.  For every pixel the call converts, k = max(R', G', B') of the pixel's transfer-curve codes at
+ * image_bit_depth -- the codes the encode computes before the forward matrix, after the clamp, premultiplication and
+ * row_matrix; for Gray / Gray+A hosts k is the Y code; alpha never counts.  The level of code k is
+ *     level(k) = (uint32_t)(PQToLinear((float)k / (float)maxCode, 1.0f) * 2^22), truncated,
+ * PQToLinear being ColorTransfer.cpp:94-117 with multiplier 1 (the absolute PQ scale, 1.0 = 10000 cd/m2) in binary32 with
+ * glibc's powf; it does not depend on pq_peak_nits.  Working on codes makes the statistic exact and independent of the
+ * order in which pixels are visited: every route gives the same integers, and NaN, +-inf and negative inputs count with
+ * the code the encode gives them.
+ *
+ * The accumulator is device memory, zeroed by the caller, and collects every call made into it. */
+typedef struct avifgpu_light_level
+{
+    uint32_t max_code;  /* atomicMax of k over the pixels converted */
+    uint32_t reserved;  /* never written */
+    uint64_t level_sum; /* sum of level(k), units of 2^-22 x 10000 cd/m2 */
+    uint64_t pixels;    /* pixels converted */
+} avifgpu_light_level;
+
+/*
+ * avifgpu_encode_rows_device, plus the content light level of the rows converted, added into *device_acc.
+ *   - Same contract as avifgpu_encode_rows_device: any row block, every dest_layout, graph capture under the same rules.
+ *     The graph holds the accumulator's address: a replay adds into whatever the accumulator holds when it runs.
+ *   - Writes the same planes, bit for bit, with the same number of kernel launches as avifgpu_encode_rows_device.
+ *   - Row blocks add up: the blocks of an image accumulate what one call over the whole image does.
+ *   - Accepts host_depth 32 with transfer AVIFGPU_TRANSFER_PQ, in any layout, channel count, alpha state, chroma,
+ *     down_filter or row_matrix.  Every other description is AVIFGPU_ERR_UNSUPPORTED and launches nothing; a NULL
+ *     device_acc is AVIFGPU_ERR_BAD_PARAM.
+ *   - The tuned kernels read level(k) from a 2^image_bit_depth-word table the context builds with the step tables
+ *     (avifgpu_prepare_encode); a call captured before it exists takes the generic kernel, which evaluates level(k) itself:
+ *     the same result, a slower kernel.
+ * Not covered: the host-pointer, asynchronous, sharded and batch calls measure nothing, and the plug-in's row shuttle does
+ * not write `clli`. */
+AVIFGPU_EXPORT int avifgpu_encode_rows_device_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
+                                                          const void* device_rows, int64_t row_stride_bytes,
+                                                          int32_t y0, int32_t nrows, const avifgpu_planes* device_dst,
+                                                          avifgpu_light_level* device_acc, void* cuda_stream);
+
+/* MaxCLL and MaxFALL in cd/m2 from an accumulator copied to the host (pure host arithmetic):
+ *   MaxCLL  = ceil(10000 * level(max_code) / 2^22)
+ *   MaxFALL = ceil(10000 * level_sum / (2^22 * pixels)), exact (128-bit integers)
+ * Both are 0 when pixels == 0.  AVIFGPU_ERR_BAD_PARAM for a NULL pointer, an image_bit_depth other than 8, 10 or 12, a
+ * max_code above 2^image_bit_depth - 1, or a level_sum above 2^22 * pixels (not an accumulator of this depth). */
+AVIFGPU_EXPORT int avifgpu_content_light_level(const avifgpu_light_level* acc, int32_t image_bit_depth,
+                                               uint16_t* out_max_cll, uint16_t* out_max_fall);
 
 /* ---- the hot path: batches of small device-resident images ------------------------------------------------ */
 

@@ -53,6 +53,14 @@ def padded(n):
     return (n + 63) // 64 * 64 + 64
 
 
+def aligned_rows(dev, rows, cols, dtype, fill):
+    """A (rows, cols) torch view on `dev` whose rows start 256 bytes apart (what the tuned kernels' vector loads and stores
+    need), filled with `fill`."""
+    import torch
+    per_line = 256 // torch.empty((), dtype=dtype).element_size()
+    return torch.full((rows, -(-cols // per_line) * per_line), fill, dtype=dtype, device=dev)[:, :cols]
+
+
 def whole(plane):
     """The plane's bytes with the row padding (the sentinel) included."""
     return plane.as_strided((plane.shape[0], plane.stride(0)), (plane.stride(0), 1)).cpu().numpy()
@@ -652,6 +660,48 @@ def assert_same_as_direct(ctx, images, checker=None, threads=1):
                 if got is not None:
                     codes = got.cpu().numpy().view(abi.code_dtype(im.desc.image_bit_depth))
                     assert np.array_equal(codes, expected[k]), ("checker", im.w, im.h, k)
+
+
+def decode_counted(gpu, desc, planes, what):
+    """Decodes host `planes` through avifgpu_decode_rows_device from and into 256-byte aligned rows, asserts that the
+    tuned launcher served it (its kernel + the generic right strip: 2 launches; the generic kernel alone makes 1) and
+    returns the host floats."""
+    import torch
+    import avifgpu
+    dev = torch.device("cuda", gpu.device)
+    device_planes = []
+    for p in planes:
+        device_planes.append(None if p is None else aligned_rows(dev, p.shape[0], p.shape[1], torch.int16, 0))
+        if p is not None:
+            device_planes[-1].copy_(torch.from_numpy(p.view(np.int16)))
+    out = aligned_rows(dev, desc.height, desc.width * abi.decode_host_channels(desc), torch.float32, 0.0)
+    gpu.prepare_decode(desc)
+    before = gpu.launch_count()
+    gpu.decode_device(desc, avifgpu.planes_from_tensors(device_planes), out.data_ptr(), out.stride(0) * 4)
+    torch.cuda.synchronize(dev)
+    made = gpu.launch_count() - before
+    assert made == 2, f"{made} launches: {what} and its right strip make 2, the generic kernel alone 1"
+    return out.contiguous().cpu().numpy()
+
+
+def differing_samples(expected, got):
+    """Where two host arrays of decoded samples differ: floats bit for bit with NaN on both sides counting as equal,
+    integers as they are."""
+    if expected.dtype != np.float32:
+        return expected != got
+    nan_e, nan_g = np.isnan(expected), np.isnan(got)
+    return (nan_e != nan_g) | (~nan_e & (expected.view(np.uint32) != got.view(np.uint32)))
+
+
+def assert_same_floats(expected, got, planes, what):
+    """Bit for bit, NaN on both sides counting as equal; names the first differing pixels by their codes."""
+    bad = differing_samples(expected, got)
+    if bad.any():
+        channels = expected.shape[1] // planes[0].shape[1]
+        at = np.argwhere(bad)[:6]
+        shown = [f"codes {tuple(int(p[y, x // channels]) for p in planes if p is not None)} channel {x % channels}: "
+                 f"{expected[y, x]!r} expected, {got[y, x]!r}" for y, x in at]
+        pytest.fail(f"{what}: {int(bad.sum())} of {bad.size} samples differ; " + "; ".join(shown))
 
 
 def bits(a):

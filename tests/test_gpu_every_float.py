@@ -39,6 +39,7 @@ import cases
 import encode_spec
 import oracle
 from avifgpu import abi
+from gpu_harness import aligned_rows, assert_same_floats, decode_counted
 
 THREADS = max(1, min(32, len(os.sched_getaffinity(0))))
 CHUNK = 1 << 22             # bit patterns per host work item
@@ -233,21 +234,13 @@ def assert_codes(got, samples, depth, what):
                         + ", ".join(f"(0x{b:08x}, {e}, {g})" for b, e, g in examples))
 
 
-def padded(dev, rows, cols, dtype, fill):
-    """A (rows, cols) device view whose rows start 256 bytes apart (what the tuned kernels' vector loads and stores need),
-    filled with `fill`."""
-    import torch
-    per_line = 256 // torch.empty((), dtype=dtype).element_size()
-    return torch.full((rows, -(-cols // per_line) * per_line), fill, dtype=dtype, device=dev)[:, :cols]
-
-
 def fill_rows(dev, samples, channels, colours):
     """(h, W * channels) float rows: the samples in order over the first `colours` channels of each pixel, the rest 1.0
     (straight alpha), trailing pixels 0."""
     import torch
     per_row = W * colours
     h = -(-samples.n // per_row)
-    rows = padded(dev, h, W * channels, torch.float32, 0.0)
+    rows = aligned_rows(dev, h, W * channels, torch.float32, 0.0)
     px = rows.view(torch.int32).view(h, W, channels)
     if channels > colours:
         px[:, :, colours:] = ALPHA_ONE
@@ -266,7 +259,7 @@ def run(ctx, desc, rows, launches, what):
     import torch
     import avifgpu
     dev = rows.device
-    planes = [None if s is None else padded(dev, s[0], s[1], torch.int16, -1) for s in abi.encode_plane_shapes(desc)]
+    planes = [None if s is None else aligned_rows(dev, s[0], s[1], torch.int16, -1) for s in abi.encode_plane_shapes(desc)]
     before = ctx.launch_count()
     ctx.encode_device(desc, rows.data_ptr(), rows.stride(0) * 4, avifgpu.planes_from_tensors(planes))
     torch.cuda.synchronize(dev)
@@ -462,41 +455,6 @@ DECODES = {
     "hlg_ootf": (cases.NCLX_2020_HLG, dict(hlg_apply_ootf=1, hlg_display_gamma=1.2, hlg_peak_nits=1000)),
     "smpte428": (cases.NCLX_2020_428, dict()),
 }
-
-
-def decode_counted(gpu, desc, planes, what):
-    """Decodes host `planes` through avifgpu_decode_rows_device from and into 256-byte aligned rows, asserts that the
-    tuned launcher served it (its kernel + the generic right strip: 2 launches; the generic kernel alone makes 1) and
-    returns the host floats."""
-    import torch
-    import avifgpu
-    dev = torch.device("cuda", gpu.device)
-    device_planes = []
-    for p in planes:
-        device_planes.append(None if p is None else padded(dev, p.shape[0], p.shape[1], torch.int16, 0))
-        if p is not None:
-            device_planes[-1].copy_(torch.from_numpy(p.view(np.int16)))
-    out = padded(dev, desc.height, desc.width * abi.decode_host_channels(desc), torch.float32, 0.0)
-    gpu.prepare_decode(desc)
-    before = gpu.launch_count()
-    gpu.decode_device(desc, avifgpu.planes_from_tensors(device_planes), out.data_ptr(), out.stride(0) * 4)
-    torch.cuda.synchronize(dev)
-    made = gpu.launch_count() - before
-    assert made == TUNED, f"{made} launches: {what} and its right strip make {TUNED}, the generic kernel alone 1"
-    return out.contiguous().cpu().numpy()
-
-
-def assert_same_floats(expected, got, planes, what):
-    """Bit for bit, NaN on both sides counting as equal; names the first differing pixels by their codes."""
-    e, g = expected.view(np.uint32), got.view(np.uint32)
-    nan_e, nan_g = np.isnan(expected), np.isnan(got)
-    bad = (nan_e != nan_g) | (~nan_e & (e != g))
-    if bad.any():
-        channels = expected.shape[1] // planes[0].shape[1]
-        at = np.argwhere(bad)[:6]
-        shown = [f"codes {tuple(int(p[y, x // channels]) for p in planes if p is not None)} channel {x % channels}: "
-                 f"{expected[y, x]!r} expected, {got[y, x]!r}" for y, x in at]
-        pytest.fail(f"{what}: {int(bad.sum())} of {bad.size} samples differ; " + "; ".join(shown))
 
 
 @pytest.mark.gpu

@@ -843,6 +843,26 @@ AVIFGPU_EXPORT int avifgpu_build_yuv_tables(const avifgpu_nclx* nclx, int32_t bi
 
 // ---- device-pointer entry points -------------------------------------------------------------------------------
 
+// The level table of the description's image depth, or nullptr when the context has none yet.
+static const uint32_t* LightLevelsFor(const avifgpu_context* ctx, const avifgpu_encode_desc& d)
+{
+    return ctx->lightLevels[d.image_bit_depth == 8 ? 0 : d.image_bit_depth == 10 ? 1 : 2];
+}
+
+// The light-level calls' own checks, after the description's: float-host PQ encodes only, and an accumulator.
+static int CheckLightLevelCall(avifgpu_context* ctx, const avifgpu_encode_desc& d, const avifgpu_light_level* acc)
+{
+    if (d.host_depth != 32 || d.transfer != AVIFGPU_TRANSFER_PQ)
+    {
+        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "the content light level is measured on float-host PQ encodes only");
+    }
+    if (acc == nullptr)
+    {
+        return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL light-level accumulator");
+    }
+    return AVIFGPU_OK;
+}
+
 // The device-pointer encode; `acc` != nullptr: the light-level call, whose description the caller has checked.
 static int EncodeRowsDevice(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const void* device_rows, int64_t row_stride_bytes, int32_t y0,
                             int32_t nrows, const avifgpu_planes* device_dst, avifgpu_light_level* acc, void* cuda_stream)
@@ -888,7 +908,7 @@ static int EncodeRowsDevice(avifgpu_context* ctx, const avifgpu_encode_desc* des
     }
     p.smCount = ctx->smCount;
     ctx->FirstUseEncode(*desc, static_cast<int64_t>(desc->width) * nrows, capturing, &p);
-    const LightSink light = { acc, ctx->lightLevels[desc->image_bit_depth == 8 ? 0 : desc->image_bit_depth == 10 ? 1 : 2] };
+    const LightSink light = { acc, LightLevelsFor(ctx, *desc) };
     if (acc != nullptr && light.levels == nullptr)
     {
         p.curveTable = nullptr; // no level table (not built yet, or its allocation failed): the generic kernel evaluates the levels
@@ -933,18 +953,14 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_device_light_level(avifgpu_context* ctx, 
     avifgpu_encode_desc full;
     desc = WidenEncodeDesc(desc, &full);
     std::string error;
-    const int status = ValidateEncodeDesc(desc, &error);
+    int status = ValidateEncodeDesc(desc, &error);
     if (status != AVIFGPU_OK)
     {
         return ctx->Fail(status, error);
     }
-    if (desc->host_depth != 32 || desc->transfer != AVIFGPU_TRANSFER_PQ)
+    if ((status = CheckLightLevelCall(ctx, *desc, device_acc)) != AVIFGPU_OK)
     {
-        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "the content light level is measured on float-host PQ encodes only");
-    }
-    if (device_acc == nullptr)
-    {
-        return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL light-level accumulator");
+        return status;
     }
     return EncodeRowsDevice(ctx, desc, device_rows, row_stride_bytes, y0, nrows, device_dst, device_acc, cuda_stream);
 }
@@ -1045,8 +1061,12 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_device(avifgpu_context* ctx, const avifgp
     return AVIFGPU_OK;
 }
 
-AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const avifgpu_batch_image* images,
-                                               int32_t count, void* cuda_stream)
+} // extern "C"
+
+// The host-described batch encode; `acc` != nullptr: the light-level call, image i adding into acc[i] through the
+// light-level family's batched kernels and, for the other images, the direct light-level route.
+static int EncodeBatchDevice(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const avifgpu_batch_image* images, int32_t count,
+                             avifgpu_light_level* acc, void* cuda_stream)
 {
     if (ctx == nullptr)
     {
@@ -1102,11 +1122,24 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
     }
     shared.smCount = ctx->smCount;
     ctx->FirstUseEncode(*desc, pixels, capturing, &shared);
+    const LightSink light = { acc, LightLevelsFor(ctx, *desc) };
+    if (acc != nullptr && light.levels == nullptr)
+    {
+        shared.curveTable = nullptr; // no level table: every image takes the generic kernel, as a direct light-level call does
+    }
     BatchPlan plan;
-    PlanEncodeBatch(shared, desc->host_depth, planeMask, images, count, &plan);
+    if (acc != nullptr)
+    {
+        PlanEncodeLightBatch(shared, planeMask, images, count, &plan);
+    }
+    else
+    {
+        PlanEncodeBatch(shared, desc->host_depth, planeMask, images, count, &plan);
+    }
     for (const BatchChunk& chunk : plan.chunks)
     {
-        const int launched = LaunchEncodeBatchChunk(shared, desc->host_depth, chunk, cuda_stream);
+        const int launched = acc != nullptr ? LaunchEncodeLightBatchChunk(shared, chunk, light, cuda_stream)
+                                            : LaunchEncodeBatchChunk(shared, desc->host_depth, chunk, cuda_stream);
         if (launched < 0)
         {
             return ctx->LaunchFailed(launched, "batched encode kernel launch", capturing);
@@ -1117,7 +1150,8 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
     {
         EncodeParams p = shared;
         AdoptBatchImage(p, planeMask, images[i]);
-        const int launched = LaunchEncode(p, desc->host_depth, cuda_stream);
+        const LightSink own = { acc + i, light.levels };
+        const int launched = LaunchEncode(p, desc->host_depth, cuda_stream, acc != nullptr ? &own : nullptr);
         if (launched < 0)
         {
             return ctx->LaunchFailed(launched, "encode kernel launch", capturing);
@@ -1125,6 +1159,44 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifg
         ctx->launches += launched;
     }
     return AVIFGPU_OK;
+}
+
+extern "C" {
+
+AVIFGPU_EXPORT int avifgpu_encode_batch_device(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const avifgpu_batch_image* images,
+                                               int32_t count, void* cuda_stream)
+{
+    return EncodeBatchDevice(ctx, desc, images, count, nullptr, cuda_stream);
+}
+
+// The description is checked at size 0 (the images carry the sizes) for the light-level refusals, which come before the
+// images' own checks.
+AVIFGPU_EXPORT int avifgpu_encode_batch_device_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const avifgpu_batch_image* images,
+                                                           int32_t count, avifgpu_light_level* device_acc, void* cuda_stream)
+{
+    if (ctx == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    if (desc == nullptr)
+    {
+        return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL description");
+    }
+    avifgpu_encode_desc full;
+    avifgpu_encode_desc d = *WidenEncodeDesc(desc, &full);
+    d.width = 0;
+    d.height = 0;
+    std::string error;
+    int status = ValidateEncodeDesc(&d, &error);
+    if (status != AVIFGPU_OK)
+    {
+        return ctx->Fail(status, error);
+    }
+    if ((status = CheckLightLevelCall(ctx, d, device_acc)) != AVIFGPU_OK)
+    {
+        return status;
+    }
+    return EncodeBatchDevice(ctx, desc, images, count, device_acc, cuda_stream);
 }
 
 AVIFGPU_EXPORT int avifgpu_decode_batch_device(avifgpu_context* ctx, const avifgpu_decode_desc* desc, const avifgpu_batch_image* images,
@@ -1246,11 +1318,11 @@ namespace
     }
 } // namespace
 
-extern "C" {
-
-AVIFGPU_EXPORT int avifgpu_encode_batch_indirect(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const avifgpu_batch_image* device_images,
-                                                 const int32_t* device_count, int32_t max_count, void* device_workspace, size_t workspace_bytes,
-                                                 int32_t* device_status, void* cuda_stream)
+// The device-described batch encode; `acc` != nullptr: the light-level call (float hosts through the light-level family's
+// batched kernels), image i adding into acc[i].
+static int EncodeBatchIndirect(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const avifgpu_batch_image* device_images,
+                               const int32_t* device_count, int32_t max_count, void* device_workspace, size_t workspace_bytes,
+                               int32_t* device_status, avifgpu_light_level* acc, bool light, void* cuda_stream)
 {
     if (ctx == nullptr)
     {
@@ -1271,11 +1343,19 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_indirect(avifgpu_context* ctx, const avi
     {
         return ctx->Fail(status, error);
     }
+    if (light && (status = CheckLightLevelCall(ctx, d, acc)) != AVIFGPU_OK)
+    {
+        return status;
+    }
     if ((status = CheckIndirect(ctx, device_images, device_count, max_count, device_workspace, workspace_bytes)) != AVIFGPU_OK)
     {
         return status;
     }
-    if ((d.host_depth != 8 && d.host_depth != 16) || d.layout != AVIFGPU_LAYOUT_PLANAR_YCBCR)
+    if (light && (d.layout != AVIFGPU_LAYOUT_PLANAR_YCBCR || d.host_channels < 3))
+    {
+        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "device-described light-level batches encode RGB(A)32f hosts into planar YCbCr");
+    }
+    if (!light && ((d.host_depth != 8 && d.host_depth != 16) || d.layout != AVIFGPU_LAYOUT_PLANAR_YCBCR))
     {
         return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "device-described batches encode 8- or 16-bit RGB(A) hosts into planar YCbCr");
     }
@@ -1294,14 +1374,46 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_indirect(avifgpu_context* ctx, const avi
     }
     shared.smCount = ctx->smCount;
     ctx->FirstUseEncode(d, 0, capturing, &shared);
-    const int launched = LaunchEncodeIndirect(shared, d.host_depth, EncodeBatchFamilyOf(shared, d.host_depth), planeMask, device_images, device_count,
-                                              max_count, device_workspace, device_status, cuda_stream);
+    int launched;
+    if (light)
+    {
+        const LightSink sink = { acc, LightLevelsFor(ctx, d) };
+        if (sink.levels == nullptr)
+        {
+            shared.curveTable = nullptr; // no level table: every image through the edge kernel, which evaluates the levels
+        }
+        launched = LaunchEncodeLightIndirect(shared, planeMask, device_images, device_count, max_count, device_workspace, device_status, sink, cuda_stream);
+    }
+    else
+    {
+        launched = LaunchEncodeIndirect(shared, d.host_depth, EncodeBatchFamilyOf(shared, d.host_depth), planeMask, device_images, device_count, max_count,
+                                        device_workspace, device_status, cuda_stream);
+    }
     if (launched < 0)
     {
         return ctx->LaunchFailed(launched, "device-described batch encode launch", capturing);
     }
     ctx->launches += launched;
     return AVIFGPU_OK;
+}
+
+extern "C" {
+
+AVIFGPU_EXPORT int avifgpu_encode_batch_indirect(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const avifgpu_batch_image* device_images,
+                                                 const int32_t* device_count, int32_t max_count, void* device_workspace, size_t workspace_bytes,
+                                                 int32_t* device_status, void* cuda_stream)
+{
+    return EncodeBatchIndirect(ctx, desc, device_images, device_count, max_count, device_workspace, workspace_bytes, device_status, nullptr, false,
+                               cuda_stream);
+}
+
+AVIFGPU_EXPORT int avifgpu_encode_batch_indirect_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
+                                                             const avifgpu_batch_image* device_images, const int32_t* device_count,
+                                                             int32_t max_count, void* device_workspace, size_t workspace_bytes,
+                                                             int32_t* device_status, avifgpu_light_level* device_acc, void* cuda_stream)
+{
+    return EncodeBatchIndirect(ctx, desc, device_images, device_count, max_count, device_workspace, workspace_bytes, device_status, device_acc, true,
+                               cuda_stream);
 }
 
 AVIFGPU_EXPORT int avifgpu_decode_batch_indirect(avifgpu_context* ctx, const avifgpu_decode_desc* desc, const avifgpu_batch_image* device_images,

@@ -135,9 +135,10 @@ AVIFGPU_HD inline int AdoptBatchImage(Params& p, int planeMask, const avifgpu_ba
 // interiors take (EncodeBatchFamilyOf: RgbInt or Generic).  An image the tuned kernel takes in a direct call gets its
 // interior and the strips CompleteEncode would hand to the generic kernel; any other non-empty image becomes one
 // whole-image window, which is what the generic kernel converts in a direct call (the device-described batch runs that
-// window; the host-described one makes the direct call).
+// window; the host-described one makes the direct call).  Interior units are `unitPixels` wide: kBatchUnitPixels for
+// EncodeBatchFamilyOf's family, kLightBatchUnitPixels for EncodeLightBatchFamilyOf's.
 AVIFGPU_HD inline BatchImagePlan PlanBatchEncodeImage(const EncodeParams& shared, int hostDepth, EncodeFamily family, int planeMask,
-                                                       const avifgpu_batch_image& image)
+                                                       const avifgpu_batch_image& image, int unitPixels)
 {
     BatchImagePlan plan{};
     EncodeParams p = shared;
@@ -155,7 +156,7 @@ AVIFGPU_HD inline BatchImagePlan PlanBatchEncodeImage(const EncodeParams& shared
         return plan;
     }
     plan.interior = RecordOf(EncodeWindow(p, hostDepth, 0, 0, inner.width, inner.rows));
-    plan.interiorUnits = BatchInteriorUnits(inner.width, inner.rows, p.ys);
+    plan.interiorUnits = BatchInteriorUnits(inner.width, inner.rows, p.ys, unitPixels);
     Strip strip[2];
     plan.windows = InteriorStrips(p.width, p.rowCount, inner, strip);
     for (int k = 0; k < plan.windows; ++k)
@@ -164,6 +165,11 @@ AVIFGPU_HD inline BatchImagePlan PlanBatchEncodeImage(const EncodeParams& shared
         plan.windowUnits[k] = BatchEdgeUnits(strip[k].width, strip[k].rows, p.xs, p.ys);
     }
     return plan;
+}
+AVIFGPU_HD inline BatchImagePlan PlanBatchEncodeImage(const EncodeParams& shared, int hostDepth, EncodeFamily family, int planeMask,
+                                                       const avifgpu_batch_image& image)
+{
+    return PlanBatchEncodeImage(shared, hostDepth, family, planeMask, image, kBatchUnitPixels);
 }
 
 // The same for decodes (`family` = DecodeBatchFamilyOf; interior units of DecodeBatchUnitPixels); edge units are runs of
@@ -203,12 +209,17 @@ AVIFGPU_HD inline BatchImagePlan PlanBatchDecodeImage(const DecodeParams& shared
 // state, `planeMask` its planes (bit k: plane k); every image has passed AdoptBatchImage's checks.
 void PlanEncodeBatch(const EncodeParams& shared, int hostDepth, int planeMask, const avifgpu_batch_image* images, int32_t count, BatchPlan* plan);
 void PlanDecodeBatch(const DecodeParams& shared, int planeMask, const avifgpu_batch_image* images, int32_t count, BatchPlan* plan);
+// The same for a light-level batch of float images: EncodeLightBatchFamilyOf's family, kLightBatchUnitPixels units.
+void PlanEncodeLightBatch(const EncodeParams& shared, int planeMask, const avifgpu_batch_image* images, int32_t count, BatchPlan* plan);
 
 // The launchers (kernels_batch.cu): the plan, interior and edge kernels of one call on `stream`.  `shared` is the
 // description's block with the context's first-use state; `family` the family its interiors take (EncodeBatchFamilyOf /
 // DecodeBatchFamilyOf).  Return 3 (the launches) or a negative status.
 int LaunchEncodeIndirect(const EncodeParams& shared, int hostDepth, EncodeFamily family, int planeMask, const avifgpu_batch_image* images,
                          const int32_t* count, int maxCount, void* workspace, int32_t* status, void* stream);
+// The light-level one (float hosts, EncodeLightBatchFamilyOf): image i adds its content light level into light.acc[i].
+int LaunchEncodeLightIndirect(const EncodeParams& shared, int planeMask, const avifgpu_batch_image* images, const int32_t* count, int maxCount,
+                              void* workspace, int32_t* status, const LightSink& light, void* stream);
 int LaunchDecodeIndirect(const DecodeParams& shared, DecodeFamily family, int planeMask, const avifgpu_batch_image* images, const int32_t* count,
                          int maxCount, void* workspace, int32_t* status, void* stream);
 

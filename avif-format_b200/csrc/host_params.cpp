@@ -716,6 +716,17 @@ void PlanEncodeBatch(const EncodeParams& shared, int hostDepth, int planeMask, c
     }
 }
 
+void PlanEncodeLightBatch(const EncodeParams& shared, int planeMask, const avifgpu_batch_image* images, int32_t count, BatchPlan* plan)
+{
+    plan->chunks.clear();
+    plan->fallback.clear();
+    const EncodeFamily family = EncodeLightBatchFamilyOf(shared, 32);
+    for (int32_t i = 0; i < count; ++i)
+    {
+        AddToBatch(PlanBatchEncodeImage(shared, 32, family, planeMask, images[i], kLightBatchUnitPixels), i, plan);
+    }
+}
+
 void PlanDecodeBatch(const DecodeParams& shared, int planeMask, const avifgpu_batch_image* images, int32_t count, BatchPlan* plan)
 {
     plan->chunks.clear();

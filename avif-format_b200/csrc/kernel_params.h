@@ -301,6 +301,10 @@ constexpr int kRgbaTableBarrierBytes = 16;
 constexpr int kRgbaLaneStrideWords = 28; // 24 colour samples + padding: 16-byte aligned, conflict-free for STS.128
 constexpr int kRgbaStagePerWarp = 32 * kRgbaLaneStrideWords * 4;
 AVIFGPU_HD constexpr int RgbaFixedBytes() { return kSharedLibm + kRgbaTableBarrierBytes + kRgbaWarps * kRgbaStagePerWarp; }
+// EncodeLightF32BatchKernel (kernels_batch.cu): the RGBA kernel's layout with its own warp count -- libm tables, the table's
+// barrier, 28 words per lane of staged colour samples, the compact table; one CTA per SM for the whole launch.
+constexpr int kLightBatchWarps = 16;
+AVIFGPU_HD constexpr int LightBatchFixedBytes() { return kSharedLibm + kRgbaTableBarrierBytes + kLightBatchWarps * kRgbaStagePerWarp; }
 // EncodeGrayF32Kernel: libm tables, the table's barrier (padded), the compact table (PQ only), within 100 KiB.
 constexpr int kGrayF32FixedBytes = kSharedLibm + 16;
 constexpr int kGrayF32SharedLimit = 100 * 1024;
@@ -539,6 +543,22 @@ inline EncodeFamily EncodeBatchFamilyOf(const EncodeParams& p, int hostDepth)
 {
     return EncodeFamilyOf(p, hostDepth) == EncodeFamily::RgbInt ? EncodeFamily::RgbInt : EncodeFamily::Generic;
 }
+// For the light-level batches (avifgpu_encode_batch_device_light_level / _indirect_light_level): float planar RGB through
+// the PQ step table and float planar RGBA through the compact table, when the single-image light route takes them (it
+// has the compact table only: FlatCompactFits) and the compact table fits EncodeLightF32BatchKernel; generic otherwise.
+// A batch thus tunes exactly the images a direct light-level call tunes.  The caller leaves curveTable null when the
+// context has no level table for the depth, as the direct call does.
+inline EncodeFamily EncodeLightBatchFamilyOf(const EncodeParams& p, int hostDepth)
+{
+    const EncodeFamily family = EncodeFamilyOf(p, hostDepth);
+    if (hostDepth != 32 || p.transfer != AVIFGPU_TRANSFER_PQ || (family != EncodeFamily::RgbF32Flat && family != EncodeFamily::RgbaF32Flat))
+    {
+        return EncodeFamily::Generic;
+    }
+    const CurveTableView& t = *p.curveTable; // a tuned family has its verified table
+    const bool fits = FlatCompactFits(t) && static_cast<size_t>(LightBatchFixedBytes()) + t.compactImageBytes <= static_cast<size_t>(kSharedLimit);
+    return fits ? family : EncodeFamily::Generic;
+}
 // For decodes: YCbCr and planar RGB into every host depth,
 // except premultiplied alpha, which only the single-image table kernel un-premultiplies; generic otherwise.
 inline DecodeFamily DecodeBatchFamilyOf(const DecodeParams& p)
@@ -597,6 +617,9 @@ struct BatchRecord
 constexpr int kBatchChunkImages = 64;
 constexpr int kBatchUnitPixels = 256; // interior unit: 256 pixels of one row (row pair for 4:2:0), one warp
 constexpr int kF32BatchUnitPixels = 128; // the float YCbCr decode's interior unit: its single-image kernel's 128-pixel tile
+// The light-level float encode's interior unit (EncodeLightBatchFamilyOf): the single-image float kernels' 128-pixel tile of
+// one row, or of a 4:2:0 row pair, one warp, a lane on 4 pixels of each row.
+constexpr int kLightBatchUnitPixels = 128;
 constexpr int kBatchEdgeThreads = 256; // edge unit: one CTA-sized run of chroma sites (encode) or pixels (decode) of one row (pair)
 
 // Units of an interior of `width` x `rows` pixels, and of an edge window.
@@ -697,6 +720,13 @@ int CompleteDecode(cudaError_t tuned, const DecodeParams& p, int coveredWidth, i
 // description's block (its pointers, strides and sizes are unused).  Returns BatchChunkLaunches(chunk) or a negative status.
 int LaunchEncodeBatchChunk(const EncodeParams& shared, int hostDepth, const BatchChunk& chunk, void* stream);
 int LaunchDecodeBatchChunk(const DecodeParams& shared, const BatchChunk& chunk, void* stream);
+// The same for a chunk of a light-level batch (PlanEncodeLightBatch; float hosts): image chunk.imageIndex[j] /
+// chunk.windowImage[j] adds its content light level into light.acc[that index].
+int LaunchEncodeLightBatchChunk(const EncodeParams& shared, const BatchChunk& chunk, const LightSink& light, void* stream);
+
+// The block the generic encode kernels read (LaunchEncodeGeneric): a float host with a verified compact table gets its
+// by-value view.
+EncodeParams GenericEncodeView(const EncodeParams& params, int hostDepth);
 
 cudaError_t BuildGray16Lut(uint16_t* deviceLut, int smpte428, uint32_t maxCode, void* stream);
 

@@ -20,6 +20,11 @@
 //                                 (float_units.cuh), in the same units; the libm tables and every code's curve (and alpha)
 //                                 entry are staged once per CTA for the whole batch, not once per CTA per image;
 //   DecodeBatchKernel             the decode windows, with DecodeChunkPixel (generic_units.cuh).
+//   EncodeLightF32BatchKernel     the light-level float encode interiors (RGB(A)32f -> planar YCbCr through the PQ compact
+//                                 step table, the content light level of every image on the side); a warp takes one
+//                                 128-pixel tile of a row (4:2:0 row pair) at a time, and the libm tables and the step
+//                                 table are staged once per CTA for the whole batch;
+//   EncodeLightPlanarBatchKernel  the light-level encode windows, with EncodePlanarSite's light-level form.
 //
 // Each is a template on where its records come from:
 //   ChunkSource      a host-described chunk (PlanEncodeBatch / PlanDecodeBatch): the records and their unit total travel
@@ -36,8 +41,10 @@
 #include "generic_units.cuh"
 #include "int_units.cuh"
 #include "kernel_params.h"
+#include "kernels_fast_common.cuh"
 #include "launch_keys.h"
 #include "stream_units.cuh"
+#include "table_staging.cuh"
 #include "../../include/avifgpu.h"
 
 #include <climits>
@@ -134,6 +141,64 @@ struct WorkspaceSource
     };
 };
 
+// The records of a light-level launch, with the caller's image of each record and the sink its statistic goes to.  A host
+// chunk carries its records' images (BatchChunk::imageIndex / windowImage); in the workspace, interior i and windows 2i,
+// 2i + 1 are image i's.
+template <typename Shared, int N>
+struct LightChunkSource : ChunkSource<Shared, N>
+{
+    int32_t image[N];
+    LightSink light;
+
+    struct Walk : ChunkSource<Shared, N>::Walk
+    {
+        const int32_t* image;
+        __device__ __forceinline__ explicit Walk(const LightChunkSource& source) : ChunkSource<Shared, N>::Walk(source), image(source.image) {}
+        __device__ __forceinline__ int ImageOf(int record) const { return image[record]; }
+    };
+};
+
+template <typename Shared, int WINDOWS>
+struct LightWorkspaceSource : WorkspaceSource<Shared, WINDOWS>
+{
+    LightSink light;
+
+    struct Walk : WorkspaceSource<Shared, WINDOWS>::Walk
+    {
+        __device__ __forceinline__ explicit Walk(const LightWorkspaceSource& source) : WorkspaceSource<Shared, WINDOWS>::Walk(source) {}
+        __device__ __forceinline__ int ImageOf(int record) const { return WINDOWS ? record >> 1 : record; }
+    };
+};
+
+// A light-level worker's statistic and the image it belongs to.  It goes into that image's accumulator (FlushLightTally,
+// the whole warp converged) when the worker's next unit belongs to another image, and at exit.  `pixels` is the pixel
+// count of the records whose first unit the worker converted: every record's first unit is converted by exactly one
+// worker, and an image's records cover it exactly once, so each image's count is added once.
+struct ImageTally
+{
+    int image = -1;
+    LightTally tally{ 0u, 0ull };
+    uint64_t pixels = 0;
+
+    __device__ __forceinline__ void Flush(avifgpu_light_level* acc) const
+    {
+        if (image >= 0)
+        {
+            FlushLightTally(tally, pixels, acc + image);
+        }
+    }
+    __device__ __forceinline__ void Switch(int owner, avifgpu_light_level* acc)
+    {
+        if (owner != image)
+        {
+            Flush(acc);
+            image = owner;
+            tally = LightTally{ 0u, 0ull };
+            pixels = 0;
+        }
+    }
+};
+
 using RgbIntChunk = ChunkSource<Rgb16Params, kBatchChunkImages>;
 using PlanarChunk = ChunkSource<EncodeParams, 2 * kBatchChunkImages>;
 using YccIntChunk = ChunkSource<IntDecodeParams, kBatchChunkImages>;
@@ -147,6 +212,9 @@ static_assert(sizeof(RgbIntChunk) <= 32764 && sizeof(PlanarChunk) <= 32764 && si
               "a chunk must fit one kernel parameter block");
 static_assert(sizeof(YccF32Chunk) <= 32764, "a float decode chunk must fit one kernel parameter block");
 static_assert(sizeof(PlanarRgbIntChunk) <= 32764 && sizeof(PlanarRgbF32Chunk) <= 32764, "a planar-RGB decode chunk must fit one kernel parameter block");
+using LightF32Chunk = LightChunkSource<fastenc::FastEncodeParams, kBatchChunkImages>;
+using LightEdgeChunk = LightChunkSource<EncodeParams, 2 * kBatchChunkImages>;
+static_assert(sizeof(LightF32Chunk) <= 32764 && sizeof(LightEdgeChunk) <= 32764, "a light-level chunk must fit one kernel parameter block");
 static_assert(kF32DecodeThreads == kRgbThreads && kStreamThreads == kRgbThreads && kTableThreads == kRgbThreads, "the batched kernels share kWarps");
 
 // Block-wide exclusive scan of a pair of counts over kPlanThreads threads; every thread gets the block's totals too.
@@ -207,6 +275,17 @@ struct EncodePlanner
     __device__ __forceinline__ BatchImagePlan operator()(const avifgpu_batch_image& image) const
     {
         return PlanBatchEncodeImage(shared, hostDepth, family, planeMask, image);
+    }
+};
+
+struct LightEncodePlanner
+{
+    EncodeParams shared;
+    EncodeFamily family; // EncodeLightBatchFamilyOf
+    int32_t planeMask;
+    __device__ __forceinline__ BatchImagePlan operator()(const avifgpu_batch_image& image) const
+    {
+        return PlanBatchEncodeImage(shared, 32, family, planeMask, image, kLightBatchUnitPixels);
     }
 };
 
@@ -353,6 +432,259 @@ __global__ void __launch_bounds__(kBatchEdgeThreads) EncodePlanarBatchKernel(con
         p.rowCount = r.rowCount;
         EncodePlanarSite<HostT, kBatchEdgeThreads>(p, t, static_cast<unsigned>(unit - r.firstUnit));
     }
+}
+
+// The single-image RGBA kernel's per-lane work (kernels_fast_rgba.cu has the commentary) on one unit of kLightBatchUnitPixels
+// pixels of a row, or of a 4:2:0 row pair, a lane on 4 pixels of each row, with the unit's record's pointers and no
+// software pipelining: the next unit may belong to another image.  RGB hosts (CHANNELS 3) take the flat kernel's samples
+// as they are, RGBA hosts the RGBA kernel's clamp / premultiplication and alpha plane.  An interior is 4-pixel aligned, so
+// a lane is wholly inside its row or wholly past its end; a lane past it converts zeros and stores nothing.  Each pixel's
+// max(R', G', B') code goes into the warp's tally with its level from the context's table.
+template <typename Source, int CHANNELS, int XS, int YS, int DEST>
+__global__ void __launch_bounds__(kLightBatchWarps * 32, 1) EncodeLightF32BatchKernel(const __grid_constant__ Source s)
+{
+    using namespace fastenc;
+    const typename Source::Walk walk(s);
+    if (walk.Idle(static_cast<long long>(blockIdx.x) * kLightBatchWarps))
+    {
+        return;
+    }
+    const int count = walk.Count();
+    constexpr int kRows = YS ? 2 : 1;
+    constexpr int kPixels = 4 * kRows;
+    constexpr int kValues = 3 * kPixels;
+    const FastEncodeParams& d = s.shared;
+    extern __shared__ __align__(16) uint8_t sharedBytes[];
+    uint64_t* libmStorage = reinterpret_cast<uint64_t*>(sharedBytes);
+    uint64_t* tableBarrier = reinterpret_cast<uint64_t*>(sharedBytes + kSharedLibm);
+    uint32_t* stageAll = reinterpret_cast<uint32_t*>(sharedBytes + kSharedLibm + kRgbaTableBarrierBytes);
+    uint32_t* compactEntries = reinterpret_cast<uint32_t*>(sharedBytes + LightBatchFixedBytes());
+    const uint32_t* firstBits = compactEntries + ((d.table.flatCount + 3) & ~3);
+    if (threadIdx.x == 0)
+    {
+        staging::BeginTableImageCopy(d.table, compactEntries, tableBarrier);
+    }
+    const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
+    __syncthreads(); // the libm tables, the table barrier's initialisation
+    staging::WaitTableImage(tableBarrier);
+
+    const int lane = threadIdx.x & 31;
+    const int warpInBlock = threadIdx.x >> 5;
+    uint32_t* myStage = stageAll + warpInBlock * (32 * kRgbaLaneStrideWords) + lane * kRgbaLaneStrideWords;
+    const uint32_t flatShift = d.table.flatShift;
+    const int32_t negativeLow = -static_cast<int32_t>(d.table.flatLow);
+    const int32_t span = static_cast<int32_t>(d.table.flatHigh - d.table.flatLow);
+    const uint32_t bandStrideLog2 = d.table.bandStrideLog2;
+    const uint32_t* __restrict__ bandBits = d.table.bandBits;
+    const uint32_t compactTopShift = 32u - flatShift;
+    const uint32_t compactCodeMask = d.table.compactCodeMask;
+    const uint32_t compactMagic = d.table.compactMagic;
+    const long long warpCount = static_cast<long long>(gridDim.x) * kLightBatchWarps;
+    int record = 0;
+    ImageTally light;
+#pragma unroll 1
+    for (long long unit = static_cast<long long>(blockIdx.x) * kLightBatchWarps + warpInBlock; unit < walk.Units(); unit += warpCount)
+    {
+        record = walk.Find(count, record, unit);
+        const BatchRecord& r = walk.Record(record);
+        light.Switch(walk.ImageOf(record), s.light.acc);
+        const int local = static_cast<int>(unit - r.firstUnit);
+        if (local == 0)
+        {
+            light.pixels += static_cast<uint64_t>(r.width) * static_cast<uint64_t>(r.rowCount);
+        }
+        const int tilesX = (r.width + kLightBatchUnitPixels - 1) / kLightBatchUnitPixels;
+        const int unitRow = local / tilesX;
+        const int x = (local - unitRow * tilesX) * kLightBatchUnitPixels + lane * 4;
+        const bool laneActive = x < r.width;
+        const int64_t y = static_cast<int64_t>(unitRow) * kRows;
+        const uint8_t* source = static_cast<const uint8_t*>(r.rows) + y * r.rowStride + static_cast<int64_t>(x) * CHANNELS * 4;
+
+        // ---- 128-bit row loads; RGBA: alpha, clamp / premultiplication; then the colour samples the curve sees ----------
+        uint32_t colourBits[kValues];
+        uint32_t alphaCode[kPixels];
+        if constexpr (CHANNELS == 3)
+        {
+#pragma unroll
+            for (int q = 0; q < 3 * kRows; ++q)
+            {
+                const uint4 w = laneActive ? __ldg(reinterpret_cast<const uint4*>(source + (q / 3) * r.rowStride + 16 * (q % 3))) : make_uint4(0u, 0u, 0u, 0u);
+                colourBits[4 * q] = w.x;
+                colourBits[4 * q + 1] = w.y;
+                colourBits[4 * q + 2] = w.z;
+                colourBits[4 * q + 3] = w.w;
+            }
+        }
+        else
+        {
+            uint4 raw[kPixels]; // pixel i of row r = raw[4 * r + i] = { R, G, B, A }
+#pragma unroll
+            for (int k = 0; k < kPixels; ++k)
+            {
+                raw[k] = laneActive ? __ldg(reinterpret_cast<const uint4*>(source + (k / 4) * r.rowStride + 16 * (k % 4))) : make_uint4(0u, 0u, 0u, 0u);
+            }
+#pragma unroll
+            for (int k = 0; k < kPixels; ++k)
+            {
+                const float alpha = ClampF(__uint_as_float(raw[k].w), 0.0f, 1.0f);
+                float colour[3] = { __uint_as_float(raw[k].x), __uint_as_float(raw[k].y), __uint_as_float(raw[k].z) };
+                if (d.premultiply && alpha < 1.0f)
+                {
+#pragma unroll
+                    for (int c = 0; c < 3; ++c)
+                    {
+                        colour[c] = (alpha == 0) ? 0.0f : PremultiplyColor(ClampF(colour[c], 0.0f, 1.0f), alpha, 1.0f);
+                    }
+                }
+                alphaCode[k] = FloatToCode(alpha, d.maxCodeFloat);
+#pragma unroll
+                for (int c = 0; c < 3; ++c)
+                {
+                    colourBits[3 * k + c] = __float_as_uint(colour[c]);
+                }
+            }
+        }
+#pragma unroll
+        for (int q = 0; q < kValues / 4; ++q)
+        {
+            *reinterpret_cast<uint4*>(myStage + 4 * q) = make_uint4(colourBits[4 * q], colourBits[4 * q + 1], colourBits[4 * q + 2], colourBits[4 * q + 3]);
+        }
+
+        // ---- float -> code through the compact step table ----------------------------------------------------------
+        float codeF[kValuesPerLane] = {}; // one row (YS 0): the second row's codes stay 0 and are not stored
+        uint32_t bandMask = 0;
+        int32_t largest = 0; // max over the samples as signed integers: > 0x7f7fffff <=> a +inf / NaN is among them
+#pragma unroll
+        for (int j = 0; j < kValues; ++j)
+        {
+            bool inBand;
+            uint32_t entry;
+            codeF[j] = LookupCurveCompact<0>(colourBits[j], compactEntries, flatShift, negativeLow, span, compactTopShift, compactCodeMask, compactMagic, inBand, entry);
+            asm("{ .reg .pred q; setp.ne.u32 q, %1, 0; @q or.b32 %0, %0, %2; }" : "+r"(bandMask) : "r"(static_cast<uint32_t>(inBand)), "r"(1u << j));
+            largest = max(largest, static_cast<int32_t>(colourBits[j]));
+        }
+
+        // ---- in-band samples: which step, how far above its first_k, one bit of the band bitmap ------------------------
+        uint32_t lowerMask = 0;
+        {
+            uint32_t pending = bandMask;
+            while (pending != 0)
+            {
+                const int j = __ffs(static_cast<int>(pending)) - 1;
+                pending &= pending - 1;
+                const uint32_t bits = myStage[j];
+                const int32_t bucket = __viaddmin_s32_relu(static_cast<int32_t>(bits) >> flatShift, negativeLow, span);
+                const uint32_t entry = compactEntries[bucket];
+                const uint32_t k = ((entry & compactCodeMask) >> kCompactLenBits) + ((entry >> compactTopShift) != 0 ? 1u : 0u);
+                const uint32_t distance = bits - firstBits[k];
+                if (k != 0 && distance < (1u << bandStrideLog2)) // else flagged by the superset test only
+                {
+                    const uint32_t bitIndex = (k << bandStrideLog2) + distance;
+                    const uint32_t word = __ldg(bandBits + (bitIndex >> 5));
+                    lowerMask |= (((word >> (bitIndex & 31u)) & 1u) ^ 1u) << j;
+                }
+            }
+        }
+        // ---- +inf / NaN: the exact evaluation, lane by lane -------------------------------------------------------------
+        if (__any_sync(0xffffffffu, largest > 0x7f7fffff))
+        {
+            for (int j = 0; j < kValues; ++j)
+            {
+                const uint32_t bits = myStage[j];
+                if (static_cast<int32_t>(bits) > 0x7f7fffff)
+                {
+                    const float exact = CodeToFloat(ExactCurveCode<kCurveLinearToPQ>(__uint_as_float(bits), d.pqMultiplier, d.maxCodeFloat, t));
+#pragma unroll
+                    for (int slot = 0; slot < kValues; ++slot)
+                    {
+                        if (slot == j)
+                        {
+                            codeF[slot] = exact;
+                        }
+                    }
+                }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < kValues; ++j)
+        {
+            if (lowerMask & (1u << j))
+            {
+                codeF[j] -= 1.0f;
+            }
+        }
+        if (!laneActive)
+        {
+            continue; // the next unit starts with the whole warp again (Switch)
+        }
+#pragma unroll
+        for (int pixel = 0; pixel < kPixels; ++pixel)
+        {
+            const uint32_t k = __float2uint_rz(fmaxf(fmaxf(codeF[3 * pixel], codeF[3 * pixel + 1]), codeF[3 * pixel + 2]));
+            TallyCode(light.tally, k, __ldg(s.light.levels + k));
+        }
+        FastEncodeParams p = d;
+        p.strideY = r.planeStride[0];
+        p.strideCb = r.planeStride[1];
+        p.strideCr = r.planeStride[2];
+        const int64_t chromaRow = YS ? unitRow : y;
+        const int64_t chromaColumn = static_cast<int64_t>(XS ? (x >> 1) : x) * 2;
+        StoreTile<XS, YS, DEST>(p, codeF, static_cast<uint8_t*>(r.plane[0]) + y * p.strideY + static_cast<int64_t>(x) * 2,
+                                static_cast<uint8_t*>(r.plane[1]) + chromaRow * p.strideCb + chromaColumn * (SourceInterleaved(DEST) ? 2 : 1),
+                                static_cast<uint8_t*>(r.plane[2]) + chromaRow * p.strideCr + chromaColumn, kRows == 2);
+        if constexpr (CHANNELS == 4)
+        {
+#pragma unroll
+            for (int row = 0; row < kRows; ++row)
+            {
+                uint8_t* alphaRow = static_cast<uint8_t*>(r.plane[3]) + (y + row) * r.planeStride[3] + static_cast<int64_t>(x) * 2;
+                __stcs(reinterpret_cast<uint2*>(alphaRow), make_uint2(MsbWord<DEST>(alphaCode[4 * row] | (alphaCode[4 * row + 1] << 16), p),
+                                                                      MsbWord<DEST>(alphaCode[4 * row + 2] | (alphaCode[4 * row + 3] << 16), p)));
+            }
+        }
+    }
+    light.Flush(s.light.acc);
+}
+
+// EncodePlanarBatchKernel's light-level form for float hosts: the generic kernel's own per-site code with its tally, the
+// level read from the context's table or evaluated in place when there is none.
+template <typename Source>
+__global__ void __launch_bounds__(kBatchEdgeThreads, 1) EncodeLightPlanarBatchKernel(const __grid_constant__ Source s)
+{
+    const typename Source::Walk walk(s);
+    if (walk.Idle(blockIdx.x))
+    {
+        return;
+    }
+    const int count = walk.Count();
+    __shared__ uint64_t libmStorage[96];
+    const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
+    __syncthreads();
+    int record = 0;
+    ImageTally light;
+#pragma unroll 1
+    for (long long unit = blockIdx.x; unit < walk.Units(); unit += gridDim.x)
+    {
+        record = walk.Find(count, record, unit);
+        const BatchRecord& r = walk.Record(record);
+        light.Switch(walk.ImageOf(record), s.light.acc);
+        if (unit == r.firstUnit && threadIdx.x < 32) // the CTA's first warp counts the record's pixels
+        {
+            light.pixels += static_cast<uint64_t>(r.width) * static_cast<uint64_t>(r.rowCount);
+        }
+        EncodeParams p = s.shared;
+        p.rows = r.rows;
+        p.rowStride = r.rowStride;
+        for (int k = 0; k < 4; ++k)
+        {
+            p.plane[k] = r.plane[k];
+            p.planeStride[k] = r.planeStride[k];
+        }
+        p.width = r.width;
+        p.rowCount = r.rowCount;
+        EncodePlanarSite<float, kBatchEdgeThreads, 1>(p, t, static_cast<unsigned>(unit - r.firstUnit), &light.tally, s.light.levels);
+    }
+    light.Flush(s.light.acc);
 }
 
 template <typename Source, typename SampleT, int XS, int YS, int ALPHA, int SOURCE>
@@ -642,6 +974,42 @@ void LaunchPlanar(const Source& s, int hostDepth, unsigned grid, cudaStream_t st
     WithIntHost(hostDepth, [&](auto host) { EncodePlanarBatchKernel<Source, TypeOf<decltype(host)>><<<grid, kBatchEdgeThreads, 0, stream>>>(s); });
 }
 
+// The light-level float encode interiors, with `bytes` of shared memory (0 for a launch that plans no interior unit).
+template <typename Source>
+void LaunchLightF32(const Source& s, const EncodeParams& d, unsigned grid, size_t bytes, cudaStream_t stream)
+{
+    WithLightF32Key(d, [&](auto channels, auto xs, auto ys, auto dest) {
+        static std::atomic<uint64_t> configuredDevices{ 0 }; // per instantiation
+        const auto kernel = EncodeLightF32BatchKernel<Source, channels(), xs(), ys(), dest()>;
+        if (AllowDynamicShared(kernel, kSharedLimit, configuredDevices) == cudaSuccess)
+        {
+            kernel<<<grid, kLightBatchWarps * 32, bytes, stream>>>(s);
+        } // else the failed attribute call is the error Launched() finds
+    });
+}
+
+// The light-level interiors' description: the single-image float kernels' parameters without an image, and the compact
+// step table when the description has one.
+fastenc::FastEncodeParams LightF32Shared(const EncodeParams& d)
+{
+    fastenc::FastEncodeParams fp{};
+    fp.premultiply = d.premultiply;
+    fp.pqMultiplier = d.pqMultiplier;
+    fp.maxCodeFloat = d.maxCodeFloat;
+    fp.maxCode = static_cast<int32_t>(d.maxCode);
+    fp.matrix = d.matrix;
+    fp.chromaOffset = d.chromaOffset;
+    fp.topLeft = d.topLeft;
+    if (d.curveTable != nullptr)
+    {
+        fp.table = *d.curveTable;
+    }
+    return fp;
+}
+
+// The shared memory of EncodeLightF32BatchKernel over the description's step table.
+size_t LightF32Bytes(const EncodeParams& d) { return static_cast<size_t>(LightBatchFixedBytes()) + d.curveTable->compactImageBytes; }
+
 // The YCbCr decode interiors into 8/16-bit hosts, with `bytes` of staged tables.
 template <typename Source>
 void LaunchYccInt(const Source& s, const DecodeParams& d, unsigned grid, size_t bytes, cudaStream_t stream)
@@ -737,6 +1105,18 @@ Chunk ChunkOf(const decltype(Chunk::shared)& shared, const BatchRecord* records,
     return b;
 }
 
+template <typename Chunk>
+Chunk LightChunkOf(const decltype(Chunk::shared)& shared, const BatchRecord* records, const int32_t* images, int count, int64_t units, const LightSink& light)
+{
+    Chunk b = ChunkOf<Chunk>(shared, records, count, units);
+    for (int i = 0; i < count; ++i)
+    {
+        b.image[i] = images[i];
+    }
+    b.light = light;
+    return b;
+}
+
 // `launches` if the launches before it succeeded, else the failure's status.
 int Launched(int launches)
 {
@@ -759,6 +1139,23 @@ int LaunchEncodeBatchChunk(const EncodeParams& shared, int hostDepth, const Batc
         return interior;
     }
     LaunchPlanar(ChunkOf<PlanarChunk>(PlanarShared(shared), chunk.window, chunk.windows, chunk.windowUnits), hostDepth, GridFor(chunk.windowUnits, cap), stream);
+    return Launched(2);
+}
+
+int LaunchEncodeLightBatchChunk(const EncodeParams& shared, const BatchChunk& chunk, const LightSink& light, void* streamHandle)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
+    const int smCount = SmCountOrDefault(shared.smCount);
+    // one warp per unit, one CTA per SM: the step table is staged once per CTA
+    LaunchLightF32(LightChunkOf<LightF32Chunk>(LightF32Shared(shared), chunk.interior, chunk.imageIndex, chunk.images, chunk.interiorUnits, light), shared,
+                   GridFor((chunk.interiorUnits + kLightBatchWarps - 1) / kLightBatchWarps, smCount), LightF32Bytes(shared), stream);
+    const int interior = Launched(1);
+    if (interior < 0 || chunk.windows == 0)
+    {
+        return interior;
+    }
+    EncodeLightPlanarBatchKernel<LightEdgeChunk><<<GridFor(chunk.windowUnits, static_cast<long long>(smCount) * kStreamBlocksPerSm), kBatchEdgeThreads, 0, stream>>>(
+        LightChunkOf<LightEdgeChunk>(GenericEncodeView(shared, 32), chunk.window, chunk.windowImage, chunk.windows, chunk.windowUnits, light));
     return Launched(2);
 }
 
@@ -817,6 +1214,41 @@ int LaunchEncodeIndirect(const EncodeParams& shared, int hostDepth, EncodeFamily
         return AVIFGPU_ERR_CUDA;
     }
     LaunchPlanar(WorkspaceSource<EncodeParams, 1>{ PlanarShared(shared), workspace, maxCount }, hostDepth, cap, stream);
+    return Launched(3);
+}
+
+int LaunchEncodeLightIndirect(const EncodeParams& shared, int planeMask, const avifgpu_batch_image* images, const int32_t* count, int maxCount,
+                              void* workspace, int32_t* status, const LightSink& light, void* streamHandle)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
+    const int smCount = SmCountOrDefault(shared.smCount);
+    LightEncodePlanner planner{};
+    planner.shared = shared;
+    planner.family = EncodeLightBatchFamilyOf(shared, 32);
+    planner.planeMask = planeMask;
+    PlanIndirectKernel<LightEncodePlanner><<<1, kPlanThreads, 0, stream>>>(planner, images, count, maxCount, workspace, status);
+    if (Launched(1) < 0)
+    {
+        return AVIFGPU_ERR_CUDA;
+    }
+    // Without the tuned family (no step or level table, as in a capture before prepare) the plan has no interior unit and
+    // the interior grid returns before staging anything, so it gets no shared memory.
+    LightWorkspaceSource<fastenc::FastEncodeParams, 0> interior{};
+    interior.shared = LightF32Shared(shared);
+    interior.workspace = workspace;
+    interior.maxCount = maxCount;
+    interior.light = light;
+    LaunchLightF32(interior, shared, static_cast<unsigned>(smCount), planner.family != EncodeFamily::Generic ? LightF32Bytes(shared) : 0, stream);
+    if (Launched(1) < 0)
+    {
+        return AVIFGPU_ERR_CUDA;
+    }
+    LightWorkspaceSource<EncodeParams, 1> edge{};
+    edge.shared = GenericEncodeView(shared, 32);
+    edge.workspace = workspace;
+    edge.maxCount = maxCount;
+    edge.light = light;
+    EncodeLightPlanarBatchKernel<LightWorkspaceSource<EncodeParams, 1>><<<static_cast<unsigned>(smCount * kStreamBlocksPerSm), kBatchEdgeThreads, 0, stream>>>(edge);
     return Launched(3);
 }
 

@@ -165,13 +165,8 @@ __global__ void __launch_bounds__(kThreads) TransferKernel(int function, float p
 
 } // namespace
 
-int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* streamHandle, const LightSink* light)
+EncodeParams GenericEncodeView(const EncodeParams& params, int hostDepth)
 {
-    cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
-    if (params.width <= 0 || params.rowCount <= 0)
-    {
-        return 0;
-    }
     EncodeParams p = params;
     p.useCurveView = 0;
     if (hostDepth == 32 && p.curveTable != nullptr && p.curveTable->compact != nullptr && p.curveTable->bandBits != nullptr &&
@@ -180,6 +175,17 @@ int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* streamH
         p.curveView = *p.curveTable;
         p.useCurveView = 1;
     }
+    return p;
+}
+
+int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* streamHandle, const LightSink* light)
+{
+    cudaStream_t stream = static_cast<cudaStream_t>(streamHandle);
+    if (params.width <= 0 || params.rowCount <= 0)
+    {
+        return 0;
+    }
+    const EncodeParams p = GenericEncodeView(params, hostDepth);
     if (p.planar)
     {
         const int sitesX = (p.width + p.xs) >> p.xs;

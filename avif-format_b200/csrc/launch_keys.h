@@ -99,6 +99,17 @@ auto WithRgbIntKey(const EncodeParams& d, int hostDepth, F&& f)
     });
 }
 
+// Light-level float encode interiors (EncodeLightF32BatchKernel).  f(CHANNELS, XS, YS, DEST): RGB (3) or RGBA (4; straight
+// or premultiplied is a runtime value, as in the single-image RGBA kernel) x chroma x destination layout.
+template <typename F>
+auto WithLightF32Key(const EncodeParams& d, F&& f)
+{
+    const auto withChannels = [&](auto channels) {
+        return WithChroma(d.xs, d.ys, [&](auto xs, auto ys) { return WithLayout(d.destLayout, [&](auto dest) { return f(channels, xs, ys, dest); }); });
+    };
+    return d.channels == 4 ? withChannels(Int<4>{}) : withChannels(Int<3>{});
+}
+
 // Decodes into 8/16-bit hosts.  f(SampleT, ALPHA): uint8_t for 8-bit hosts, uint16_t for anything else, x alpha.  The
 // planar-RGB kernels (StreamDecodeKernel, DecodePlanarRgbIntBatchKernel) take 3 + ALPHA channels, the monochrome
 // instantiations of StreamDecodeKernel 1 + ALPHA.

@@ -76,7 +76,11 @@ def library():
         [ctx_p, C.POINTER(abi.EncodeDesc), C.POINTER(abi.BatchImage), C.c_int32, C.c_void_p])
     sig("avifgpu_decode_batch_device", C.c_int,
         [ctx_p, C.POINTER(abi.DecodeDesc), C.POINTER(abi.BatchImage), C.c_int32, C.c_void_p])
+    sig("avifgpu_encode_batch_device_light_level", C.c_int,
+        [ctx_p, C.POINTER(abi.EncodeDesc), C.POINTER(abi.BatchImage), C.c_int32, C.c_void_p, C.c_void_p])
     sig("avifgpu_batch_workspace_bytes", C.c_int, [C.c_int32, C.POINTER(C.c_size_t)])
+    sig("avifgpu_encode_batch_indirect_light_level", C.c_int,
+        [ctx_p, C.POINTER(abi.EncodeDesc), C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p])
     for name, desc_type in (("avifgpu_encode_batch_indirect", abi.EncodeDesc), ("avifgpu_decode_batch_indirect", abi.DecodeDesc)):
         sig(name, C.c_int, [ctx_p, C.POINTER(desc_type), C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p])
     sig("avifgpu_transfer_f32", C.c_int, [ctx_p, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_size_t])
@@ -146,6 +150,7 @@ EXPORTED_SYMBOLS = [
     "avifgpu_shard_group_synchronize", "avifgpu_shard_row_blocks", "avifgpu_encode_rows_sharded", "avifgpu_decode_rows_sharded",
     "avifgpu_encode_rows_sharded_device", "avifgpu_icc_to_rec2020_linear_matrix",
     "avifgpu_encode_rows_device_light_level", "avifgpu_content_light_level",
+    "avifgpu_encode_batch_device_light_level", "avifgpu_encode_batch_indirect_light_level",
 ]
 
 
@@ -337,6 +342,11 @@ class Context:
         """avifgpu_encode_batch_device: `images` is a ctypes array of abi.BatchImage (see batch_images_from_tensors)."""
         self._check(self.lib.avifgpu_encode_batch_device(self.handle, C.byref(desc), images, len(images), stream))
 
+    def encode_batch_device_light_level(self, desc, images, acc_ptr, stream=0):
+        """avifgpu_encode_batch_device_light_level: encode_batch_device, plus image i's content light level added into the
+        device accumulator acc_ptr[i] (len(images) abi.LightLevel entries, zeroed by the caller)."""
+        self._check(self.lib.avifgpu_encode_batch_device_light_level(self.handle, C.byref(desc), images, len(images), acc_ptr, stream))
+
     def decode_batch_device(self, desc, images, stream=0):
         """avifgpu_decode_batch_device: `images` is a ctypes array of abi.BatchImage (planes = source, rows = destination)."""
         self._check(self.lib.avifgpu_decode_batch_device(self.handle, C.byref(desc), images, len(images), stream))
@@ -346,6 +356,13 @@ class Context:
         `status` (max_count int32, or None) are CUDA tensors, read when the work runs on `stream`."""
         self._check(self.lib.avifgpu_encode_batch_indirect(self.handle, C.byref(desc), *_indirect_args(images, count, max_count, workspace, status),
                                                            stream))
+
+    def encode_batch_indirect_light_level(self, desc, images, count, max_count, workspace, acc_ptr, status=None, stream=0):
+        """avifgpu_encode_batch_indirect_light_level: encode_batch_indirect, plus image i's content light level added into
+        the device accumulator acc_ptr[i] (max_count abi.LightLevel entries, zeroed by the caller)."""
+        self._check(self.lib.avifgpu_encode_batch_indirect_light_level(self.handle, C.byref(desc),
+                                                                       *_indirect_args(images, count, max_count, workspace, status), acc_ptr,
+                                                                       stream))
 
     def decode_batch_indirect(self, desc, images, count, max_count, workspace, status=None, stream=0):
         """avifgpu_decode_batch_indirect: as encode_batch_indirect (planes = source, rows = destination)."""

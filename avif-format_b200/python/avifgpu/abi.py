@@ -8,7 +8,7 @@ import ctypes as C
 
 import numpy as np
 
-API_VERSION = 12
+API_VERSION = 13
 
 # avifgpu_status
 OK = 0

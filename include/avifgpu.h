@@ -50,7 +50,7 @@ extern "C" {
 #define AVIFGPU_EXPORT __attribute__((visibility("default")))
 #endif
 
-#define AVIFGPU_API_VERSION 12
+#define AVIFGPU_API_VERSION 13
 
 typedef enum avifgpu_status
 {
@@ -438,8 +438,9 @@ typedef struct avifgpu_light_level
  *   - The tuned kernels read level(k) from a 2^image_bit_depth-word table the context builds with the step tables
  *     (avifgpu_prepare_encode); a call captured before it exists takes the generic kernel, which evaluates level(k) itself:
  *     the same result, a slower kernel.
- * Not covered: the host-pointer, asynchronous, sharded and batch calls measure nothing, and the plug-in's row shuttle does
- * not write `clli`. */
+ * Since API version 13 the batch calls have light-level forms too (avifgpu_encode_batch_device_light_level,
+ * avifgpu_encode_batch_indirect_light_level, below): one accumulator per image.  Not covered: the host-pointer,
+ * asynchronous and sharded calls measure nothing, and the plug-in's row shuttle does not write `clli`. */
 AVIFGPU_EXPORT int avifgpu_encode_rows_device_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
                                                           const void* device_rows, int64_t row_stride_bytes,
                                                           int32_t y0, int32_t nrows, const avifgpu_planes* device_dst,
@@ -553,6 +554,43 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_indirect(avifgpu_context* ctx, const avi
                                                  const avifgpu_batch_image* device_images, const int32_t* device_count,
                                                  int32_t max_count, void* device_workspace, size_t workspace_bytes,
                                                  int32_t* device_status, void* cuda_stream);
+
+/* ---- content light level of batches (since API version 13) ------------------------------------------------------- */
+
+/*
+ * The batch calls plus each image's content light level: thumbnails, previews, image collections and burst or bracket
+ * sets of HDR stills, every one of which carries its own `clli`.
+ *   - Statistic: avifgpu_light_level, level(k) and avifgpu_content_light_level as in API version 12.  device_acc[i]
+ *     (device memory, zeroed by the caller; calls add into it) gains exactly what one avifgpu_encode_rows_device_light_level
+ *     call over image i whole (y0 = 0, nrows = height) adds.  Empty images, images the device-described call rejects
+ *     (device_status[i] = AVIFGPU_ERR_BAD_PARAM) and every image of an out-of-range *device_count leave their entry as it is.
+ *   - Planes: the host-described call writes, bit for bit, what avifgpu_encode_batch_device writes for the same images
+ *     (one direct call per image), padding included; the device-described call writes what the direct call writes for
+ *     every accepted image.
+ *   - Descriptions: the host-described call accepts what avifgpu_encode_rows_device_light_level accepts (host_depth 32,
+ *     AVIFGPU_TRANSFER_PQ; any layout, channel count, alpha state, chroma, down_filter, row_matrix, dest_layout); the
+ *     device-described call the planar YCbCr part of that (AVIFGPU_LAYOUT_PLANAR_YCBCR, RGB or RGBA hosts, any
+ *     dest_layout).  Anything else is AVIFGPU_ERR_UNSUPPORTED and launches nothing; a NULL device_acc is
+ *     AVIFGPU_ERR_BAD_PARAM.  Every check of the plain calls applies as it stands (images validated before any launch,
+ *     max_count, workspace size, NULLs).
+ *   - Launches: RGB32f and RGBA32f images the direct light-level call tunes (planar YCbCr through the PQ compact step table,
+ *     aligned buffers, width >= 4) go in chunks of up to 64 images, at most two launches per chunk (interiors, then right
+ *     strips and odd last 4:2:0 rows); every other non-empty image takes one direct light-level call, with that call's
+ *     route and launches, after the chunks.  The device-described call makes exactly three launches (plan, interiors,
+ *     edges), n = 0 included.  avifgpu_launch_count counts them.
+ *   - Capture: as for the device calls; the graph holds the accumulator array's address.  A call captured before
+ *     avifgpu_prepare_encode has no step table and no level table and sends every image through the generic per-site code,
+ *     which evaluates level(k) itself: the same planes and integers, a slower kernel.
+ *   - Workspace: the device-described call's is sized by avifgpu_batch_workspace_bytes, as for the plain call.
+ */
+AVIFGPU_EXPORT int avifgpu_encode_batch_device_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
+                                                           const avifgpu_batch_image* images, int32_t count,
+                                                           avifgpu_light_level* device_acc, void* cuda_stream);
+AVIFGPU_EXPORT int avifgpu_encode_batch_indirect_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
+                                                             const avifgpu_batch_image* device_images, const int32_t* device_count,
+                                                             int32_t max_count, void* device_workspace, size_t workspace_bytes,
+                                                             int32_t* device_status, avifgpu_light_level* device_acc,
+                                                             void* cuda_stream);
 
 /* ---- the hot path across several GPUs of one box (SURVEY.md 8e) ------------------------------------------------ */
 

@@ -141,6 +141,12 @@ struct avifgpu_context
         // What the slot still owes the caller once its stream has drained: owed[b] copies pinned[b] into pageable caller
         // memory (libheif's planes on the encode side, pageable host rows on the decode side); rows == 0 when nothing.
         RowCopy owed[kSlotBuffers] = {};
+        // The light-level host encode's per-slice statistic: a device accumulator and its pinned mirror, allocated at the
+        // first light-level slice.  owedLight is the caller's accumulator the mirror still has to be merged into (a debt
+        // like owed[], paid once the slice is done), nullptr when nothing.
+        avifgpu_light_level* lightDevice = nullptr;
+        avifgpu_light_level* lightMirror = nullptr;
+        avifgpu_light_level* owedLight = nullptr;
     };
     Slot slots[kPipelineStreams];
     int nextSlot = 0;
@@ -690,6 +696,8 @@ AVIFGPU_EXPORT void avifgpu_destroy(avifgpu_context* ctx)
             if (slot.device[b].ptr) cudaFree(slot.device[b].ptr);
             if (slot.pinned[b].ptr) cudaFreeHost(slot.pinned[b].ptr);
         }
+        if (slot.lightDevice) cudaFree(slot.lightDevice);
+        if (slot.lightMirror) cudaFreeHost(slot.lightMirror);
     }
     for (auto& b : ctx->transferScratch)
     {
@@ -1483,8 +1491,9 @@ AVIFGPU_EXPORT int avifgpu_decode_batch_indirect(avifgpu_context* ctx, const avi
 // A call is cut into row-block slices; slice i uses pipeline slot i mod kPipelineStreams (a stream, device staging,
 // pinned bounce buffers).  Caller memory that is not page-locked is bounced through the slot's pinned buffers on BOTH
 // sides -- a copy to or from pageable memory would make the driver stage it synchronously and serialise the pipeline.
-// The bounce -> pageable copies of a slot's last slice stay owed (its debts) until the slot's next slice or a retire
-// pays them.  Slots retire in issue order, so "everything up to ticket t" is a prefix.
+// The bounce -> pageable copies of a slot's last slice, and a light-level encode's merge of the slice's statistic into the
+// caller's accumulator, stay owed (its debts) until the slot's next slice or a retire pays them.  Slots retire in issue
+// order, so "everything up to ticket t" is a prefix.
 //
 // Both directions run a slice through the same steps: AcquireSlot, StageIn, the kernel launch, StageOut, CloseSlice.
 // Every pinned buffer those steps write into or regrow comes from TakePinned, which first pays the debts that read it.
@@ -1662,13 +1671,34 @@ static int WaitSlot(avifgpu_context* ctx, Slot& slot)
     if (status != AVIFGPU_OK)
     {
         for (RowCopy& c : slot.owed) c.rows = 0;
+        slot.owedLight = nullptr;
     }
     slot.busy = false;
     return status;
 }
 
+// Adds a partial statistic into a host accumulator (the statistic does not depend on the order of its parts);
+// `reserved` is never written.
+static void AddLightLevel(avifgpu_light_level& acc, const avifgpu_light_level& part)
+{
+    acc.max_code = std::max(acc.max_code, part.max_code);
+    acc.level_sum += part.level_sum;
+    acc.pixels += part.pixels;
+}
+
+// Merges the light-level mirror of a waited-for slot into the caller's accumulator it is owed to, on the caller's thread.
+static void PayLightDebt(Slot& slot)
+{
+    if (slot.owedLight != nullptr)
+    {
+        AddLightLevel(*slot.owedLight, *slot.lightMirror);
+        slot.owedLight = nullptr;
+    }
+}
+
 // Pays, in one batch for the copy pool, what a waited-for slot owes out of the pinned buffers marked in `buffers` (out
-// of all of them when nullptr).  Separate batches would cost a wake-up and a wait each.
+// of all of them, and the light-level merge, when nullptr: whoever takes or retires the slot then finds it owing nothing,
+// so every debt stays with the ticket of the slice that made it).  Separate batches would cost a wake-up and a wait each.
 static void PayDebts(Slot& slot, const bool* buffers = nullptr)
 {
     RowCopy batch[kSlotBuffers];
@@ -1682,6 +1712,7 @@ static void PayDebts(Slot& slot, const bool* buffers = nullptr)
         }
     }
     if (count > 0) CopyPool::Instance().Copy(batch, count); // the pool's threads start at the first copy
+    if (buffers == nullptr) PayLightDebt(slot);
 }
 
 // Retires, oldest first, every slot issued by a call with ticket <= `ticket`.
@@ -1691,7 +1722,7 @@ static int RetireThrough(avifgpu_context* ctx, int64_t ticket)
     for (int i = 0; i < kPipelineStreams; ++i)
     {
         Slot& slot = ctx->slots[(ctx->nextSlot + i) % kPipelineStreams]; // nextSlot is the oldest
-        bool owes = false;
+        bool owes = slot.owedLight != nullptr;
         for (const RowCopy& c : slot.owed) owes = owes || c.rows > 0;
         if ((slot.busy || owes) && slot.ticket <= ticket)
         {
@@ -1721,6 +1752,7 @@ static int AbandonCall(avifgpu_context* ctx, int status)
     {
         cudaStreamSynchronize(slot.stream);
         for (RowCopy& c : slot.owed) c.rows = 0;
+        slot.owedLight = nullptr;
         slot.busy = false;
     }
     cudaGetLastError();
@@ -1888,8 +1920,39 @@ static int CloseSlice(avifgpu_context* ctx, Slot& slot, int64_t ticket)
     return status;
 }
 
+// The light-level slice's first step, once the slot is acquired: the slot's accumulator, allocated at first use, cleared.
+static int ClearSliceLight(avifgpu_context* ctx, Slot& slot)
+{
+    int status = AVIFGPU_OK;
+    if (slot.lightDevice == nullptr)
+    {
+        status = ctx->Cuda(cudaMalloc(&slot.lightDevice, sizeof(avifgpu_light_level)), "cudaMalloc");
+    }
+    if (status == AVIFGPU_OK && slot.lightMirror == nullptr)
+    {
+        status = ctx->Cuda(cudaHostAlloc(&slot.lightMirror, sizeof(avifgpu_light_level), cudaHostAllocDefault), "cudaHostAlloc");
+    }
+    return status != AVIFGPU_OK ? status : ctx->Cuda(cudaMemsetAsync(slot.lightDevice, 0, sizeof(avifgpu_light_level), slot.stream), "cudaMemsetAsync");
+}
+
+// Queues, after the slice's kernel and StageOut, the copy of the slot's accumulator into its pinned mirror, and makes
+// merging the mirror into the caller's `acc` a debt of the slot.  Like a pinned buffer, the mirror is not rewritten while
+// the slot still owes out of it: StageOut has paid every debt of the slot's previous slice, its merge included.
+static int StageLightOut(avifgpu_context* ctx, Slot& slot, avifgpu_light_level* acc)
+{
+    const int status = ctx->Cuda(cudaMemcpyAsync(slot.lightMirror, slot.lightDevice, sizeof(avifgpu_light_level), cudaMemcpyDeviceToHost, slot.stream),
+                                 "D2H light level");
+    if (status == AVIFGPU_OK)
+    {
+        slot.owedLight = acc;
+    }
+    return status;
+}
+
+// The host-pointer encode; `measure`: the light-level call, which adds the content light level of the rows into the host
+// accumulator `acc` through the slots' own accumulators (merged as slot debts, see avifgpu.h for when `acc` is complete).
 static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const void* host_rows, int64_t row_stride_bytes, int32_t y0,
-                          int32_t nrows, const avifgpu_planes* dst, bool wait, int64_t* out_ticket)
+                          int32_t nrows, const avifgpu_planes* dst, bool wait, int64_t* out_ticket, bool measure, avifgpu_light_level* acc)
 {
     if (ctx == nullptr)
     {
@@ -1902,6 +1965,10 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
     if (status != AVIFGPU_OK)
     {
         return ctx->Fail(status, error);
+    }
+    if (measure && (status = CheckLightLevelCall(ctx, *desc, acc)) != AVIFGPU_OK)
+    {
+        return status;
     }
     if (DestLayoutOf(*desc) != AVIFGPU_SOURCE_PLANAR)
     {
@@ -1942,6 +2009,11 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
 
     base.smCount = ctx->smCount;
     ctx->FirstUseEncode(*desc, static_cast<int64_t>(desc->width) * nrows, false, &base);
+    const uint32_t* levels = LightLevelsFor(ctx, *desc);
+    if (measure && levels == nullptr)
+    {
+        base.curveTable = nullptr; // no level table: the generic kernel evaluates the levels (as EncodeRowsDevice)
+    }
     const int64_t rowPayload = static_cast<int64_t>(desc->width) * EncodeHostColBytes(*desc);
     const int64_t deviceRowStride = (rowPayload + 255) & ~255ll;
     const bool rowsPinned = IsPinned(host_rows);
@@ -1988,14 +2060,17 @@ static int EncodeRowsHost(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
             p.plane[out[i].buffer] = slot.device[out[i].buffer].ptr;
             p.planeStride[out[i].buffer] = out[i].deviceStride;
         }
-        const int launched = LaunchEncode(p, desc->host_depth, slot.stream);
+        if (measure && (status = ClearSliceLight(ctx, slot)) != AVIFGPU_OK) return AbandonCall(ctx, status);
+        const LightSink light = { slot.lightDevice, levels };
+        const int launched = LaunchEncode(p, desc->host_depth, slot.stream, measure ? &light : nullptr);
         if (launched < 0)
         {
             return AbandonCall(ctx, ctx->LaunchFailed(launched, "encode kernel launch"));
         }
         ctx->launches += launched;
 
-        if ((status = StageOut(ctx, slot, out, planes)) != AVIFGPU_OK || (status = CloseSlice(ctx, slot, ticket)) != AVIFGPU_OK) return AbandonCall(ctx, status);
+        if ((status = StageOut(ctx, slot, out, planes)) != AVIFGPU_OK || (measure && (status = StageLightOut(ctx, slot, acc)) != AVIFGPU_OK) ||
+            (status = CloseSlice(ctx, slot, ticket)) != AVIFGPU_OK) return AbandonCall(ctx, status);
     }
     status = FinishCall(ctx, previousRows, ticket, wait);
     if (status == AVIFGPU_OK && !wait && recordedCallRows)
@@ -2108,7 +2183,7 @@ extern "C" {
 AVIFGPU_EXPORT int avifgpu_encode_rows(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const void* host_rows,
                                        int64_t row_stride_bytes, int32_t y0, int32_t nrows, const avifgpu_planes* dst)
 {
-    return EncodeRowsHost(ctx, desc, host_rows, row_stride_bytes, y0, nrows, dst, true, nullptr);
+    return EncodeRowsHost(ctx, desc, host_rows, row_stride_bytes, y0, nrows, dst, true, nullptr, false, nullptr);
 }
 
 AVIFGPU_EXPORT int avifgpu_decode_rows(avifgpu_context* ctx, const avifgpu_decode_desc* desc, const avifgpu_planes* src,
@@ -2121,7 +2196,21 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_async(avifgpu_context* ctx, const avifgpu
                                              int64_t row_stride_bytes, int32_t y0, int32_t nrows, const avifgpu_planes* dst,
                                              int64_t* out_ticket)
 {
-    return EncodeRowsHost(ctx, desc, host_rows, row_stride_bytes, y0, nrows, dst, false, out_ticket);
+    return EncodeRowsHost(ctx, desc, host_rows, row_stride_bytes, y0, nrows, dst, false, out_ticket, false, nullptr);
+}
+
+AVIFGPU_EXPORT int avifgpu_encode_rows_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const void* host_rows,
+                                                   int64_t row_stride_bytes, int32_t y0, int32_t nrows, const avifgpu_planes* dst,
+                                                   avifgpu_light_level* host_acc)
+{
+    return EncodeRowsHost(ctx, desc, host_rows, row_stride_bytes, y0, nrows, dst, true, nullptr, true, host_acc);
+}
+
+AVIFGPU_EXPORT int avifgpu_encode_rows_async_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const void* host_rows,
+                                                         int64_t row_stride_bytes, int32_t y0, int32_t nrows, const avifgpu_planes* dst,
+                                                         avifgpu_light_level* host_acc, int64_t* out_ticket)
+{
+    return EncodeRowsHost(ctx, desc, host_rows, row_stride_bytes, y0, nrows, dst, false, out_ticket, true, host_acc);
 }
 
 AVIFGPU_EXPORT int avifgpu_decode_rows_async(avifgpu_context* ctx, const avifgpu_decode_desc* desc, const avifgpu_planes* src,
@@ -2357,13 +2446,12 @@ AVIFGPU_EXPORT int avifgpu_shard_group_synchronize(avifgpu_shard_group* group)
     return result;
 }
 
-AVIFGPU_EXPORT int avifgpu_encode_rows_sharded(avifgpu_shard_group* group, const avifgpu_encode_desc* desc, const void* host_rows,
-                                               int64_t row_stride_bytes, int32_t y0, int32_t nrows, const avifgpu_planes* dst)
+} // extern "C"
+
+// The sharded host-pointer encode; `partials` != nullptr: the light-level call, member r adding into partials[r].
+static int EncodeRowsSharded(avifgpu_shard_group* group, const avifgpu_encode_desc* desc, const void* host_rows, int64_t row_stride_bytes,
+                             int32_t y0, int32_t nrows, const avifgpu_planes* dst, avifgpu_light_level* partials)
 {
-    if (group == nullptr)
-    {
-        return AVIFGPU_ERR_BAD_PARAM;
-    }
     const int n = static_cast<int>(group->members.size());
     if (nrows < 0 || y0 < 0)
     {
@@ -2384,8 +2472,47 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_sharded(avifgpu_shard_group* group, const
             return AVIFGPU_OK;
         }
         const uint8_t* rows = host_rows ? static_cast<const uint8_t*>(host_rows) + static_cast<int64_t>(blockY0[r] - y0) * row_stride_bytes : nullptr;
-        return avifgpu_encode_rows(group->members[r], desc, rows, row_stride_bytes, blockY0[r], blockRows[r], dst);
+        return partials != nullptr ? avifgpu_encode_rows_light_level(group->members[r], desc, rows, row_stride_bytes, blockY0[r], blockRows[r], dst, partials + r)
+                                   : avifgpu_encode_rows(group->members[r], desc, rows, row_stride_bytes, blockY0[r], blockRows[r], dst);
     });
+}
+
+extern "C" {
+
+AVIFGPU_EXPORT int avifgpu_encode_rows_sharded(avifgpu_shard_group* group, const avifgpu_encode_desc* desc, const void* host_rows,
+                                               int64_t row_stride_bytes, int32_t y0, int32_t nrows, const avifgpu_planes* dst)
+{
+    if (group == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    return EncodeRowsSharded(group, desc, host_rows, row_stride_bytes, y0, nrows, dst, nullptr);
+}
+
+AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_light_level(avifgpu_shard_group* group, const avifgpu_encode_desc* desc, const void* host_rows,
+                                                           int64_t row_stride_bytes, int32_t y0, int32_t nrows, const avifgpu_planes* dst,
+                                                           avifgpu_light_level* host_acc)
+{
+    if (group == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    if (host_acc == nullptr)
+    {
+        return group->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL light-level accumulator");
+    }
+    // Each member adds into a zeroed partial of its own; *host_acc changes only once every member has succeeded.
+    std::vector<avifgpu_light_level> partials(group->members.size(), avifgpu_light_level{});
+    const int status = EncodeRowsSharded(group, desc, host_rows, row_stride_bytes, y0, nrows, dst, partials.data());
+    if (status != AVIFGPU_OK)
+    {
+        return status;
+    }
+    for (const avifgpu_light_level& part : partials)
+    {
+        AddLightLevel(*host_acc, part);
+    }
+    return AVIFGPU_OK;
 }
 
 AVIFGPU_EXPORT int avifgpu_decode_rows_sharded(avifgpu_shard_group* group, const avifgpu_decode_desc* desc, const avifgpu_planes* src,

@@ -29,6 +29,8 @@ namespace
     void* g_transformUser = nullptr;
     avifgpu_host::ShuttleTimes g_times{};
     bool g_gpuRowMatrix = true;
+    bool g_contentLightLevel = false;
+    avifgpu_host::ContentLightLevel g_lastLightLevel{};
 
     using Clock = std::chrono::steady_clock;
     double Seconds(Clock::time_point from) { return std::chrono::duration<double>(Clock::now() - from).count(); }
@@ -317,9 +319,17 @@ namespace
                                      const SaveUIOptions& saveOptions, int hostDepth, bool gray)
     {
         CallTimer callTimer;
+        g_lastLightLevel = avifgpu_host::ContentLightLevel{};
         avifgpu_context* ctx = avifgpu_host::SharedContext();
         const bool hasAlpha = alphaState != AlphaState::None;
         const int bitDepth = HeifBitDepth(saveOptions.imageBitDepth);
+        const bool measure = g_contentLightLevel && hostDepth == 32 && saveOptions.hdrTransferFunction == ColorTransferFunction::PQ;
+#if !defined(AVIFGPU_HOST_USE_PLUGIN_HEADERS)
+        if (measure && heif_image_set_content_light_level == nullptr) // compat/PluginTypes.h declares it weak
+        {
+            throw std::runtime_error("the libheif linked in has no heif_image_set_content_light_level");
+        }
+#endif
         const int channels = (gray ? 1 : 3) + (hasAlpha ? 1 : 0);
 
         avifgpu_encode_desc desc{};
@@ -418,6 +428,7 @@ namespace
         const int32 blockRows = staging.blockRows;
         g_times.rowsPerBlock = blockRows;
         RecordDataGuard guard(formatRecord);
+        avifgpu_light_level light{}; // one accumulator for every block of the image; outlives the drain below
         DrainOnExit drain{ ctx };
         formatRecord->rowBytes = static_cast<int32>(rowBytes);
 
@@ -450,7 +461,8 @@ namespace
             if (g_group != nullptr)
             {
                 // every GPU of the group takes a part of the block over its own PCIe link
-                const int status = avifgpu_encode_rows_sharded(g_group, &desc, rows, rowBytes, top, bottom - top, &planes);
+                const int status = measure ? avifgpu_encode_rows_sharded_light_level(g_group, &desc, rows, rowBytes, top, bottom - top, &planes, &light)
+                                           : avifgpu_encode_rows_sharded(g_group, &desc, rows, rowBytes, top, bottom - top, &planes);
                 if (status != AVIFGPU_OK)
                 {
                     if (status == AVIFGPU_ERR_BAD_PARAM) throw OSErrException(formatBadParameters);
@@ -462,11 +474,19 @@ namespace
             {
                 // returns once the block is queued: the host fills the other buffer while this one is on the wire;
                 // the buffer handed over in the previous iteration is free again when this call returns
-                ThrowIfFailed(ctx, avifgpu_encode_rows_async(ctx, &desc, rows, rowBytes, top, bottom - top, &planes, nullptr));
+                ThrowIfFailed(ctx, measure ? avifgpu_encode_rows_async_light_level(ctx, &desc, rows, rowBytes, top, bottom - top, &planes, &light, nullptr)
+                                           : avifgpu_encode_rows_async(ctx, &desc, rows, rowBytes, top, bottom - top, &planes, nullptr));
             }
         }
         g_times.blocks = block;
-        ThrowIfFailed(ctx, avifgpu_wait(ctx, 0)); // the planes are complete
+        ThrowIfFailed(ctx, avifgpu_wait(ctx, 0)); // the planes (and the light level) are complete
+        if (measure)
+        {
+            heif_content_light_level clli{};
+            ThrowIfFailed(ctx, avifgpu_content_light_level(&light, bitDepth, &clli.max_content_light_level, &clli.max_pic_average_light_level));
+            heif_image_set_content_light_level(image.get(), &clli);
+            g_lastLightLevel = avifgpu_host::ContentLightLevel{ true, clli.max_content_light_level, clli.max_pic_average_light_level };
+        }
         return image;
     }
 
@@ -708,6 +728,10 @@ void SetRowTransformFactory(RowTransformFactory factory, void* user)
 }
 
 void SetGpuRowMatrixEnabled(bool enabled) { g_gpuRowMatrix = enabled; }
+
+void SetContentLightLevelEnabled(bool enabled) { g_contentLightLevel = enabled; }
+
+ContentLightLevel LastContentLightLevel() { return g_lastLightLevel; }
 
 ShuttleTimes LastShuttleTimes() { return g_times; }
 

@@ -72,6 +72,22 @@ void SetRowTransformFactory(RowTransformFactory factory, void* user);
 // default where the FormatRecord holds the profile bytes; any other profile falls through to the RowTransformFactory.
 void SetGpuRowMatrixEnabled(bool enabled);
 
+// 32-bit PQ saves (CreateHeifImageRGBThirtyTwoBit / CreateHeifImageGrayThirtyTwoBit with the PQ transfer) measure the
+// image's content light level while they convert (avifgpu_encode_rows_async_light_level, or the sharded form under
+// UseDevices) and attach it to the returned image with heif_image_set_content_light_level, which libheif writes as the
+// `clli` property.  It covers the pixels encoded: after the host row transform and the GPU row matrix.  Off by default.
+void SetContentLightLevelEnabled(bool enabled);
+
+// The content light level (cd/m2) attached by the last CreateHeifImage* call; measured == false when that call attached
+// none (another save, the setting off, a cancelled or failed save).
+struct ContentLightLevel
+{
+    bool measured;
+    uint16_t maxCll;
+    uint16_t maxFall;
+};
+ContentLightLevel LastContentLightLevel();
+
 // Where the time of the last CreateHeifImage* / ReadHeifImage* call went (seconds).
 struct ShuttleTimes
 {

@@ -114,6 +114,16 @@ int heif_image_get_bits_per_pixel_range(const struct heif_image* image, enum hei
 enum heif_chroma heif_image_get_chroma_format(const struct heif_image* image);
 enum heif_colorspace heif_image_get_colorspace(const struct heif_image* image);
 void heif_image_release(const struct heif_image* image);
+struct heif_content_light_level
+{
+    uint16_t max_content_light_level;
+    uint16_t max_pic_average_light_level;
+};
+int heif_image_has_content_light_level(const struct heif_image* image);
+void heif_image_get_content_light_level(const struct heif_image* image, struct heif_content_light_level* out);
+// Weak: the stand-alone shuttle links against whatever libheif (or stand-in) it is given, and one without content light
+// level support leaves this NULL.  The shuttle then refuses a save that would measure, instead of dropping the property.
+__attribute__((weak)) void heif_image_set_content_light_level(const struct heif_image* image, const struct heif_content_light_level* in);
 }
 
 namespace detail

@@ -93,6 +93,11 @@ def library():
     sig("avifgpu_decode_rows_async", C.c_int,
         [ctx_p, C.POINTER(abi.DecodeDesc), C.POINTER(abi.Planes), C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)])
     sig("avifgpu_wait", C.c_int, [ctx_p, C.c_int64])
+    sig("avifgpu_encode_rows_light_level", C.c_int,
+        [ctx_p, C.POINTER(abi.EncodeDesc), C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(abi.Planes), C.POINTER(abi.LightLevel)])
+    sig("avifgpu_encode_rows_async_light_level", C.c_int,
+        [ctx_p, C.POINTER(abi.EncodeDesc), C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(abi.Planes), C.POINTER(abi.LightLevel),
+         C.POINTER(C.c_int64)])
     group_p = C.c_void_p
     sig("avifgpu_shard_group_create", C.c_int, [C.POINTER(C.c_int32), C.c_int32, C.POINTER(group_p)])
     sig("avifgpu_shard_group_destroy", None, [group_p])
@@ -107,6 +112,8 @@ def library():
         [group_p, C.POINTER(abi.EncodeDesc), C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(abi.Planes)])
     sig("avifgpu_decode_rows_sharded", C.c_int,
         [group_p, C.POINTER(abi.DecodeDesc), C.POINTER(abi.Planes), C.c_int32, C.c_int32, C.c_void_p, C.c_int64])
+    sig("avifgpu_encode_rows_sharded_light_level", C.c_int,
+        [group_p, C.POINTER(abi.EncodeDesc), C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(abi.Planes), C.POINTER(abi.LightLevel)])
     sig("avifgpu_encode_rows_sharded_device", C.c_int,
         [group_p, C.POINTER(abi.EncodeDesc), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(abi.Planes), C.c_int32])
     sig("avifgpu_icc_to_rec2020_linear_matrix", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int32)])
@@ -151,6 +158,7 @@ EXPORTED_SYMBOLS = [
     "avifgpu_encode_rows_sharded_device", "avifgpu_icc_to_rec2020_linear_matrix",
     "avifgpu_encode_rows_device_light_level", "avifgpu_content_light_level",
     "avifgpu_encode_batch_device_light_level", "avifgpu_encode_batch_indirect_light_level",
+    "avifgpu_encode_rows_light_level", "avifgpu_encode_rows_async_light_level", "avifgpu_encode_rows_sharded_light_level",
 ]
 
 
@@ -266,6 +274,19 @@ class Context:
                                                  y0, nrows, C.byref(p)))
         return planes
 
+    def encode_light_level(self, desc, rows, acc, y0=0, nrows=None, planes=None, pad=0):
+        """avifgpu_encode_rows_light_level: encode, plus the content light level of the rows added into `acc` (an
+        abi.LightLevel in host memory, zeroed by the caller).  Returns the planes."""
+        nrows = desc.height - y0 if nrows is None else nrows
+        assert rows.dtype == abi.host_dtype(desc.host_depth) and rows.ndim == 2
+        assert rows.size == 0 or rows.strides[1] == rows.itemsize
+        if planes is None:
+            planes = alloc_planes(abi.encode_plane_shapes(desc), abi.code_dtype(desc.image_bit_depth), pad)
+        p = abi.planes_from_arrays(planes)
+        self._check(self.lib.avifgpu_encode_rows_light_level(self.handle, C.byref(desc), rows.ctypes.data, rows.strides[0],
+                                                             y0, nrows, C.byref(p), C.byref(acc)))
+        return planes
+
     def decode(self, desc, planes, y0=0, nrows=None, out=None):
         nrows = desc.height - y0 if nrows is None else nrows
         channels = abi.decode_host_channels(desc)
@@ -283,6 +304,17 @@ class Context:
         ticket = C.c_int64()
         self._check(self.lib.avifgpu_encode_rows_async(self.handle, C.byref(desc), rows.ctypes.data, rows.strides[0], y0, nrows, C.byref(p),
                                                        C.byref(ticket)))
+        return ticket.value
+
+    def encode_async_light_level(self, desc, rows, planes, acc, y0=0, nrows=None):
+        """avifgpu_encode_rows_async_light_level: encode_async, plus the content light level of the rows added into `acc`
+        (an abi.LightLevel, zeroed by the caller), which is complete -- like the planes -- once wait() with the returned
+        ticket has returned; it must stay alive until then."""
+        nrows = desc.height - y0 if nrows is None else nrows
+        p = abi.planes_from_arrays(planes)
+        ticket = C.c_int64()
+        self._check(self.lib.avifgpu_encode_rows_async_light_level(self.handle, C.byref(desc), rows.ctypes.data, rows.strides[0], y0, nrows,
+                                                                   C.byref(p), C.byref(acc), C.byref(ticket)))
         return ticket.value
 
     def decode_async(self, desc, planes, out, y0=0, nrows=None):
@@ -432,6 +464,18 @@ class ShardGroup:
             planes = alloc_planes(abi.encode_plane_shapes(desc), abi.code_dtype(desc.image_bit_depth))
         p = abi.planes_from_arrays(planes)
         self._check(self.lib.avifgpu_encode_rows_sharded(self.handle, C.byref(desc), rows.ctypes.data, rows.strides[0], y0, nrows, C.byref(p)))
+        return planes
+
+    def encode_light_level(self, desc, rows, acc, y0=0, nrows=None, planes=None):
+        """avifgpu_encode_rows_sharded_light_level: encode, plus the content light level of the rows added into `acc`
+        (an abi.LightLevel, zeroed by the caller) once every member has succeeded.  Returns the planes."""
+        nrows = desc.height - y0 if nrows is None else nrows
+        assert rows.dtype == abi.host_dtype(desc.host_depth) and rows.ndim == 2
+        if planes is None:
+            planes = alloc_planes(abi.encode_plane_shapes(desc), abi.code_dtype(desc.image_bit_depth))
+        p = abi.planes_from_arrays(planes)
+        self._check(self.lib.avifgpu_encode_rows_sharded_light_level(self.handle, C.byref(desc), rows.ctypes.data, rows.strides[0], y0, nrows,
+                                                                     C.byref(p), C.byref(acc)))
         return planes
 
     def decode(self, desc, planes, y0=0, nrows=None, out=None):

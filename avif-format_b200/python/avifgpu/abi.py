@@ -196,7 +196,9 @@ class CurveStats(C.Structure):
 
 
 class LightLevel(C.Structure):
-    """avifgpu_light_level: the device accumulator of avifgpu_encode_rows_device_light_level (24 bytes)."""
+    """avifgpu_light_level (24 bytes): the device accumulator of avifgpu_encode_rows_device_light_level and the batch
+    light-level calls, and the host accumulator of avifgpu_encode_rows_light_level / _async_light_level /
+    _sharded_light_level, which take it by reference (ctypes.byref)."""
     _fields_ = [
         ("max_code", C.c_uint32),
         ("reserved", C.c_uint32),

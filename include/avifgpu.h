@@ -439,8 +439,9 @@ typedef struct avifgpu_light_level
  *     (avifgpu_prepare_encode); a call captured before it exists takes the generic kernel, which evaluates level(k) itself:
  *     the same result, a slower kernel.
  * Since API version 13 the batch calls have light-level forms too (avifgpu_encode_batch_device_light_level,
- * avifgpu_encode_batch_indirect_light_level, below): one accumulator per image.  Not covered: the host-pointer,
- * asynchronous and sharded calls measure nothing, and the plug-in's row shuttle does not write `clli`. */
+ * avifgpu_encode_batch_indirect_light_level, below): one accumulator per image; and so do the host-pointer, asynchronous
+ * and sharded calls (avifgpu_encode_rows_light_level and its siblings, below), into a host accumulator.  Not covered:
+ * avifgpu_encode_rows_sharded_device measures nothing. */
 AVIFGPU_EXPORT int avifgpu_encode_rows_device_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
                                                           const void* device_rows, int64_t row_stride_bytes,
                                                           int32_t y0, int32_t nrows, const avifgpu_planes* device_dst,
@@ -592,6 +593,40 @@ AVIFGPU_EXPORT int avifgpu_encode_batch_indirect_light_level(avifgpu_context* ct
                                                              int32_t* device_status, avifgpu_light_level* device_acc,
                                                              void* cuda_stream);
 
+/* ---- content light level of host-pointer encodes (additions within API version 13) -------------------------------- */
+
+/*
+ * avifgpu_encode_rows, avifgpu_encode_rows_async and avifgpu_encode_rows_sharded plus the content light level of the rows
+ * converted, added into a HOST accumulator: what an HDR save from host memory (the plug-in's row shuttle, a libheif
+ * integrator) needs for its `clli`, with no second pass over the frame on the CPU.  These three calls were added within
+ * API version 13: avifgpu_api_version() does not tell whether a library has them; look them up by symbol.
+ *   - Same call as the plain one: the contract of avifgpu_encode_rows / _async / _sharded as it stands -- rows, planes,
+ *     staging, the release of the previous asynchronous encode's rows, tickets and errors.  The planes are bit-identical
+ *     to the plain call's, padding included, with the same number of kernel launches (avifgpu_launch_count).
+ *   - The accumulator is host memory and may be pageable.  The caller zeroes it; calls add into it (max_code takes the
+ *     max, level_sum and pixels add, reserved is never written), so several calls may share one accumulator -- the row
+ *     blocks of one image, say.  For any row block *host_acc gains exactly what avifgpu_encode_rows_device_light_level
+ *     adds over the same rows: the same integers, whatever slicing, pipeline slots or group members the call used.
+ *   - When it is complete: for the synchronous and sharded calls, on an AVIFGPU_OK return.  For the asynchronous call,
+ *     once avifgpu_wait() with a ticket covering the call, or avifgpu_synchronize(), has returned AVIFGPU_OK; until then
+ *     the library may write it during any later host-pointer call on the context, on the caller's thread, and the caller
+ *     must not read, write or free it -- exactly as for the destination planes.
+ *   - Descriptions: what avifgpu_encode_rows_device_light_level accepts (host_depth 32, AVIFGPU_TRANSFER_PQ; any layout,
+ *     channel count, alpha state, chroma, down_filter, row_matrix), with dest_layout 0 as for every host-pointer call.
+ *   - Refusals: another description is AVIFGPU_ERR_UNSUPPORTED, a NULL host_acc AVIFGPU_ERR_BAD_PARAM, and every check of
+ *     the plain call applies.  A refused call launches nothing, leaves *host_acc untouched and releases nothing.
+ *   - Failures: a call that fails once it has started queueing work leaves the accumulators of this call and of earlier
+ *     unfinished calls on the context unspecified, as the plain call leaves their planes; nothing writes them after the
+ *     return.  The sharded call adds into *host_acc only when every member has succeeded: a failure leaves it untouched.
+ */
+AVIFGPU_EXPORT int avifgpu_encode_rows_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
+                                                   const void* host_rows, int64_t row_stride_bytes, int32_t y0, int32_t nrows,
+                                                   const avifgpu_planes* dst, avifgpu_light_level* host_acc);
+AVIFGPU_EXPORT int avifgpu_encode_rows_async_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
+                                                         const void* host_rows, int64_t row_stride_bytes, int32_t y0,
+                                                         int32_t nrows, const avifgpu_planes* dst, avifgpu_light_level* host_acc,
+                                                         int64_t* out_ticket);
+
 /* ---- the hot path across several GPUs of one box (SURVEY.md 8e) ------------------------------------------------ */
 
 /*
@@ -633,6 +668,13 @@ AVIFGPU_EXPORT int avifgpu_shard_row_blocks(int32_t y0, int32_t nrows, int32_t p
 AVIFGPU_EXPORT int avifgpu_encode_rows_sharded(avifgpu_shard_group* group, const avifgpu_encode_desc* desc,
                                                const void* host_rows, int64_t row_stride_bytes,
                                                int32_t y0, int32_t nrows, const avifgpu_planes* dst);
+/* avifgpu_encode_rows_sharded plus the content light level of the rows, added into the host accumulator *host_acc (see
+ * avifgpu_encode_rows_light_level): each member measures its row block into a partial of its own, and the partials are
+ * added into *host_acc once every member has succeeded.  An addition within API version 13. */
+AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_light_level(avifgpu_shard_group* group, const avifgpu_encode_desc* desc,
+                                                           const void* host_rows, int64_t row_stride_bytes,
+                                                           int32_t y0, int32_t nrows, const avifgpu_planes* dst,
+                                                           avifgpu_light_level* host_acc);
 AVIFGPU_EXPORT int avifgpu_decode_rows_sharded(avifgpu_shard_group* group, const avifgpu_decode_desc* desc,
                                                const avifgpu_planes* src, int32_t y0, int32_t nrows,
                                                void* host_rows, int64_t row_stride_bytes);

@@ -857,19 +857,25 @@ static const uint32_t* LightLevelsFor(const avifgpu_context* ctx, const avifgpu_
     return ctx->lightLevels[d.image_bit_depth == 8 ? 0 : d.image_bit_depth == 10 ? 1 : 2];
 }
 
-// The light-level calls' own checks, after the description's: float-host PQ encodes only, and an accumulator.
-static int CheckLightLevelCall(avifgpu_context* ctx, const avifgpu_encode_desc& d, const avifgpu_light_level* acc)
+} // extern "C"
+
+// The light-level calls' own checks, after the description's: float-host PQ encodes only, and an accumulator.  `caller`
+// is the context, or the shard group, whose Fail keeps the message.
+template <typename Caller>
+static int CheckLightLevelCall(Caller* caller, const avifgpu_encode_desc& d, const avifgpu_light_level* acc)
 {
     if (d.host_depth != 32 || d.transfer != AVIFGPU_TRANSFER_PQ)
     {
-        return ctx->Fail(AVIFGPU_ERR_UNSUPPORTED, "the content light level is measured on float-host PQ encodes only");
+        return caller->Fail(AVIFGPU_ERR_UNSUPPORTED, "the content light level is measured on float-host PQ encodes only");
     }
     if (acc == nullptr)
     {
-        return ctx->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL light-level accumulator");
+        return caller->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL light-level accumulator");
     }
     return AVIFGPU_OK;
 }
+
+extern "C" {
 
 // The device-pointer encode; `acc` != nullptr: the light-level call, whose description the caller has checked.
 static int EncodeRowsDevice(avifgpu_context* ctx, const avifgpu_encode_desc* desc, const void* device_rows, int64_t row_stride_bytes, int32_t y0,
@@ -2246,6 +2252,13 @@ struct avifgpu_shard_group
     std::vector<uint8_t> peer; // peer[from * n + to]
     std::string lastError;
 
+    // The sharded device light-level call's state, allocated at its first call and freed with the group.  lightPartial[r]
+    // (member r's memory) is member r's statistic of its block, lightCopied[r] recorded on its stream once the partial is
+    // copied into the owner's gather array.  Per owner o: lightGather[o] (o's memory) has one slot per member, and
+    // lightMerged[o] is recorded on o's stream after the merge that reads it.  All nullptr until allocated.
+    std::vector<avifgpu_light_level*> lightPartial, lightGather;
+    std::vector<cudaEvent_t> lightCopied, lightMerged;
+
     int Fail(int status, const std::string& message)
     {
         lastError = message;
@@ -2391,6 +2404,20 @@ AVIFGPU_EXPORT void avifgpu_shard_group_destroy(avifgpu_shard_group* group)
     if (group == nullptr)
     {
         return;
+    }
+    // Every member drains before anything is freed: a copy into owner o's gather array runs on the member's stream.
+    for (size_t r = 0; r < group->lightPartial.size(); ++r)
+    {
+        DeviceGuard guard(group->devices[r]);
+        cudaDeviceSynchronize();
+    }
+    for (size_t r = 0; r < group->lightPartial.size(); ++r)
+    {
+        DeviceGuard guard(group->devices[r]);
+        if (group->lightPartial[r]) cudaFree(group->lightPartial[r]);
+        if (group->lightGather[r]) cudaFree(group->lightGather[r]);
+        if (group->lightCopied[r]) cudaEventDestroy(group->lightCopied[r]);
+        if (group->lightMerged[r]) cudaEventDestroy(group->lightMerged[r]);
     }
     for (avifgpu_context* ctx : group->members)
     {
@@ -2544,14 +2571,121 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_sharded(avifgpu_shard_group* group, const
     });
 }
 
-AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_device(avifgpu_shard_group* group, const avifgpu_encode_desc* desc,
-                                                      const void* const* device_rows, const int64_t* row_stride_bytes,
-                                                      const avifgpu_planes* owner_planes, int32_t owner)
+} // extern "C"
+
+// Allocates, on first need, the group's light-level state for calls with this owner: every member's partial and copy
+// event, and the owner's gather array and merge event.
+static int PrepareShardLight(avifgpu_shard_group* group, int owner)
 {
-    if (group == nullptr)
+    const int n = static_cast<int>(group->members.size());
+    if (group->lightPartial.empty())
     {
-        return AVIFGPU_ERR_BAD_PARAM;
+        group->lightPartial.assign(n, nullptr);
+        group->lightGather.assign(n, nullptr);
+        group->lightCopied.assign(n, nullptr);
+        group->lightMerged.assign(n, nullptr);
     }
+    for (int r = 0; r < n; ++r)
+    {
+        avifgpu_context* ctx = group->members[r];
+        DeviceGuard guard(ctx->device);
+        int status = AVIFGPU_OK;
+        void* memory = nullptr;
+        cudaEvent_t event = nullptr;
+        if (group->lightPartial[r] == nullptr && (status = ctx->Cuda(cudaMalloc(&memory, sizeof(avifgpu_light_level)), "cudaMalloc")) == AVIFGPU_OK)
+        {
+            group->lightPartial[r] = static_cast<avifgpu_light_level*>(memory);
+        }
+        if (status == AVIFGPU_OK && group->lightCopied[r] == nullptr &&
+            (status = ctx->Cuda(cudaEventCreateWithFlags(&event, cudaEventDisableTiming), "cudaEventCreate")) == AVIFGPU_OK)
+        {
+            group->lightCopied[r] = event;
+        }
+        if (status == AVIFGPU_OK && r == owner && group->lightGather[r] == nullptr &&
+            (status = ctx->Cuda(cudaMalloc(&memory, n * sizeof(avifgpu_light_level)), "cudaMalloc")) == AVIFGPU_OK)
+        {
+            group->lightGather[r] = static_cast<avifgpu_light_level*>(memory);
+        }
+        if (status == AVIFGPU_OK && r == owner && group->lightMerged[r] == nullptr &&
+            (status = ctx->Cuda(cudaEventCreateWithFlags(&event, cudaEventDisableTiming), "cudaEventCreate")) == AVIFGPU_OK)
+        {
+            group->lightMerged[r] = event;
+        }
+        if (status != AVIFGPU_OK)
+        {
+            return group->Fail(status, "member " + std::to_string(r) + ": " + ctx->lastError);
+        }
+    }
+    return AVIFGPU_OK;
+}
+
+// Member r's part of the light-level call, on its stream: clear its partial, encode its block through the device
+// light-level route into the partial, copy the partial into slot r of the owner's gather array and record lightCopied[r].
+static int MeasureShardBlock(avifgpu_shard_group* group, int r, int owner, const avifgpu_encode_desc* desc, const void* rows,
+                             int64_t row_stride_bytes, int32_t y0, int32_t nrows, const avifgpu_planes* owner_planes)
+{
+    avifgpu_context* ctx = group->members[r];
+    DeviceGuard guard(ctx->device);
+    const cudaStream_t stream = ctx->slots[0].stream;
+    avifgpu_light_level* partial = group->lightPartial[r];
+    int status = ctx->Cuda(cudaMemsetAsync(partial, 0, sizeof(avifgpu_light_level), stream), "cudaMemsetAsync");
+    if (status == AVIFGPU_OK)
+    {
+        status = EncodeRowsDevice(ctx, desc, rows, row_stride_bytes, y0, nrows, owner_planes, partial, stream);
+    }
+    // The owner's previous merge reads slot r, and nothing orders it before this copy when calls follow each other
+    // without a synchronize: wait for it, or this call could overwrite the previous call's partial before it is merged.
+    if (status == AVIFGPU_OK)
+    {
+        status = ctx->Cuda(cudaStreamWaitEvent(stream, group->lightMerged[owner], 0), "cudaStreamWaitEvent");
+    }
+    if (status == AVIFGPU_OK)
+    {
+        status = ctx->Cuda(cudaMemcpyPeerAsync(group->lightGather[owner] + r, group->devices[owner], partial, group->devices[r],
+                                               sizeof(avifgpu_light_level), stream),
+                           "cudaMemcpyPeerAsync");
+    }
+    return status != AVIFGPU_OK ? status : ctx->Cuda(cudaEventRecord(group->lightCopied[r], stream), "cudaEventRecord");
+}
+
+// The light-level call's last step, once every member's part is enqueued: the owner's stream waits for the copies of the
+// members in `measured` (bit r for member r), one warp merges their slots of the gather array into *acc, and
+// lightMerged[owner] is recorded for the next call's copies.
+static int MergeShardLight(avifgpu_shard_group* group, int owner, uint64_t measured, avifgpu_light_level* acc)
+{
+    avifgpu_context* ctx = group->members[owner];
+    DeviceGuard guard(ctx->device);
+    const cudaStream_t stream = ctx->slots[0].stream;
+    int status = AVIFGPU_OK;
+    for (int r = 0; r < static_cast<int>(group->members.size()) && status == AVIFGPU_OK; ++r)
+    {
+        if ((measured >> r) & 1u)
+        {
+            status = ctx->Cuda(cudaStreamWaitEvent(stream, group->lightCopied[r], 0), "cudaStreamWaitEvent");
+        }
+    }
+    if (status == AVIFGPU_OK)
+    {
+        const int launched = LaunchMergeLightPartials(group->lightGather[owner], measured, acc, stream);
+        if (launched < 0)
+        {
+            status = ctx->LaunchFailed(launched, "light-level merge launch");
+        }
+        else
+        {
+            ctx->launches += launched;
+            status = ctx->Cuda(cudaEventRecord(group->lightMerged[owner], stream), "cudaEventRecord");
+        }
+    }
+    return status != AVIFGPU_OK ? group->Fail(status, "member " + std::to_string(owner) + ": " + ctx->lastError) : AVIFGPU_OK;
+}
+
+// The sharded device-pointer encode; `acc` != nullptr: the light-level call (avifgpu.h), whose members measure their
+// blocks into partials of their own, merged into *acc on the owner's stream once every member's launch has succeeded.
+static int EncodeRowsShardedDevice(avifgpu_shard_group* group, const avifgpu_encode_desc* desc, const void* const* device_rows,
+                                   const int64_t* row_stride_bytes, const avifgpu_planes* owner_planes, int32_t owner,
+                                   avifgpu_light_level* acc)
+{
     const int n = static_cast<int>(group->members.size());
     if (desc == nullptr || device_rows == nullptr || row_stride_bytes == nullptr || owner_planes == nullptr || owner < 0 || owner >= n)
     {
@@ -2563,6 +2697,20 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_device(avifgpu_shard_group* group
     {
         return group->Fail(AVIFGPU_ERR_UNSUPPORTED, "the sharded calls write planar, low-bit planes only (libheif's layout)");
     }
+    if (acc != nullptr)
+    {
+        // The plain call lets every member validate the description; this one refuses before any member enqueues.
+        std::string error;
+        int status = ValidateEncodeDesc(desc, &error);
+        if (status != AVIFGPU_OK)
+        {
+            return group->Fail(status, error);
+        }
+        if ((status = CheckLightLevelCall(group, *desc, acc)) != AVIFGPU_OK)
+        {
+            return status;
+        }
+    }
     std::vector<int32_t> blockY0(n), blockRows(n);
     RowBlocks(0, desc->height, n, blockY0.data(), blockRows.data());
     for (int r = 0; r < n; ++r)
@@ -2572,7 +2720,13 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_device(avifgpu_shard_group* group
             return group->Fail(AVIFGPU_ERR_UNSUPPORTED, "member " + std::to_string(r) + " has no peer access to the owner's memory");
         }
     }
+    int status;
+    if (acc != nullptr && (status = PrepareShardLight(group, owner)) != AVIFGPU_OK)
+    {
+        return status;
+    }
     // Launches are asynchronous: a plain loop enqueues all of them in microseconds, each on its member's own stream.
+    uint64_t measured = 0;
     for (int r = 0; r < n; ++r)
     {
         if (blockRows[r] == 0)
@@ -2580,14 +2734,45 @@ AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_device(avifgpu_shard_group* group
             continue;
         }
         avifgpu_context* ctx = group->members[r];
-        const int status = avifgpu_encode_rows_device(ctx, desc, device_rows[r], row_stride_bytes[r], blockY0[r], blockRows[r], owner_planes,
-                                                      ctx->slots[0].stream);
+        status = acc == nullptr ? avifgpu_encode_rows_device(ctx, desc, device_rows[r], row_stride_bytes[r], blockY0[r], blockRows[r], owner_planes,
+                                                             ctx->slots[0].stream)
+                                : MeasureShardBlock(group, r, owner, desc, device_rows[r], row_stride_bytes[r], blockY0[r], blockRows[r], owner_planes);
         if (status != AVIFGPU_OK)
         {
             return group->Fail(status, "member " + std::to_string(r) + ": " + ctx->lastError);
         }
+        measured |= uint64_t{ 1 } << r;
     }
-    return AVIFGPU_OK;
+    return acc == nullptr ? AVIFGPU_OK : MergeShardLight(group, owner, measured, acc);
+}
+
+extern "C" {
+
+AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_device(avifgpu_shard_group* group, const avifgpu_encode_desc* desc,
+                                                      const void* const* device_rows, const int64_t* row_stride_bytes,
+                                                      const avifgpu_planes* owner_planes, int32_t owner)
+{
+    if (group == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    return EncodeRowsShardedDevice(group, desc, device_rows, row_stride_bytes, owner_planes, owner, nullptr);
+}
+
+AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_device_light_level(avifgpu_shard_group* group, const avifgpu_encode_desc* desc,
+                                                                  const void* const* device_rows, const int64_t* row_stride_bytes,
+                                                                  const avifgpu_planes* owner_planes, int32_t owner,
+                                                                  avifgpu_light_level* device_acc)
+{
+    if (group == nullptr)
+    {
+        return AVIFGPU_ERR_BAD_PARAM;
+    }
+    if (device_acc == nullptr)
+    {
+        return group->Fail(AVIFGPU_ERR_BAD_PARAM, "NULL light-level accumulator");
+    }
+    return EncodeRowsShardedDevice(group, desc, device_rows, row_stride_bytes, owner_planes, owner, device_acc);
 }
 
 // ---- preparation ------------------------------------------------------------------------------------------------

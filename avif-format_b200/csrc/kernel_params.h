@@ -693,6 +693,9 @@ int LaunchEncodeGeneric(const EncodeParams& params, int hostDepth, void* stream,
 int LaunchDecodeGeneric(const DecodeParams& params, void* stream);
 int LaunchTransfer(int function, float param, const float* in, float* out, size_t count, void* stream);
 int LaunchHlgOotf(int inverse, const float luma[3], float displayGamma, float peak, const float* in, float* out, size_t pixels, void* stream);
+// One warp adding the partials parts[r] whose bit r is set in `members` into *acc (the sharded device light-level call's
+// merge, kernels_generic.cu).  Returns 1, or a negative status.
+int LaunchMergeLightPartials(const avifgpu_light_level* parts, uint64_t members, avifgpu_light_level* acc, void* stream);
 
 // The tuned launchers (kernels_fast*.cu): each fills its kernel's parameters for the interior `inner` of the block `p`
 // that the route gave its family, enqueues the kernel and returns the launch's status.

@@ -119,6 +119,38 @@ __global__ void __launch_bounds__(kThreads) EncodePlanarLightKernel(const Encode
     EncodePlanarSite<float, kThreads, 1>(p, t, blockIdx.x, &tally, light.levels);
     FlushLightTally(tally, LaunchPixelsForFirstWarp(static_cast<uint64_t>(p.width) * p.rowCount), light.acc);
 }
+
+// The sharded device light-level call's merge on the owner: one warp adds the gathered partials whose bit is set in
+// `members` (at most 64, two per lane) into the caller's accumulator -- max of max_code, sums of level_sum and pixels.
+// Atomics, as the light-level kernels flush: other work may add into the same accumulator concurrently.
+__global__ void __launch_bounds__(32) MergeLightPartialsKernel(const avifgpu_light_level* __restrict__ parts, uint64_t members,
+                                                               avifgpu_light_level* acc)
+{
+    uint32_t maxCode = 0;
+    unsigned long long levelSum = 0, pixels = 0;
+    for (int r = threadIdx.x; r < 64; r += 32)
+    {
+        if ((members >> r) & 1u)
+        {
+            maxCode = max(maxCode, parts[r].max_code);
+            levelSum += parts[r].level_sum;
+            pixels += parts[r].pixels;
+        }
+    }
+    maxCode = __reduce_max_sync(0xffffffffu, maxCode);
+#pragma unroll
+    for (int offset = 16; offset > 0; offset >>= 1)
+    {
+        levelSum += __shfl_down_sync(0xffffffffu, levelSum, offset);
+        pixels += __shfl_down_sync(0xffffffffu, pixels, offset);
+    }
+    if (threadIdx.x == 0)
+    {
+        atomicMax(&acc->max_code, maxCode);
+        atomicAdd(reinterpret_cast<unsigned long long*>(&acc->level_sum), levelSum);
+        atomicAdd(reinterpret_cast<unsigned long long*>(&acc->pixels), pixels);
+    }
+}
 // ---- decode ----------------------------------------------------------------------------------------------
 
 // PlaneT uint8_t pairs with HostT uint8_t; PlaneT uint16_t with HostT uint16_t or float.
@@ -317,6 +349,13 @@ int LaunchHlgOotf(int inverse, const float luma[3], float displayGamma, float pe
     }
     HlgOotfKernel<<<static_cast<unsigned>(blocks), kThreads, 0, static_cast<cudaStream_t>(streamHandle)>>>(inverse, luma[0], luma[1], luma[2], displayGamma, peak, in,
                                                                                                       out, pixels);
+    const cudaError_t launchError = cudaGetLastError();
+    return launchError == cudaSuccess ? 1 : ReportLaunchFailure(static_cast<int>(launchError));
+}
+
+int LaunchMergeLightPartials(const avifgpu_light_level* parts, uint64_t members, avifgpu_light_level* acc, void* streamHandle)
+{
+    MergeLightPartialsKernel<<<1, 32, 0, static_cast<cudaStream_t>(streamHandle)>>>(parts, members, acc);
     const cudaError_t launchError = cudaGetLastError();
     return launchError == cudaSuccess ? 1 : ReportLaunchFailure(static_cast<int>(launchError));
 }

@@ -116,6 +116,8 @@ def library():
         [group_p, C.POINTER(abi.EncodeDesc), C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(abi.Planes), C.POINTER(abi.LightLevel)])
     sig("avifgpu_encode_rows_sharded_device", C.c_int,
         [group_p, C.POINTER(abi.EncodeDesc), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(abi.Planes), C.c_int32])
+    sig("avifgpu_encode_rows_sharded_device_light_level", C.c_int,
+        [group_p, C.POINTER(abi.EncodeDesc), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(abi.Planes), C.c_int32, C.c_void_p])
     sig("avifgpu_icc_to_rec2020_linear_matrix", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int32)])
     _lib = lib
     return lib
@@ -159,6 +161,7 @@ EXPORTED_SYMBOLS = [
     "avifgpu_encode_rows_device_light_level", "avifgpu_content_light_level",
     "avifgpu_encode_batch_device_light_level", "avifgpu_encode_batch_indirect_light_level",
     "avifgpu_encode_rows_light_level", "avifgpu_encode_rows_async_light_level", "avifgpu_encode_rows_sharded_light_level",
+    "avifgpu_encode_rows_sharded_device_light_level",
 ]
 
 
@@ -491,6 +494,16 @@ class ShardGroup:
         pointers = (C.c_void_p * n)(*[int(v) if v else None for v in row_pointers])
         strides = (C.c_int64 * n)(*[int(v) for v in row_strides])
         self._check(self.lib.avifgpu_encode_rows_sharded_device(self.handle, C.byref(desc), pointers, strides, C.byref(owner_planes), owner))
+
+    def encode_device_light_level(self, desc, row_pointers, row_strides, owner_planes, acc_ptr, owner=0):
+        """avifgpu_encode_rows_sharded_device_light_level: encode_device, plus the content light level of the whole image
+        added into the device accumulator at `acc_ptr` (24 bytes in the owner's memory, zeroed by the caller; see
+        abi.LightLevel), complete after synchronize()."""
+        n = self.size()
+        pointers = (C.c_void_p * n)(*[int(v) if v else None for v in row_pointers])
+        strides = (C.c_int64 * n)(*[int(v) for v in row_strides])
+        self._check(self.lib.avifgpu_encode_rows_sharded_device_light_level(self.handle, C.byref(desc), pointers, strides, C.byref(owner_planes),
+                                                                            owner, acc_ptr))
 
 
 _pinned_owners = {}

@@ -439,9 +439,9 @@ typedef struct avifgpu_light_level
  *     (avifgpu_prepare_encode); a call captured before it exists takes the generic kernel, which evaluates level(k) itself:
  *     the same result, a slower kernel.
  * Since API version 13 the batch calls have light-level forms too (avifgpu_encode_batch_device_light_level,
- * avifgpu_encode_batch_indirect_light_level, below): one accumulator per image; and so do the host-pointer, asynchronous
- * and sharded calls (avifgpu_encode_rows_light_level and its siblings, below), into a host accumulator.  Not covered:
- * avifgpu_encode_rows_sharded_device measures nothing. */
+ * avifgpu_encode_batch_indirect_light_level, below): one accumulator per image; so do the host-pointer, asynchronous
+ * and sharded calls (avifgpu_encode_rows_light_level and its siblings, below), into a host accumulator; and so does the
+ * sharded device-pointer call (avifgpu_encode_rows_sharded_device_light_level, below), into the owner's memory. */
 AVIFGPU_EXPORT int avifgpu_encode_rows_device_light_level(avifgpu_context* ctx, const avifgpu_encode_desc* desc,
                                                           const void* device_rows, int64_t row_stride_bytes,
                                                           int32_t y0, int32_t nrows, const avifgpu_planes* device_dst,
@@ -688,6 +688,36 @@ AVIFGPU_EXPORT int avifgpu_decode_rows_sharded(avifgpu_shard_group* group, const
 AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_device(avifgpu_shard_group* group, const avifgpu_encode_desc* desc,
                                                       const void* const* device_rows, const int64_t* row_stride_bytes,
                                                       const avifgpu_planes* owner_planes, int32_t owner);
+/*
+ * avifgpu_encode_rows_sharded_device plus the content light level of the whole image, added into *device_acc in the
+ * owner's memory: a device-resident HDR frame spread over several GPUs gets its `clli` with no second pass.  An addition
+ * within API version 13: look it up by symbol.
+ *   - Same call as the plain one: arguments, row blocks, the peer-access requirement and enqueue-and-return as in
+ *     avifgpu_encode_rows_sharded_device.  The planes are bit-identical to the plain call's, padding included.
+ *   - Launches: every member's avifgpu_launch_count rises by what the plain call adds, and the owner's by one more, for
+ *     the merge described below.
+ *   - The accumulator is device memory of the owner, zeroed by the caller; calls add into it (max_code takes the max,
+ *     level_sum and pixels add, reserved is never written).  It gains exactly what one
+ *     avifgpu_encode_rows_device_light_level call over the whole image (y0 = 0, nrows = height) adds on one device, whatever
+ *     the number of members and wherever the block boundaries fall.
+ *   - How: each member with a non-empty block measures it on its own stream into a partial in its own memory and copies
+ *     the partial into the owner's memory (no atomics across devices); the owner's stream then waits for every member and
+ *     one single-warp kernel adds the partials into *device_acc.
+ *   - When it is complete: after avifgpu_shard_group_synchronize(), like the planes.  Since the owner's stream waits for
+ *     every member, work ordered after it -- avifgpu_synchronize() of the owner's context included -- sees both the
+ *     accumulator and the planes complete.
+ *   - Descriptions: what avifgpu_encode_rows_device_light_level accepts (host_depth 32, AVIFGPU_TRANSFER_PQ; any layout,
+ *     channel count, alpha state, chroma, down_filter, row_matrix), with dest_layout 0 as for every sharded call.
+ *   - Refusals, before anything is enqueued on any member and leaving *device_acc untouched: another description is
+ *     AVIFGPU_ERR_UNSUPPORTED, a NULL device_acc AVIFGPU_ERR_BAD_PARAM, and every check of the plain call applies (an
+ *     owner outside the group, a member with no peer access to the owner, ...).
+ *   - Failures: the merge is enqueued only once every member's launch has succeeded, so a call that fails while its
+ *     members are being enqueued leaves *device_acc untouched, and the planes as the plain call leaves them.
+ */
+AVIFGPU_EXPORT int avifgpu_encode_rows_sharded_device_light_level(avifgpu_shard_group* group, const avifgpu_encode_desc* desc,
+                                                                  const void* const* device_rows, const int64_t* row_stride_bytes,
+                                                                  const avifgpu_planes* owner_planes, int32_t owner,
+                                                                  avifgpu_light_level* device_acc);
 
 /* ---- preparation (optional) --------------------------------------------------------------------------- */
 

@@ -21,10 +21,11 @@
 //                                 entry are staged once per CTA for the whole batch, not once per CTA per image;
 //   DecodeBatchKernel             the decode windows, with DecodeChunkPixel (generic_units.cuh).
 //   EncodeLightF32BatchKernel     the light-level float encode interiors (RGB(A)32f -> planar YCbCr through the PQ compact
-//                                 step table, the content light level of every image on the side); a warp takes one
-//                                 128-pixel tile of a row (4:2:0 row pair) at a time, and the libm tables and the step
-//                                 table are staged once per CTA for the whole batch;
-//   EncodeLightPlanarBatchKernel  the light-level encode windows, with EncodePlanarSite's light-level form.
+//                                 step table, the content light level of every image on the side), with the single-image
+//                                 RGBA kernel's lane code (kernels_fast_common.cuh); a warp takes one 128-pixel tile of a
+//                                 row (4:2:0 row pair) at a time, and the libm tables and the step table are staged once
+//                                 per CTA for the whole batch;
+//   EncodeLightPlanarBatchKernel  the light-level encode windows: EncodePlanarBatchKernel's body with the tally.
 //
 // Each is a template on where its records come from:
 //   ChunkSource      a host-described chunk (PlanEncodeBatch / PlanDecodeBatch): the records and their unit total travel
@@ -403,8 +404,11 @@ __global__ void __launch_bounds__(kRgbThreads) EncodeRgbIntBatchKernel(const __g
     }
 }
 
-template <typename Source, typename HostT>
-__global__ void __launch_bounds__(kBatchEdgeThreads) EncodePlanarBatchKernel(const __grid_constant__ Source s)
+// EncodePlanarBatchKernel's body and, LIGHT = 1 (float hosts), EncodeLightPlanarBatchKernel's: the generic kernel's own
+// per-site code, with its tally into the image's statistic, the level read from the context's table (`light`) or
+// evaluated in place when there is none.
+template <typename Source, typename HostT, int LIGHT = 0>
+__device__ __forceinline__ void EncodePlanarBatchBody(const Source& s, const LightSink& light = {})
 {
     const typename Source::Walk walk(s);
     if (walk.Idle(blockIdx.x))
@@ -416,10 +420,19 @@ __global__ void __launch_bounds__(kBatchEdgeThreads) EncodePlanarBatchKernel(con
     const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
     __syncthreads();
     int record = 0;
+    ImageTally image;
     for (long long unit = blockIdx.x; unit < walk.Units(); unit += gridDim.x)
     {
         record = walk.Find(count, record, unit);
         const BatchRecord& r = walk.Record(record);
+        if constexpr (LIGHT != 0)
+        {
+            image.Switch(walk.ImageOf(record), light.acc);
+            if (unit == r.firstUnit && threadIdx.x < 32) // the CTA's first warp counts the record's pixels
+            {
+                image.pixels += static_cast<uint64_t>(r.width) * static_cast<uint64_t>(r.rowCount);
+            }
+        }
         EncodeParams p = s.shared;
         p.rows = r.rows;
         p.rowStride = r.rowStride;
@@ -430,16 +443,27 @@ __global__ void __launch_bounds__(kBatchEdgeThreads) EncodePlanarBatchKernel(con
         }
         p.width = r.width;
         p.rowCount = r.rowCount;
-        EncodePlanarSite<HostT, kBatchEdgeThreads>(p, t, static_cast<unsigned>(unit - r.firstUnit));
+        EncodePlanarSite<HostT, kBatchEdgeThreads, LIGHT>(p, t, static_cast<unsigned>(unit - r.firstUnit), &image.tally, light.levels);
+    }
+    if constexpr (LIGHT != 0)
+    {
+        image.Flush(light.acc);
     }
 }
 
-// The single-image RGBA kernel's per-lane work (kernels_fast_rgba.cu has the commentary) on one unit of kLightBatchUnitPixels
-// pixels of a row, or of a 4:2:0 row pair, a lane on 4 pixels of each row, with the unit's record's pointers and no
-// software pipelining: the next unit may belong to another image.  RGB hosts (CHANNELS 3) take the flat kernel's samples
-// as they are, RGBA hosts the RGBA kernel's clamp / premultiplication and alpha plane.  An interior is 4-pixel aligned, so
-// a lane is wholly inside its row or wholly past its end; a lane past it converts zeros and stores nothing.  Each pixel's
-// max(R', G', B') code goes into the warp's tally with its level from the context's table.
+template <typename Source, typename HostT>
+__global__ void __launch_bounds__(kBatchEdgeThreads) EncodePlanarBatchKernel(const __grid_constant__ Source s)
+{
+    EncodePlanarBatchBody<Source, HostT>(s);
+}
+
+// The single-image RGBA kernel's lane work (kernels_fast_common.cuh: PrepareRgbaSamples, LookUpLaneCodes,
+// ResolveLaneCodes) on one unit of kLightBatchUnitPixels pixels of a row, or of a 4:2:0 row pair, a lane on 4 pixels of each
+// row, with the unit's record's pointers and no software pipelining: the next unit may belong to another image.  RGB hosts
+// (CHANNELS 3) take the flat kernel's samples as they are, RGBA hosts the RGBA kernel's clamp / premultiplication and alpha
+// plane.  An interior is 4-pixel aligned, so a lane is wholly inside its row or wholly past its end; a lane past it converts
+// zeros and stores nothing.  Each pixel's max(R', G', B') code goes into the warp's tally with its level from the context's
+// table.
 template <typename Source, int CHANNELS, int XS, int YS, int DEST>
 __global__ void __launch_bounds__(kLightBatchWarps * 32, 1) EncodeLightF32BatchKernel(const __grid_constant__ Source s)
 {
@@ -459,7 +483,6 @@ __global__ void __launch_bounds__(kLightBatchWarps * 32, 1) EncodeLightF32BatchK
     uint64_t* tableBarrier = reinterpret_cast<uint64_t*>(sharedBytes + kSharedLibm);
     uint32_t* stageAll = reinterpret_cast<uint32_t*>(sharedBytes + kSharedLibm + kRgbaTableBarrierBytes);
     uint32_t* compactEntries = reinterpret_cast<uint32_t*>(sharedBytes + LightBatchFixedBytes());
-    const uint32_t* firstBits = compactEntries + ((d.table.flatCount + 3) & ~3);
     if (threadIdx.x == 0)
     {
         staging::BeginTableImageCopy(d.table, compactEntries, tableBarrier);
@@ -471,14 +494,7 @@ __global__ void __launch_bounds__(kLightBatchWarps * 32, 1) EncodeLightF32BatchK
     const int lane = threadIdx.x & 31;
     const int warpInBlock = threadIdx.x >> 5;
     uint32_t* myStage = stageAll + warpInBlock * (32 * kRgbaLaneStrideWords) + lane * kRgbaLaneStrideWords;
-    const uint32_t flatShift = d.table.flatShift;
-    const int32_t negativeLow = -static_cast<int32_t>(d.table.flatLow);
-    const int32_t span = static_cast<int32_t>(d.table.flatHigh - d.table.flatLow);
-    const uint32_t bandStrideLog2 = d.table.bandStrideLog2;
-    const uint32_t* __restrict__ bandBits = d.table.bandBits;
-    const uint32_t compactTopShift = 32u - flatShift;
-    const uint32_t compactCodeMask = d.table.compactCodeMask;
-    const uint32_t compactMagic = d.table.compactMagic;
+    const CompactTable compact = CompactTableOf(d.table, compactEntries);
     const long long warpCount = static_cast<long long>(gridDim.x) * kLightBatchWarps;
     int record = 0;
     ImageTally light;
@@ -500,7 +516,7 @@ __global__ void __launch_bounds__(kLightBatchWarps * 32, 1) EncodeLightF32BatchK
         const int64_t y = static_cast<int64_t>(unitRow) * kRows;
         const uint8_t* source = static_cast<const uint8_t*>(r.rows) + y * r.rowStride + static_cast<int64_t>(x) * CHANNELS * 4;
 
-        // ---- 128-bit row loads; RGBA: alpha, clamp / premultiplication; then the colour samples the curve sees ----------
+        // 128-bit row loads; RGBA: alpha, clamp / premultiplication
         uint32_t colourBits[kValues];
         uint32_t alphaCode[kPixels];
         if constexpr (CHANNELS == 3)
@@ -523,106 +539,18 @@ __global__ void __launch_bounds__(kLightBatchWarps * 32, 1) EncodeLightF32BatchK
             {
                 raw[k] = laneActive ? __ldg(reinterpret_cast<const uint4*>(source + (k / 4) * r.rowStride + 16 * (k % 4))) : make_uint4(0u, 0u, 0u, 0u);
             }
-#pragma unroll
-            for (int k = 0; k < kPixels; ++k)
-            {
-                const float alpha = ClampF(__uint_as_float(raw[k].w), 0.0f, 1.0f);
-                float colour[3] = { __uint_as_float(raw[k].x), __uint_as_float(raw[k].y), __uint_as_float(raw[k].z) };
-                if (d.premultiply && alpha < 1.0f)
-                {
-#pragma unroll
-                    for (int c = 0; c < 3; ++c)
-                    {
-                        colour[c] = (alpha == 0) ? 0.0f : PremultiplyColor(ClampF(colour[c], 0.0f, 1.0f), alpha, 1.0f);
-                    }
-                }
-                alphaCode[k] = FloatToCode(alpha, d.maxCodeFloat);
-#pragma unroll
-                for (int c = 0; c < 3; ++c)
-                {
-                    colourBits[3 * k + c] = __float_as_uint(colour[c]);
-                }
-            }
+            PrepareRgbaSamples(d, raw, alphaCode, colourBits);
         }
-#pragma unroll
-        for (int q = 0; q < kValues / 4; ++q)
-        {
-            *reinterpret_cast<uint4*>(myStage + 4 * q) = make_uint4(colourBits[4 * q], colourBits[4 * q + 1], colourBits[4 * q + 2], colourBits[4 * q + 3]);
-        }
-
-        // ---- float -> code through the compact step table ----------------------------------------------------------
         float codeF[kValuesPerLane] = {}; // one row (YS 0): the second row's codes stay 0 and are not stored
-        uint32_t bandMask = 0;
-        int32_t largest = 0; // max over the samples as signed integers: > 0x7f7fffff <=> a +inf / NaN is among them
-#pragma unroll
-        for (int j = 0; j < kValues; ++j)
-        {
-            bool inBand;
-            uint32_t entry;
-            codeF[j] = LookupCurveCompact<0>(colourBits[j], compactEntries, flatShift, negativeLow, span, compactTopShift, compactCodeMask, compactMagic, inBand, entry);
-            asm("{ .reg .pred q; setp.ne.u32 q, %1, 0; @q or.b32 %0, %0, %2; }" : "+r"(bandMask) : "r"(static_cast<uint32_t>(inBand)), "r"(1u << j));
-            largest = max(largest, static_cast<int32_t>(colourBits[j]));
-        }
-
-        // ---- in-band samples: which step, how far above its first_k, one bit of the band bitmap ------------------------
-        uint32_t lowerMask = 0;
-        {
-            uint32_t pending = bandMask;
-            while (pending != 0)
-            {
-                const int j = __ffs(static_cast<int>(pending)) - 1;
-                pending &= pending - 1;
-                const uint32_t bits = myStage[j];
-                const int32_t bucket = __viaddmin_s32_relu(static_cast<int32_t>(bits) >> flatShift, negativeLow, span);
-                const uint32_t entry = compactEntries[bucket];
-                const uint32_t k = ((entry & compactCodeMask) >> kCompactLenBits) + ((entry >> compactTopShift) != 0 ? 1u : 0u);
-                const uint32_t distance = bits - firstBits[k];
-                if (k != 0 && distance < (1u << bandStrideLog2)) // else flagged by the superset test only
-                {
-                    const uint32_t bitIndex = (k << bandStrideLog2) + distance;
-                    const uint32_t word = __ldg(bandBits + (bitIndex >> 5));
-                    lowerMask |= (((word >> (bitIndex & 31u)) & 1u) ^ 1u) << j;
-                }
-            }
-        }
-        // ---- +inf / NaN: the exact evaluation, lane by lane -------------------------------------------------------------
-        if (__any_sync(0xffffffffu, largest > 0x7f7fffff))
-        {
-            for (int j = 0; j < kValues; ++j)
-            {
-                const uint32_t bits = myStage[j];
-                if (static_cast<int32_t>(bits) > 0x7f7fffff)
-                {
-                    const float exact = CodeToFloat(ExactCurveCode<kCurveLinearToPQ>(__uint_as_float(bits), d.pqMultiplier, d.maxCodeFloat, t));
-#pragma unroll
-                    for (int slot = 0; slot < kValues; ++slot)
-                    {
-                        if (slot == j)
-                        {
-                            codeF[slot] = exact;
-                        }
-                    }
-                }
-            }
-        }
-#pragma unroll
-        for (int j = 0; j < kValues; ++j)
-        {
-            if (lowerMask & (1u << j))
-            {
-                codeF[j] -= 1.0f;
-            }
-        }
+        uint32_t bandMask;
+        int32_t largest;
+        LookUpLaneCodes(compact, colourBits, myStage, codeF, bandMask, largest);
+        ResolveLaneCodes<kCurveLinearToPQ, kValues>(d, t, compact, myStage, bandMask, largest, codeF);
         if (!laneActive)
         {
             continue; // the next unit starts with the whole warp again (Switch)
         }
-#pragma unroll
-        for (int pixel = 0; pixel < kPixels; ++pixel)
-        {
-            const uint32_t k = __float2uint_rz(fmaxf(fmaxf(codeF[3 * pixel], codeF[3 * pixel + 1]), codeF[3 * pixel + 2]));
-            TallyCode(light.tally, k, __ldg(s.light.levels + k));
-        }
+        TallyLaneCodes<kPixels>(light.tally, codeF, s.light.levels, kRows == 2);
         FastEncodeParams p = d;
         p.strideY = r.planeStride[0];
         p.strideCb = r.planeStride[1];
@@ -637,54 +565,18 @@ __global__ void __launch_bounds__(kLightBatchWarps * 32, 1) EncodeLightF32BatchK
 #pragma unroll
             for (int row = 0; row < kRows; ++row)
             {
-                uint8_t* alphaRow = static_cast<uint8_t*>(r.plane[3]) + (y + row) * r.planeStride[3] + static_cast<int64_t>(x) * 2;
-                __stcs(reinterpret_cast<uint2*>(alphaRow), make_uint2(MsbWord<DEST>(alphaCode[4 * row] | (alphaCode[4 * row + 1] << 16), p),
-                                                                      MsbWord<DEST>(alphaCode[4 * row + 2] | (alphaCode[4 * row + 3] << 16), p)));
+                StoreAlphaRow<DEST>(p, static_cast<uint8_t*>(r.plane[3]) + (y + row) * r.planeStride[3] + static_cast<int64_t>(x) * 2, alphaCode, 4 * row);
             }
         }
     }
     light.Flush(s.light.acc);
 }
 
-// EncodePlanarBatchKernel's light-level form for float hosts: the generic kernel's own per-site code with its tally, the
-// level read from the context's table or evaluated in place when there is none.
+// EncodePlanarBatchKernel with the content light level of every image (float hosts).
 template <typename Source>
 __global__ void __launch_bounds__(kBatchEdgeThreads, 1) EncodeLightPlanarBatchKernel(const __grid_constant__ Source s)
 {
-    const typename Source::Walk walk(s);
-    if (walk.Idle(blockIdx.x))
-    {
-        return;
-    }
-    const int count = walk.Count();
-    __shared__ uint64_t libmStorage[96];
-    const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
-    __syncthreads();
-    int record = 0;
-    ImageTally light;
-#pragma unroll 1
-    for (long long unit = blockIdx.x; unit < walk.Units(); unit += gridDim.x)
-    {
-        record = walk.Find(count, record, unit);
-        const BatchRecord& r = walk.Record(record);
-        light.Switch(walk.ImageOf(record), s.light.acc);
-        if (unit == r.firstUnit && threadIdx.x < 32) // the CTA's first warp counts the record's pixels
-        {
-            light.pixels += static_cast<uint64_t>(r.width) * static_cast<uint64_t>(r.rowCount);
-        }
-        EncodeParams p = s.shared;
-        p.rows = r.rows;
-        p.rowStride = r.rowStride;
-        for (int k = 0; k < 4; ++k)
-        {
-            p.plane[k] = r.plane[k];
-            p.planeStride[k] = r.planeStride[k];
-        }
-        p.width = r.width;
-        p.rowCount = r.rowCount;
-        EncodePlanarSite<float, kBatchEdgeThreads, 1>(p, t, static_cast<unsigned>(unit - r.firstUnit), &light.tally, s.light.levels);
-    }
-    light.Flush(s.light.acc);
+    EncodePlanarBatchBody<Source, float, 1>(s, s.light);
 }
 
 template <typename Source, typename SampleT, int XS, int YS, int ALPHA, int SOURCE>

@@ -231,6 +231,150 @@ __device__ __forceinline__ void StoreTile(const FastEncodeParams& p, const float
     }
 }
 
+// ---- a lane's float -> code conversion through the compact step table, for the RGBA kernel (kernels_fast_rgba.cu) and
+// the batched light-level kernel (kernels_batch.cu).  N is the lane's number of colour samples: 24 for 2 rows x 4 pixels,
+// 12 for one row; the samples are row-major, interleaved R, G, B, and codeF always has room for 24 (StoreTile's shape).
+
+// The compact table (one-word entries + first_k in shared memory, kernels_fast_flat.cu has the commentary) and its band
+// bitmap, with the look-up's constants.
+struct CompactTable
+{
+    const uint32_t* entries;
+    const uint32_t* firstBits;
+    uint32_t flatShift;
+    int32_t negativeLow;
+    int32_t span;
+    uint32_t bandStrideLog2;
+    const uint32_t* bandBits;
+    uint32_t topShift;
+    uint32_t codeMask;
+    uint32_t magic;
+};
+
+// `entries` is where BeginTableImageCopy (table_staging.cuh) lands the table's image.
+__device__ __forceinline__ CompactTable CompactTableOf(const CurveTableView& table, const uint32_t* entries)
+{
+    return CompactTable{ entries, entries + ((table.flatCount + 3) & ~3), table.flatShift, -static_cast<int32_t>(table.flatLow),
+                         static_cast<int32_t>(table.flatHigh - table.flatLow), table.bandStrideLog2, table.bandBits, 32u - table.flatShift,
+                         table.compactCodeMask, table.compactMagic };
+}
+
+// RGBA hosts: alpha, clamp / premultiplication (WriteHeifImage.cpp:1043-1077), then the colour samples the curve sees.
+// raw[k] = { R, G, B, A } of the lane's pixel k; alphaCode[k] is its alpha code.
+template <int PIXELS>
+__device__ __forceinline__ void PrepareRgbaSamples(const FastEncodeParams& p, const uint4 (&raw)[PIXELS], uint32_t (&alphaCode)[PIXELS],
+                                                   uint32_t (&colourBits)[3 * PIXELS])
+{
+#pragma unroll
+    for (int k = 0; k < PIXELS; ++k)
+    {
+        const float alpha = ClampF(__uint_as_float(raw[k].w), 0.0f, 1.0f);
+        float colour[3] = { __uint_as_float(raw[k].x), __uint_as_float(raw[k].y), __uint_as_float(raw[k].z) };
+        if (p.premultiply && alpha < 1.0f)
+        {
+#pragma unroll
+            for (int c = 0; c < 3; ++c)
+            {
+                colour[c] = (alpha == 0) ? 0.0f : PremultiplyColor(ClampF(colour[c], 0.0f, 1.0f), alpha, 1.0f);
+            }
+        }
+        alphaCode[k] = FloatToCode(alpha, p.maxCodeFloat);
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+        {
+            colourBits[3 * k + c] = __float_as_uint(colour[c]);
+        }
+    }
+}
+
+// The samples are parked in the lane's staging slot (16-byte aligned, for the band-bitmap probes and the exact
+// evaluations), then each goes through the table: codeF[j] is right unless bit j of bandMask is set (in or near a step's
+// fuzzy band); `largest` is the max of the samples as signed integers, > 0x7f7fffff <=> a +inf / NaN is among them.
+template <int N>
+__device__ __forceinline__ void LookUpLaneCodes(const CompactTable& c, const uint32_t (&colourBits)[N], uint32_t* myStage, float (&codeF)[kValuesPerLane],
+                                                uint32_t& bandMask, int32_t& largest)
+{
+#pragma unroll
+    for (int q = 0; q < N / 4; ++q)
+    {
+        *reinterpret_cast<uint4*>(myStage + 4 * q) = make_uint4(colourBits[4 * q], colourBits[4 * q + 1], colourBits[4 * q + 2], colourBits[4 * q + 3]);
+    }
+    bandMask = 0;
+    largest = 0;
+#pragma unroll
+    for (int j = 0; j < N; ++j)
+    {
+        bool inBand;
+        uint32_t entry;
+        codeF[j] = LookupCurveCompact<0>(colourBits[j], c.entries, c.flatShift, c.negativeLow, c.span, c.topShift, c.codeMask, c.magic, inBand, entry);
+        asm("{ .reg .pred q; setp.ne.u32 q, %1, 0; @q or.b32 %0, %0, %2; }" : "+r"(bandMask) : "r"(static_cast<uint32_t>(inBand)), "r"(1u << j));
+        largest = max(largest, static_cast<int32_t>(colourBits[j]));
+    }
+}
+
+// The exact codes of the samples LookUpLaneCodes left open: an in-band sample is one below the table's code when its bit
+// of the band bitmap (found through first_k) is clear; +inf / NaN take the exact evaluation, lane by lane.
+template <int CURVE, int N>
+__device__ __forceinline__ void ResolveLaneCodes(const FastEncodeParams& p, const avifmath::LibmTables& t,const CompactTable& c, const uint32_t* myStage,
+                                                 uint32_t bandMask, int32_t largest, float (&codeF)[kValuesPerLane])
+{
+    uint32_t lowerMask = 0;
+    {
+        uint32_t pending = bandMask;
+        while (pending != 0)
+        {
+            const int j = __ffs(static_cast<int>(pending)) - 1;
+            pending &= pending - 1;
+            const uint32_t bits = myStage[j];
+            const int32_t bucket = __viaddmin_s32_relu(static_cast<int32_t>(bits) >> c.flatShift, c.negativeLow, c.span);
+            const uint32_t entry = c.entries[bucket];
+            const uint32_t k = ((entry & c.codeMask) >> kCompactLenBits) + ((entry >> c.topShift) != 0 ? 1u : 0u);
+            const uint32_t distance = bits - c.firstBits[k];
+            if (k != 0 && distance < (1u << c.bandStrideLog2)) // else flagged by the superset test only
+            {
+                const uint32_t bitIndex = (k << c.bandStrideLog2) + distance;
+                const uint32_t word = __ldg(c.bandBits + (bitIndex >> 5));
+                lowerMask |= (((word >> (bitIndex & 31u)) & 1u) ^ 1u) << j;
+            }
+        }
+    }
+    if (__any_sync(0xffffffffu, largest > 0x7f7fffff))
+    {
+        for (int j = 0; j < N; ++j)
+        {
+            const uint32_t bits = myStage[j];
+            if (static_cast<int32_t>(bits) > 0x7f7fffff)
+            {
+                const float exact = CodeToFloat(ExactCurveCode<CURVE>(__uint_as_float(bits), p.pqMultiplier, p.maxCodeFloat, t));
+#pragma unroll
+                for (int slot = 0; slot < N; ++slot)
+                {
+                    if (slot == j)
+                    {
+                        codeF[slot] = exact;
+                    }
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < N; ++j)
+    {
+        if (lowerMask & (1u << j))
+        {
+            codeF[j] -= 1.0f;
+        }
+    }
+}
+
+// One row of a lane's alpha plane: its 4 pixels' codes from alphaCode[first].
+template <int DEST, int PIXELS>
+__device__ __forceinline__ void StoreAlphaRow(const FastEncodeParams& p, uint8_t* alphaRow, const uint32_t (&alphaCode)[PIXELS], int first)
+{
+    __stcs(reinterpret_cast<uint2*>(alphaRow), make_uint2(MsbWord<DEST>(alphaCode[first] | (alphaCode[first + 1] << 16), p),
+                                                          MsbWord<DEST>(alphaCode[first + 2] | (alphaCode[first + 3] << 16), p)));
+}
+
 } // namespace fastenc
 
 // kernels_fast_rgba.cu; `dest` is the description's avifgpu_source_layout bits (EncodeParams::destLayout)

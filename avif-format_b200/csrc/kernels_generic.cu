@@ -22,58 +22,10 @@ namespace
 
 constexpr int kThreads = 256;
 
-// Reference layout: one thread per pixel.
-template <typename HostT>
-__global__ void __launch_bounds__(kThreads) EncodeReferenceLayoutKernel(const EncodeParams p)
-{
-    __shared__ uint64_t libmStorage[96];
-    const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
-    __syncthreads();
-
-    const int chunks = (p.width + kThreads - 1) / kThreads;
-    const int x = static_cast<int>(blockIdx.x % chunks) * kThreads + threadIdx.x;
-    const int y = static_cast<int>(blockIdx.x / chunks);
-    if (x >= p.width || y >= p.rowCount)
-    {
-        return;
-    }
-    const HostT* px = reinterpret_cast<const HostT*>(static_cast<const uint8_t*>(p.rows) + static_cast<int64_t>(y) * p.rowStride) +
-                      static_cast<int64_t>(x) * p.channels;
-    uint32_t codes[4] = { 0, 0, 0, 0 };
-    HostPixelToCodes<HostT>(p, px, codes, t);
-
-    const bool wide = p.imageDepth > 8;
-    if (p.channels <= 2)
-    {
-        StoreCode(p.plane[0], p.planeStride[0], y, x, wide, codes[0]);
-        if (p.hasAlpha)
-        {
-            StoreCode(p.plane[3], p.planeStride[3], y, x, wide, codes[1]);
-        }
-    }
-    else
-    {
-        for (int i = 0; i < p.channels; ++i)
-        {
-            StoreCode(p.plane[0], p.planeStride[0], y, x * p.channels + i, wide, codes[i]);
-        }
-    }
-}
-
-// Planar YCbCr layout: one thread per chroma site (1x1, 2x1 or 2x2 pixels).
-template <typename HostT>
-__global__ void __launch_bounds__(kThreads) EncodePlanarKernel(const EncodeParams p)
-{
-    __shared__ uint64_t libmStorage[96];
-    const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
-    __syncthreads();
-
-    EncodePlanarSite<HostT, kThreads>(p, t, blockIdx.x);
-}
-
-// The light-level kernels (float hosts, PQ; light_level.cuh): the kernels above, every pixel's codes into the thread's tally,
-// one flush per warp.  No thread leaves early: the flush needs the whole warp.
-__global__ void __launch_bounds__(kThreads) EncodeReferenceLayoutLightKernel(const EncodeParams p, const LightSink light)
+// Reference layout: one thread per pixel.  LIGHT = 1 (float hosts, PQ; light_level.cuh): every pixel's codes also go into
+// the thread's tally, one flush per warp; no thread leaves early then, as the flush needs the whole warp.
+template <typename HostT, int LIGHT>
+__device__ __forceinline__ void EncodeReferenceLayoutBody(const EncodeParams& p, const LightSink& light = {})
 {
     __shared__ uint64_t libmStorage[96];
     const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
@@ -83,41 +35,81 @@ __global__ void __launch_bounds__(kThreads) EncodeReferenceLayoutLightKernel(con
     const int chunks = (p.width + kThreads - 1) / kThreads;
     const int x = static_cast<int>(blockIdx.x % chunks) * kThreads + threadIdx.x;
     const int y = static_cast<int>(blockIdx.x / chunks);
+    if (!LIGHT && (x >= p.width || y >= p.rowCount))
+    {
+        return;
+    }
     if (x < p.width && y < p.rowCount)
     {
-        const float* px = reinterpret_cast<const float*>(static_cast<const uint8_t*>(p.rows) + static_cast<int64_t>(y) * p.rowStride) +
+        const HostT* px = reinterpret_cast<const HostT*>(static_cast<const uint8_t*>(p.rows) + static_cast<int64_t>(y) * p.rowStride) +
                           static_cast<int64_t>(x) * p.channels;
         uint32_t codes[4] = { 0, 0, 0, 0 };
-        HostPixelToCodes<float>(p, px, codes, t);
-        TallyPixel(tally, light.levels, p, codes, t);
+        HostPixelToCodes<HostT>(p, px, codes, t);
+        if constexpr (LIGHT != 0)
+        {
+            TallyPixel(tally, light.levels, p, codes, t);
+        }
+
+        const bool wide = LIGHT != 0 || p.imageDepth > 8; // a light-level encode is PQ, 10 or 12 bits
         if (p.channels <= 2)
         {
-            StoreCode(p.plane[0], p.planeStride[0], y, x, true, codes[0]);
+            StoreCode(p.plane[0], p.planeStride[0], y, x, wide, codes[0]);
             if (p.hasAlpha)
             {
-                StoreCode(p.plane[3], p.planeStride[3], y, x, true, codes[1]);
+                StoreCode(p.plane[3], p.planeStride[3], y, x, wide, codes[1]);
             }
         }
         else
         {
             for (int i = 0; i < p.channels; ++i)
             {
-                StoreCode(p.plane[0], p.planeStride[0], y, x * p.channels + i, true, codes[i]);
+                StoreCode(p.plane[0], p.planeStride[0], y, x * p.channels + i, wide, codes[i]);
             }
         }
     }
-    FlushLightTally(tally, LaunchPixelsForFirstWarp(static_cast<uint64_t>(p.width) * p.rowCount), light.acc);
+    if constexpr (LIGHT != 0)
+    {
+        FlushLightTally(tally, LaunchPixelsForFirstWarp(static_cast<uint64_t>(p.width) * p.rowCount), light.acc);
+    }
 }
 
-__global__ void __launch_bounds__(kThreads) EncodePlanarLightKernel(const EncodeParams p, const LightSink light)
+// Planar YCbCr layout: one thread per chroma site (1x1, 2x1 or 2x2 pixels).  LIGHT = 1 as above.
+template <typename HostT, int LIGHT>
+__device__ __forceinline__ void EncodePlanarBody(const EncodeParams& p, const LightSink& light = {})
 {
     __shared__ uint64_t libmStorage[96];
     const LibmTables t = avifmath::StageLibmTables(libmStorage, threadIdx.x, blockDim.x);
     __syncthreads();
 
     LightTally tally{ 0u, 0ull };
-    EncodePlanarSite<float, kThreads, 1>(p, t, blockIdx.x, &tally, light.levels);
-    FlushLightTally(tally, LaunchPixelsForFirstWarp(static_cast<uint64_t>(p.width) * p.rowCount), light.acc);
+    EncodePlanarSite<HostT, kThreads, LIGHT>(p, t, blockIdx.x, &tally, light.levels);
+    if constexpr (LIGHT != 0)
+    {
+        FlushLightTally(tally, LaunchPixelsForFirstWarp(static_cast<uint64_t>(p.width) * p.rowCount), light.acc);
+    }
+}
+
+template <typename HostT>
+__global__ void __launch_bounds__(kThreads) EncodeReferenceLayoutKernel(const EncodeParams p)
+{
+    EncodeReferenceLayoutBody<HostT, 0>(p);
+}
+
+template <typename HostT>
+__global__ void __launch_bounds__(kThreads) EncodePlanarKernel(const EncodeParams p)
+{
+    EncodePlanarBody<HostT, 0>(p);
+}
+
+// The light-level kernels: the kernels above with the content light level (float hosts, PQ).
+__global__ void __launch_bounds__(kThreads) EncodeReferenceLayoutLightKernel(const EncodeParams p, const LightSink light)
+{
+    EncodeReferenceLayoutBody<float, 1>(p, light);
+}
+
+__global__ void __launch_bounds__(kThreads) EncodePlanarLightKernel(const EncodeParams p, const LightSink light)
+{
+    EncodePlanarBody<float, 1>(p, light);
 }
 
 // The sharded device light-level call's merge on the owner: one warp adds the gathered partials whose bit is set in

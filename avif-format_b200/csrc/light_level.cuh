@@ -47,6 +47,22 @@ __device__ __forceinline__ void TallyCode(LightTally& tally, uint32_t code, uint
     tally.levelSum += level;
 }
 
+// A tuned float kernel's lane: PIXELS pixels of R'G'B' codes (as floats, row-major, interleaved; pixels 4.. are the second
+// row, taken only when it exists), max(R', G', B') of each with its level from the context's table.
+template <int PIXELS, int N>
+__device__ __forceinline__ void TallyLaneCodes(LightTally& tally, const float (&codeF)[N], const uint32_t* levels, bool secondRow)
+{
+#pragma unroll
+    for (int pixel = 0; pixel < PIXELS; ++pixel)
+    {
+        if (pixel < 4 || secondRow)
+        {
+            const uint32_t k = __float2uint_rz(fmaxf(fmaxf(codeF[3 * pixel], codeF[3 * pixel + 1]), codeF[3 * pixel + 2]));
+            TallyCode(tally, k, __ldg(levels + k));
+        }
+    }
+}
+
 // The whole warp, converged, once at exit: one atomicMax and one 64-bit atomicAdd per warp that saw a non-zero code.
 // `pixels` is the launch's pixel count when this is the grid's first warp, else 0: a launch converts exactly its window,
 // so the count is added once per launch instead of being tallied per pixel.
